@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- the BASELINE.json metric on B200: train iters/sec (+ render Mpix/s fwd+bwd) of the
+"""bench.py -- the BASELINE.json metric on H100: train iters/sec (+ render Mpix/s fwd+bwd) of the
 joint pose+Gaussian optimisation loop at 1M Gaussians / 12 views / 1920x1080 / SH degree 3
 (BASELINE.json configs[2]; configs[0] is the CPU-only correctness case, configs[1] a parity size).
 
@@ -48,6 +48,9 @@ def parse():
     ap.add_argument("--exchange", default="fused_p2p", choices=["allreduce", "fused_p2p", "fused_p2p_nccl"],
                     help="multi-GPU gradient exchange: NCCL all-reduce + Adam, or the fused P2P "
                          "reduce-scatter->Adam->all-gather kernel (default)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (rendered image, loss, "
+                         "poses, a fixed seeded row sample of every parameter tensor) as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -57,7 +60,7 @@ def workload_name(idx, sc):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -106,7 +109,56 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "not measured: H100 SXM data sheet HBM3 bandwidth (3.35 TB/s)"
+
+
+def gpu_identity(dev):
+    """The card a number was measured on: name, SM count, L2 size and (from nvidia-smi) power limit and max SM clock."""
+    props = torch.cuda.get_device_properties(dev)
+    out = {"name": props.name, "sm_count": props.multi_processor_count,
+           "l2_mb": getattr(props, "L2_cache_size", 0) / 2**20, "power_limit_w": None, "sm_max_mhz": None}
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
+                            "-i", str(dev.index or 0)], capture_output=True, text=True, timeout=30).stdout.split(",")
+        out["power_limit_w"], out["sm_max_mhz"] = float(q[0]), float(q[1])
+    except Exception:
+        pass
+    return out
+
+
+# ----------------------------------------------------------------------------------------------
+# --dump-outputs: what the timed path computed in its last step, so that two builds can be compared output for output
+# ----------------------------------------------------------------------------------------------
+DUMP_IMAGE_PIXELS = 1 << 21     # 25 MB of image: every pixel up to 1920x1080, a fixed sample above
+DUMP_PARAM_ROWS = 1 << 16       # 15 MB of parameters (59 floats per Gaussian)
+
+
+def grab_outputs(tr):
+    """Host copies of the last step's results: the rendered image of its view, its loss, and -- after its optimizer
+    update -- the pose table and every parameter tensor.  Larger outputs are reduced to a sample fixed by a seed and
+    the shapes alone, so every run with the same arguments samples the same elements."""
+    g = torch.Generator().manual_seed(0)
+
+    def sample(n, cap):
+        return None if n <= cap else torch.randperm(n, generator=g)[:cap].sort().values.to(tr.dev)
+
+    img = tr.color.reshape(3, -1)
+    pix = sample(img.shape[1], DUMP_IMAGE_PIXELS)
+    out = {"image": img.reshape(tr.color.shape) if pix is None else img[:, pix],
+           "loss": tr.loss_value().double().reshape(1), "poses": tr.poses}
+    rows = sample(tr.P, DUMP_PARAM_ROWS)
+    from instantsplat_b200.trainer import SEGMENTS
+    for name, _ in SEGMENTS:
+        p = tr.view(tr.params, name)
+        out[name] = p if rows is None else p[rows]
+    return {k: v.detach().cpu().numpy().copy() for k, v in out.items()}
+
+
+def write_outputs(out_dir, arrays):
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 # ----------------------------------------------------------------------------------------------
@@ -115,11 +167,10 @@ def measured_peaks():
 def cpu_sample_plan(sc, n_steps):
     """What one CPU step computes -- a pure function of the workload and of the number of steps (no wall-clock
     probing, so two runs sample the same work).  About 12 s of CPU work per step (all Gaussians, 128 stratified tiles,
-    the full frame's loss) for up to 32 steps -- the default bench's cpu_baseline (1 warm-up + 3 timed) and the driver's
+    the full frame's loss) for up to 32 steps -- the default bench's cpu_baseline (1 warm-up + 3 timed) and
     `--impl reference --steps 20 --warmup 5` (about 5 minutes) -- and a sample shrinking to no less than 1/8 of that for
     longer runs.  Smaller samples are NOT used: PyTorch's per-operator overhead dominates small tensors and the
-    extrapolation then under-reports the CPU (full sample 0.0069 it/s, 1/7 sample 0.0031, 1/51 sample 0.0010:
-    profiles/r02_bench_reference_*.json)."""
+    extrapolation then under-reports the CPU."""
     gx, gy = (sc.width + 15) // 16, (sc.height + 15) // 16
     T = gx * gy
     shrink = 1 if n_steps <= 32 else min(8, (n_steps + 31) // 32)
@@ -253,7 +304,7 @@ def gpu_torch_pieces(sc, dev, img, gt, reps=10):
 
     return {"pose_pretransform_activations_cat_fwd_bwd_ms": clock(pre), "l1_ssim_fwd_bwd_ms": clock(loss),
             "per_point_adam_ms": clock(adam),
-            "what": "torch restatement (oracle/gs_oracle.py) of /root/reference/gaussian_renderer/__init__.py:81-92,102,121, "
+            "what": "torch restatement (oracle/gs_oracle.py) of the reference's gaussian_renderer/__init__.py:81-92,102,121, "
                     "utils/loss_utils.py:39-85 and scene/per_point_adam.py:34-98 run on the same GPU"}
 
 
@@ -272,7 +323,7 @@ def run_reference(args):
                              "sample": r["sample"], "spread": r["spread"]},
             "e2e": {"value": r["value"], "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
             "note": "reference CUDA path (diff-gaussian-rasterization / fused-ssim) is an empty submodule in "
-                    "/root/reference: this arm is the CPU oracle port of the same path"}
+                    "the reference checkout: this arm is the CPU oracle port of the same path"}
     return line
 
 
@@ -302,9 +353,8 @@ def run_b200(args):
     torch.cuda.empty_cache()
     gt_host = gt_dev.cpu().pin_memory()
     # N=1: graph replay is the default.  N>1: capturable with the flag-barrier exchange and bit-exact
-    # (tests/test_multigpu.py "fused_p2p+graph"), but measured no faster than eager launches at N=2 (2.19 vs 2.13
-    # ms/step, profiles/r02_bench_n2_graph*.json): the host already runs ahead of a step that waits on its peers, so
-    # eager stays the default there and --graph opts in
+    # (tests/test_multigpu.py "fused_p2p+graph"), but no faster than eager launches at N=2 when it was measured: the
+    # host already runs ahead of a step that waits on its peers, so eager stays the default there and --graph opts in
     use_graph = (world == 1 and not args.no_graph) or (world > 1 and args.graph and args.exchange == "fused_p2p")
     tr = I.JointTrainer(sc, dev, gt_images=gt_dev, world_size=world, rank=rank, exchange=args.exchange,
                         use_graph=use_graph)
@@ -385,6 +435,7 @@ def run_b200(args):
         # timed region 1 (the reported value): the iteration replayed from CUDA graphs, no instrumentation inside
         ms_dev = timed(lambda s: (device_step(s), Rs.append(tr.last_R)), K, W_)
         clocks = sampler.stop() if rank == 0 else None
+        dumped = grab_outputs(tr) if args.dump_outputs and rank == 0 else None
         # timed region 2 (per-kernel table / roofline): the same steps launched eagerly with CUDA events around
         # every kernel on the launching stream
         tr.use_graph = False
@@ -399,6 +450,7 @@ def run_b200(args):
         L.gsb_profile_enable(1)
         launches0 = L.gsb_launch_count()
         ms_dev = timed(lambda s: (device_step(s), Rs.append(tr.last_R)), K, W_)
+        dumped = grab_outputs(tr) if args.dump_outputs and rank == 0 else None
         launches = int(L.gsb_launch_count() - launches0)
         L.gsb_profile_collect(ms_sum, cnt, nk)
         L.gsb_profile_enable(0)
@@ -412,8 +464,8 @@ def run_b200(args):
         e2e_step(W_ + K + s)
     ms_e2e = timed(e2e_step, K, W_ + K + n_e2e_warm)
     # ---- the same iteration through the reference's own operator API (boundaries B1-B4): the loop body of
-    # /root/reference/train.py:140-211 transcribed onto the repo's mirror of GaussianModel (the GPU box has no
-    # /root/reference; tests/test_reference_shims_cpu.py runs the real reference modules on the same interfaces).
+    # the reference's train.py:140-211 transcribed onto the repo's mirror of GaussianModel (the reference tree is not
+    # a dependency of this repository; tests/test_reference_shims_cpu.py checks the mirror against it on the CPU).
     dropin, e2e_plugin = None, None
     if world == 1:
         sys.path.insert(0, os.path.join(ROOT, "shims"))
@@ -535,17 +587,14 @@ def run_b200(args):
             row.update(alg_bytes=int(alg_map[name]), gbs=round(gbs, 1), frac_hbm=round(gbs / peak, 4))
         kernels[name] = row
     dom = max((k for k in kernels if k in alg_map), key=lambda k: kernels[k]["ms"])
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tpath):
-        traffic = json.load(open(tpath)).get(dom)
+    gpu = gpu_identity(dev)
     # pair statistics (instrumented re-run of the blend kernels, outside the timed region): the blend kernels are
     # bound by instruction issue over (pixel, Gaussian) pairs, so the pair rate is the roof that binds them
     pair = None
     try:
         ps = tr.blend_stats(view_for_step(sc.n_views, world, rank, 0))
-        sm_clk = (clocks or {}).get("sm_mhz") or 1965.0
-        issue_peak = 148 * 4 * sm_clk * 1e6            # warp instructions / s (4 schedulers per SM)
+        sm_clk = (clocks or {}).get("sm_mhz") or gpu["sm_max_mhz"] or 1980.0
+        issue_peak = gpu["sm_count"] * 4 * sm_clk * 1e6    # warp instructions / s (4 schedulers per SM)
         pair = dict(ps)
         for d, kname in (("fwd", "blend_fwd"), ("bwd", "blend_bwd")):
             if kname in kernels:
@@ -559,7 +608,7 @@ def run_b200(args):
     except Exception as e:
         pair = {"error": f"{type(e).__name__}: {e}"}
     roof = {"bound": "hbm", "kernel": dom, "pairs": pair, "achieved": kernels[dom]["gbs"], "peak": peak, "unit": "GB/s",
-            "frac": kernels[dom]["frac_hbm"], "traffic": traffic, "peak_source": peak_src,
+            "frac": kernels[dom]["frac_hbm"], "peak_source": peak_src,
             "alg_bytes_per_launch": kernels[dom]["alg_bytes"], "ms_per_launch": kernels[dom]["ms"],
             "note": "algorithmic bytes = SURVEY.md 8(d) formulas with the measured R; the blend kernels are "
                     "bound by FP32/MUFU issue on (pixel,Gaussian) pairs, not by HBM (see DESIGN.md)"}
@@ -594,7 +643,8 @@ def run_b200(args):
                    "launch_mode": ("CUDA-graph replay of the whole iteration (one graph per view); per-kernel table from "
                                    f"a second, eagerly launched timed region of {Kp} steps at {ms_prof / Kp:.3f} ms/step")
                    if use_graph else "eager launches",
-                   "l2": "working set (params+grads+moments 944 MB at 1M) exceeds the 126 MB L2; no explicit flush",
+                   "l2": f"working set (params+grads+moments 944 MB at 1M) exceeds the {gpu['l2_mb']:.0f} MB L2; "
+                         "no explicit flush",
                    "iteration": "one view: render fwd + L1/DSSIM + bwd + per-point Adam (+ all-reduce if N>1)",
                    "scaling_note": "iters/s counts VIEWS; with N GPUs one optimizer step consumes N views (mean gradient) "
                                    "at the reference's per-view learning-rate schedule, so N-GPU numbers are throughput, "
@@ -604,7 +654,11 @@ def run_b200(args):
         "e2e_trainer": e2e_trainer,
         "gpu_launches": launches, "gpu_launches_note": "every kernel on the path is libgsb200.so's own (no library sort/scan)",
         "dropin_boundary": dropin, "ref_python_pieces_gpu": torch_pieces, "kernels": kernels, "roofline": roof, "clocks": clocks, "cpu_baseline": cpu_base, "impl": "b200",
+        "gpu": gpu,
     }
+    if dumped is not None:
+        write_outputs(args.dump_outputs, dumped)
+        line["dumped_outputs"] = {k: [list(v.shape), str(v.dtype)] for k, v in dumped.items()}
     if world > 1:
         dist.destroy_process_group()
     return line

@@ -1,11 +1,11 @@
-/* gsb200.h -- C ABI of libgsb200.so, the B200-native (sm_100a) replacement for the native code
+/* gsb200.h -- C ABI of libgsb200.so, the H100-native (sm_90a) replacement for the native code
  * under InstantSplat's training hot path.  Plain pointers and sizes only; no torch types.
  * All pointers are DEVICE pointers unless the name ends in _host.  All tensors fp32, contiguous.
  * Every entry point enqueues work on `stream` and returns 0 on success or a negative error code
  * (GSB_ERR_*); none of them throws.  Buffers are caller-owned (the Python layer uses torch
  * allocations), sized with the gsb_*_bytes() helpers.
  *
- * What each entry point replaces in the reference (files under /root/reference):
+ * What each entry point replaces in the reference (files of the InstantSplat tree):
  *
  *   gsb_preprocess + gsb_render   ->  diff_gaussian_rasterization._C.rasterize_gaussians, called by
  *                                     GaussianRasterizer.forward at gaussian_renderer/__init__.py:126-135
@@ -266,7 +266,7 @@ GSB_API void gsb_profile_enable(int on);
 GSB_API int gsb_profile_collect(double* ms_sum, int64_t* count, int n_ids);
 GSB_API uint64_t gsb_launch_count(void);
 /* Tuning switches: "blend_version" = 1 (one pixel per lane, 8 warps per tile; the in-library cross-check) | 2 (two
- * pixels per lane, packed f32x2; default); "stage_bulk" = 1 (slab chunks staged with cp.async.bulk/TMA +
+ * pixels per lane; default); "stage_bulk" = 1 (slab chunks staged with cp.async.bulk/TMA +
  * mbarrier, double buffered; default) | 0. */
 GSB_API int gsb_set_option(const char* name, int value);
 

@@ -1,4 +1,4 @@
-"""instantsplat_b200 -- B200-native (sm_100a) replacement for the native code under InstantSplat's
+"""instantsplat_b200 -- H100-native (sm_90a) replacement for the native code under InstantSplat's
 training hot path: differentiable Gaussian rasterizer (+ fused camera-pose transform), fused
 L1/SSIM loss and per-point Adam, behind the reference's own Python interfaces.
 

@@ -75,7 +75,7 @@ class GsbError(RuntimeError):
 
 
 def build(verbose: bool = False) -> str:
-    """Compile libgsb200.so for sm_100a with nvcc (cross-compiles without a GPU)."""
+    """Compile libgsb200.so for sm_90a with nvcc (cross-compiles without a GPU)."""
     out = subprocess.run(["make", "-C", CSRC, "-j4"], capture_output=True, text=True)
     if out.returncode != 0:
         raise GsbError("building libgsb200.so failed:\n" + out.stdout + out.stderr)

@@ -5,8 +5,8 @@ import torch
 
 
 def projection_matrix(znear: float, zfar: float, fovx: float, fovy: float) -> torch.Tensor:
-    """/root/reference/utils/graphics_utils.py:71-91 (NOT transposed; callers store P^T like
-    /root/reference/scene/cameras.py:55)."""
+    """utils/graphics_utils.py:71-91 (NOT transposed; callers store P^T like
+    scene/cameras.py:55)."""
     ty, tx = math.tan(fovy / 2), math.tan(fovx / 2)
     top, right = ty * znear, tx * znear
     P = torch.zeros(4, 4)
@@ -20,7 +20,7 @@ def projection_matrix(znear: float, zfar: float, fovx: float, fovy: float) -> to
 
 class SimpleCamera:
     """The attributes `render()` reads from a viewpoint camera
-    (/root/reference/gaussian_renderer/__init__.py:51-62)."""
+    (gaussian_renderer/__init__.py:51-62)."""
 
     def __init__(self, width, height, fovx, fovy, device="cuda", znear=0.01, zfar=100.0):
         self.image_width, self.image_height = int(width), int(height)

@@ -1,7 +1,7 @@
-// Fused per-point Adam for sm_100a: all parameter tensors of the Gaussian model (and the pose
+// Fused per-point Adam for sm_90a: all parameter tensors of the Gaussian model (and the pose
 // table) in ONE launch, no host synchronisation.
 //
-// Semantics are those of /root/reference/scene/per_point_adam.py:34-98:
+// Semantics are those of scene/per_point_adam.py:34-98:
 //   * whole-tensor gate  mask = grad.norm() > 0  (:66-67): moments are updated only when the
 //     gradient tensor is not identically zero; evaluated on the device by k_adam_gate
 //   * old-style bias correction folded into step_size = lr*sqrt(1-b2^t)/(1-b1^t) (:76-81),

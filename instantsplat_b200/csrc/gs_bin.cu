@@ -1,8 +1,8 @@
-// Binning for the B200 rasterizer: from per-Gaussian splat records to per-tile, depth-ordered slabs --
+// Binning for the rasterizer: from per-Gaussian splat records to per-tile, depth-ordered slabs --
 // hand-written, no library sort/scan, no host round trip.
 //
 // The reference pipeline (SURVEY.md section 2.3: InclusiveSum -> duplicateWithKeys -> 64-bit SortPairs ->
-// identifyTileRanges, driven from /root/reference/gaussian_renderer/__init__.py:126-135) sorts ALL R
+// identifyTileRanges, driven from gaussian_renderer/__init__.py:126-135) sorts ALL R
 // (tile | depth) keys globally and needs R on the host to size its buffers.  Here the order is produced
 // tile-locally instead:
 //
@@ -14,7 +14,7 @@
 //                  (one adaptive-range bucket pass + per-bucket insertion sort; flip-bitonic fallback for
 //                  skewed depth distributions) and written out as the tile's id list.  No per-instance copy of the
 //                  splat records is materialised: the blend kernels stage id chunks with TMA bulk copies and gather
-//                  the 48-byte records with cp.async out of the L2-resident record table, only as far as they walk
+//                  the 48-byte records with cp.async out of the record table, only as far as they walk
 //
 // Result order = (tile, depth bits ascending, Gaussian index ascending): exactly the reference's stable radix
 // sort of keys emitted in index order (Appendix A.2.9) -- deterministic although emission uses atomics.
@@ -387,7 +387,6 @@ constexpr int kSmallNT = 256, kSmallKPT = 8;     // lists of up to 2048 entries:
 constexpr int kLargeNT = 512, kLargeKPT = 16;    // up to 8192 entries: 96 KB shared memory
 static_assert(kSmallNT * kSmallKPT == (int)kSmallList && kLargeNT * kLargeKPT == (int)kLargeList, "size classes");
 constexpr size_t kSmallSmem = (size_t)kSmallList * 12, kLargeSmem = (size_t)kLargeList * 12;
-constexpr int kQueueCtas = 148;                  // persistent CTAs draining the long-list queues (one per SM)
 
 // one CTA per tile; tiles with longer lists were queued by k_tile_scan and are skipped here
 __global__ void __launch_bounds__(kSmallNT, 5) k_tile_sort(GeomView gv, BinView bv, uint32_t cap) {
@@ -422,9 +421,9 @@ int gsb_launch_tile_scan(const GeomView& gv, int ntiles, cudaStream_t st) {
 int gsb_launch_big_rects(int P, const GeomView& gv, unsigned long long* pairs, int W, int H, int exact_cull, uint32_t cap,
                          cudaStream_t st) {
   const int gx = (W + kBlock - 1) / kBlock;
-  constexpr int kGrid = 148 * 2;
-  if (pairs) k_big_rects<true><<<kGrid, kBigT, 0, st>>>(P, gv, pairs, W, H, gx, exact_cull, cap);
-  else k_big_rects<false><<<kGrid, kBigT, 0, st>>>(P, gv, nullptr, W, H, gx, exact_cull, cap);
+  const int grid = 2 * gsb_sm_count();
+  if (pairs) k_big_rects<true><<<grid, kBigT, 0, st>>>(P, gv, pairs, W, H, gx, exact_cull, cap);
+  else k_big_rects<false><<<grid, kBigT, 0, st>>>(P, gv, nullptr, W, H, gx, exact_cull, cap);
   GSB_CUDA(cudaGetLastError());
   return GSB_OK;
 }
@@ -451,7 +450,8 @@ int gsb_launch_binning(int P, const GeomView& gv, const BinView& bv, int W, int 
   {
     ProfScope ps(GSB_K_SORT_TILE, st, 2);
     k_tile_sort<<<gx * gy, kSmallNT, kSmallSmem, st>>>(gv, bv, cap);
-    k_tile_sort_long<<<kQueueCtas, kLargeNT, kLargeSmem, st>>>(gv, bv, cap);
+    // persistent CTAs draining the long-list queues, one per SM
+    k_tile_sort_long<<<gsb_sm_count(), kLargeNT, kLargeSmem, st>>>(gv, bv, cap);
   }
   GSB_CUDA(cudaGetLastError());
   return GSB_OK;

@@ -1,12 +1,12 @@
-// Per-tile alpha blend of the B200 rasterizer, forward and backward (SURVEY.md Appendix A.2.10 / A.3;
-// reference call site /root/reference/gaussian_renderer/__init__.py:126-135).
+// Per-tile alpha blend of the rasterizer, forward and backward (SURVEY.md Appendix A.2.10 / A.3;
+// reference call site gaussian_renderer/__init__.py:126-135).
 //
-//   k_blend_fwd2 / k_blend_bwd2   CTA = 16x16 tile (4 warps), warp = 8x8 block, TWO pixels per lane sharing dx;
-//                                 per-pair math issued as packed f32x2 (FFMA2/FMUL2/FADD2); per-warp
+//   k_blend_fwd2 / k_blend_bwd2   CTA = 16x16 tile (4 warps), warp = 8x8 block, TWO pixels per lane sharing dx
+//                                 (per-pair math on float2 lanes); per-warp
 //                                 ballot-compacted exact sub-tile culling.  Staging, three-deep software pipeline:
 //                                 the tile's sorted ID chunk arrives by a TMA bulk copy (cp.async.bulk + mbarrier)
 //                                 two chunks ahead, the 48-byte splat records of those ids are GATHERED with
-//                                 cp.async (LDGSTS) out of the L2-resident record table one chunk ahead, the
+//                                 cp.async (LDGSTS) out of the record table (mostly L2 hits) one chunk ahead, the
 //                                 current chunk is blended from shared memory.  No per-instance copy of the records
 //                                 is ever written to HBM, and nothing is fetched for the part of a list that early
 //                                 termination never reaches.
@@ -134,8 +134,25 @@ k_blend_fwd(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids, 
   }
 }
 
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+// *dscale = max |dL[i]| (float bits of non-negative floats order like the floats, so the integer max is exact and
+// independent of the order of the atomics)
+__global__ void __launch_bounds__(kThreads) k_abs_max(size_t n, const float* __restrict__ dL, uint32_t* __restrict__ dscale) {
+  float m = 0.f;
+  for (size_t e = (size_t)blockIdx.x * kThreads + threadIdx.x; e < n; e += (size_t)gridDim.x * kThreads)
+    m = fmaxf(m, fabsf(__ldg(dL + e)));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) atomicMax(dscale, __float_as_uint(m));
+}
+
+// Adds the warp's totals to a Gaussian's fixed-point slots.  After warp_reduce9 / warp_reduce8, lane 4i holds total i
+// (i < 8) in v0 and every lane holds total 8 in v8; lane 1 adds slot 8 when `ninth`.
+__device__ __forceinline__ void flush_fixed(unsigned long long* dst, float v0, float v8, float radius, float inv_m, int lane,
+                                            bool ninth) {
+  if ((lane & 3) == 0 || (ninth && lane == 1)) {
+    const int slot = (lane & 3) ? 8 : lane >> 2;
+    atomicAdd(dst + slot, fix_encode((lane & 3) ? v8 : v0, fix_scale(slot, radius, inv_m)));
+  }
 }
 
 // Reduce 9 per-lane values over the warp with 14 shuffles.  On return, lane l with (l & 3) == 0
@@ -216,9 +233,10 @@ __global__ void __launch_bounds__(kThreads)
 k_blend_bwd(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids, const float4* __restrict__ rec,
             const float* __restrict__ bg, int W, int H, int gx,
             const float* __restrict__ final_T, const uint32_t* __restrict__ n_contrib,
-            const float* __restrict__ dL_dpix, float* __restrict__ dacc) {
+            const float* __restrict__ dL_dpix, unsigned long long* __restrict__ dacc, const uint32_t* __restrict__ dscale) {
   __shared__ float4 sm0[kChunk1], sm1[kChunk1], sm2[kChunk1];
   __shared__ int s_bmax;
+  const float inv_m = fix_inv_m(dscale);
   const int tile = blockIdx.x;
   const int tx = tile % gx, ty = tile / gx;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -302,14 +320,7 @@ k_blend_bwd(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids, 
             v[8] = dchannel_dcolor * dLb;
           }
           warp_reduce9(v, lane);
-          // lane 4i holds total i (i < 8): pull 4 consecutive totals into lanes 0 and 16 and issue two
-          // 128-bit reductions (REDG.E.ADD.F32x4) + one scalar instead of nine scalar atomics
-          const float a1 = __shfl_down_sync(0xffffffffu, v[0], 4);
-          const float a2 = __shfl_down_sync(0xffffffffu, v[0], 8);
-          const float a3 = __shfl_down_sync(0xffffffffu, v[0], 12);
-          float* dst = dacc + (size_t)__float_as_uint(e1.w) * 12;
-          if ((lane & 15) == 0) red_add_v4(dst + (lane >> 2), v[0], a1, a2, a3);
-          if (lane == 1) atomicAdd(dst + 8, v[8]);
+          flush_fixed(dacc + (size_t)__float_as_uint(e1.w) * kDaccSlots, v[0], v[8], sm2[b + k].w, inv_m, lane, true);
         }
       }
     }
@@ -319,8 +330,8 @@ k_blend_bwd(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids, 
 
 // ------------------------------------------------------------------------------------------
 // blend v2: 4 warps per tile, each warp owns an 8x8 block = two 8x4 halves; every lane carries TWO
-// pixels (x, y) and (x, y+4) that share dx, and the per-pair arithmetic is issued as packed
-// FFMA2/FMUL2/FADD2 (Blackwell f32x2), so one instruction stream serves 64 (pixel, Gaussian) pairs.
+// pixels (x, y) and (x, y+4) that share dx, so the per-Gaussian loads, dx terms, cull test and
+// warp reduction are shared by 64 (pixel, Gaussian) pairs.
 // The sub-tile cull is evaluated per half and the loop runs over the union of the two masks.
 // ------------------------------------------------------------------------------------------
 constexpr int kThreads2 = 128;
@@ -480,20 +491,20 @@ k_blend_fwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids,
           const float2 dy = f2(e0.y - fy.x, e0.y - fy.y);
           const float c1 = e0.w * dx, c0 = e0.z * dx * dx;
           // power' = c0 + dy * (c1 + C' * dy)
-          const float2 pw = __ffma2_rn(dy, __ffma2_rn(f2s(e1.x), dy, f2s(c1)), f2s(c0));
+          const float2 pw = fma2(dy, fma2(f2s(e1.x), dy, f2s(c1)), f2s(c0));
           const float2 G = f2(ex2_approx(pw.x), ex2_approx(pw.y));
-          float2 al = __fmul2_rn(f2s(e1.y), G);
+          float2 al = mul2(f2s(e1.y), G);
           al.x = fminf(0.99f, al.x); al.y = fminf(0.99f, al.y);
           bool vA = !doneA && pw.x <= 0.f && al.x >= kAlphaMin;
           bool vB = !doneB && pw.y <= 0.f && al.y >= kAlphaMin;
-          const float2 tT = __fmul2_rn(T, __ffma2_rn(al, f2s(-1.f), f2s(1.f)));
+          const float2 tT = mul2(T, fma2(al, f2s(-1.f), f2s(1.f)));
           if (vA && tT.x < kTEps) { doneA = true; vA = false; }
           if (vB && tT.y < kTEps) { doneB = true; vB = false; }
-          float2 w = __fmul2_rn(al, T);
+          float2 w = mul2(al, T);
           w.x = vA ? w.x : 0.f; w.y = vB ? w.y : 0.f;
-          Cr = __ffma2_rn(f2s(c.x), w, Cr);
-          Cg = __ffma2_rn(f2s(c.y), w, Cg);
-          Cb = __ffma2_rn(f2s(c.z), w, Cb);
+          Cr = fma2(f2s(c.x), w, Cr);
+          Cg = fma2(f2s(c.y), w, Cg);
+          Cb = fma2(f2s(c.z), w, Cb);
           const uint32_t pos = (uint32_t)(base + b + k + 1);
           T.x = vA ? tT.x : T.x; T.y = vB ? tT.y : T.y;
           lastA = vA ? pos : lastA; lastB = vB ? pos : lastB;
@@ -534,9 +545,10 @@ __global__ void __launch_bounds__(kThreads2, GSB_BWD_MINB)
 k_blend_bwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids, const float4* __restrict__ rec,
              const float* __restrict__ bg, int W, int H, int gx,
              const float* __restrict__ final_T, const uint32_t* __restrict__ n_contrib,
-             const float* __restrict__ dL_dpix, float* __restrict__ dacc,
-             unsigned long long* __restrict__ stats = nullptr) {
+             const float* __restrict__ dL_dpix, unsigned long long* __restrict__ dacc,
+             const uint32_t* __restrict__ dscale, unsigned long long* __restrict__ stats = nullptr) {
   unsigned int st_iter = 0, st_red = 0, st_valid = 0;
+  const float inv_m = fix_inv_m(dscale);
   __shared__ __align__(128) SlabStage stg[2];
   __shared__ __align__(16) uint32_t sid[BULK ? 3 : 1][kIdRow];
   __shared__ __align__(8) uint64_t bars[3];
@@ -563,7 +575,7 @@ k_blend_bwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids,
   if (inA) { dLr.x = dL_dpix[pixA]; dLg.x = dL_dpix[hw + pixA]; dLb.x = dL_dpix[2 * hw + pixA]; }
   if (inB) { dLr.y = dL_dpix[pixB]; dLg.y = dL_dpix[hw + pixB]; dLb.y = dL_dpix[2 * hw + pixB]; }
   const float b0 = bg[0], b1 = bg[1], b2 = bg[2];
-  const float2 tf_bg = __fmul2_rn(T_final, f2(b0 * dLr.x + b1 * dLg.x + b2 * dLb.x, b0 * dLr.y + b1 * dLg.y + b2 * dLb.y));
+  const float2 tf_bg = mul2(T_final, f2(b0 * dLr.x + b1 * dLg.x + b2 * dLb.x, b0 * dLr.y + b1 * dLg.y + b2 * dLb.y));
   int wmaxA = lcA, wmaxB = lcB;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
@@ -619,9 +631,9 @@ k_blend_bwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids,
           const float dx = e0.x - fx;
           const float2 dy = f2(e0.y - fy.x, e0.y - fy.y);
           const float c1 = e0.w * dx, c0 = e0.z * dx * dx;
-          const float2 pw = __ffma2_rn(dy, __ffma2_rn(f2s(e1.x), dy, f2s(c1)), f2s(c0));
+          const float2 pw = fma2(dy, fma2(f2s(e1.x), dy, f2s(c1)), f2s(c0));
           const float2 G = f2(ex2_approx(pw.x), ex2_approx(pw.y));
-          const float2 alu = __fmul2_rn(f2s(e1.y), G);           // opacity * G (unclamped: the straight-through alpha)
+          const float2 alu = mul2(f2s(e1.y), G);           // opacity * G (unclamped: the straight-through alpha)
           const bool vA = inA && pos < lcA && pw.x <= 0.f && alu.x >= kAlphaMin;      // min(0.99, a) >= 1/255 <=> a >= 1/255
           const bool vB = inB && pos < lcB && pw.y <= 0.f && alu.y >= kAlphaMin;
           if (STATS) { ++st_iter; st_valid += (vA ? 1u : 0u) + (vB ? 1u : 0u); }
@@ -631,25 +643,25 @@ k_blend_bwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids,
           // masked alphas: an invalid pixel behaves as alpha = 0 (T, accumulator and every moment unchanged)
           const float2 aw = f2(vA ? alu.x : 0.f, vB ? alu.y : 0.f);              // weight of the moments (unclamped)
           const float2 am = f2(fminf(0.99f, aw.x), fminf(0.99f, aw.y));          // blending alpha (clamped)
-          const float2 one_m = __ffma2_rn(am, f2s(-1.f), f2s(1.f));
+          const float2 one_m = fma2(am, f2s(-1.f), f2s(1.f));
           const float2 inv = f2(rcp_approx(one_m.x), rcp_approx(one_m.y));
-          T = __fmul2_rn(T, inv);
-          const float2 dcol = __fmul2_rn(am, T);                 // dchannel/dcolor = alpha * T
+          T = mul2(T, inv);
+          const float2 dcol = mul2(am, T);                 // dchannel/dcolor = alpha * T
           // acc = colour composited from everything BEHIND this entry (the reference's accum_rec);
           // dL/dalpha = T * sum_ch (c - acc) dL_ch  -  T_final/(1-alpha) * bg.dL ; then acc += alpha (c - acc)
-          const float2 d_r = __fadd2_rn(f2s(c.x), f2(-acc_r.x, -acc_r.y));
-          const float2 d_g = __fadd2_rn(f2s(c.y), f2(-acc_g.x, -acc_g.y));
-          const float2 d_b = __fadd2_rn(f2s(c.z), f2(-acc_b.x, -acc_b.y));
-          float2 da = __ffma2_rn(d_b, dLb, __ffma2_rn(d_g, dLg, __fmul2_rn(d_r, dLr)));
-          da = __fmul2_rn(da, T);
-          da = __ffma2_rn(f2(-tf_bg.x, -tf_bg.y), inv, da);
-          acc_r = __ffma2_rn(am, d_r, acc_r);
-          acc_g = __ffma2_rn(am, d_g, acc_g);
-          acc_b = __ffma2_rn(am, d_b, acc_b);
+          const float2 d_r = add2(f2s(c.x), f2(-acc_r.x, -acc_r.y));
+          const float2 d_g = add2(f2s(c.y), f2(-acc_g.x, -acc_g.y));
+          const float2 d_b = add2(f2s(c.z), f2(-acc_b.x, -acc_b.y));
+          float2 da = fma2(d_b, dLb, fma2(d_g, dLg, mul2(d_r, dLr)));
+          da = mul2(da, T);
+          da = fma2(f2(-tf_bg.x, -tf_bg.y), inv, da);
+          acc_r = fma2(am, d_r, acc_r);
+          acc_g = fma2(am, d_g, acc_g);
+          acc_b = fma2(am, d_b, acc_b);
           // w = dL/dalpha * opacity * G, zero on invalid pixels through aw.  The warp accumulates the raw moments of w;
           // the per-Gaussian constants (conic, 1/opacity) are applied once in k_preprocess_bwd.
-          const float2 w = __fmul2_rn(aw, da);
-          const float2 wy = __fmul2_rn(w, dy);
+          const float2 w = mul2(aw, da);
+          const float2 wy = mul2(w, dy);
           const float ws = w.x + w.y;
           float v[9];
           v[0] = ws * dx;                                        // S w dx
@@ -662,14 +674,8 @@ k_blend_bwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids,
           v[8] = dcol.x * dLb.x + dcol.y * dLb.y;
           v[5] = POSE_ONLY ? v[8] : ws;                          // S w (or dL/db in the 8-value layout)
           if (POSE_ONLY) warp_reduce8(v, lane); else warp_reduce9(v, lane);
-          const float a1 = __shfl_down_sync(0xffffffffu, v[0], 4);
-          const float a2 = __shfl_down_sync(0xffffffffu, v[0], 8);
-          const float a3 = __shfl_down_sync(0xffffffffu, v[0], 12);
-          float* dst = dacc + (size_t)__float_as_uint(e1.w) * 12;
-          if (!STATS) {
-            if ((lane & 15) == 0) red_add_v4(dst + (lane >> 2), v[0], a1, a2, a3);
-            if (!POSE_ONLY && lane == 1) atomicAdd(dst + 8, v[8]);
-          }
+          if (!STATS)
+            flush_fixed(dacc + (size_t)__float_as_uint(e1.w) * kDaccSlots, v[0], v[8], c.w, inv_m, lane, !POSE_ONLY);
         }
       }
     }
@@ -709,22 +715,26 @@ int gsb_launch_blend_fwd(const GeomView& gv, const BinView& bv, const ImgView& i
 }
 
 int gsb_launch_blend_bwd(const GeomView& gv, const BinView& bv, const ImgView& iv, const float* bg, int W, int H, const float* dL_dout,
-                         float* dacc, bool pose_only, cudaStream_t st) {
+                         bool pose_only, cudaStream_t st) {
   const int gx = (W + kBlock - 1) / kBlock, gy = (H + kBlock - 1) / kBlock;
-  ProfScope ps(GSB_K_BLEND_BWD, st);
+  ProfScope ps(GSB_K_BLEND_BWD, st, 2);
+  const size_t n = (size_t)3 * W * H;
+  const size_t nb = (n + kThreads - 1) / kThreads, max_blocks = 4 * (size_t)gsb_sm_count();
+  k_abs_max<<<(int)(nb < max_blocks ? nb : max_blocks), kThreads, 0, st>>>(n, dL_dout, gv.dscale);
   const int ver = gsb_option_blend_version(), bulk = gsb_option_stage_bulk();
+  unsigned long long* dacc = gv.dacc;
   if (pose_only)
     k_blend_bwd2<true, false, true><<<gx * gy, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, iv.final_T,
-                                                                   iv.n_contrib, dL_dout, dacc);
+                                                                   iv.n_contrib, dL_dout, dacc, gv.dscale);
   else if (ver == 2 && bulk)
     k_blend_bwd2<true><<<gx * gy, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, iv.final_T,
-                                                      iv.n_contrib, dL_dout, dacc);
+                                                      iv.n_contrib, dL_dout, dacc, gv.dscale);
   else if (ver == 2)
     k_blend_bwd2<false><<<gx * gy, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, iv.final_T,
-                                                       iv.n_contrib, dL_dout, dacc);
+                                                       iv.n_contrib, dL_dout, dacc, gv.dscale);
   else
     k_blend_bwd<<<gx * gy, kThreads, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, iv.final_T, iv.n_contrib,
-                                              dL_dout, dacc);
+                                              dL_dout, dacc, gv.dscale);
   GSB_CUDA(cudaGetLastError());
   return GSB_OK;
 }
@@ -749,7 +759,7 @@ extern "C" GSB_API int gsb_blend_stats(const GsbCamera* cam, int32_t P, void* ge
                                                           iv.final_T, iv.n_contrib, stats);
   if (dL_dout)
     k_blend_bwd2<true, true><<<gx * gy, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, cam->bg, W, H, gx, iv.final_T,
-                                                            iv.n_contrib, dL_dout, (float*)gv.dacc, stats);
+                                                            iv.n_contrib, dL_dout, gv.dacc, gv.dscale, stats);
   GSB_CUDA(cudaGetLastError());
   return GSB_OK;
 }

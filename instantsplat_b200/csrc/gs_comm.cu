@@ -1,4 +1,4 @@
-// Fused reduce-scatter -> per-point Adam -> all-gather over NVLink peer memory (sm_100a).
+// Fused reduce-scatter -> per-point Adam -> all-gather over NVLink peer memory (sm_90a).
 //
 // Multi-GPU exchange of the view-sharded optimisation loop (SURVEY.md section 8e / 5.8): every rank
 // holds a full replica of the flat parameter buffer and has just written its view's gradients into

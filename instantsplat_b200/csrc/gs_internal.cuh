@@ -42,6 +42,7 @@ struct ProfScope {
 };
 int gsb_option_blend_version();
 int gsb_option_stage_bulk();
+int gsb_sm_count();
 
 namespace gsb {
 
@@ -58,6 +59,40 @@ enum { kStR = 0, kStOverflow = 1, kStMaxList = 2, kStHugeTiles = 3, kStNLarge = 
 // kernel; longer lists are queued by k_tile_scan and drained by two persistent kernels
 constexpr uint32_t kSmallList = 2048, kLargeList = 8192;
 
+// ---- fixed-point backward accumulators ----------------------------------------------------
+// The blend backward adds per-Gaussian pixel moments from many tiles.  Floating-point atomics would make each sum
+// depend on the order in which the CTAs arrive, so the gradients -- and, through Adam, a whole training run -- would
+// differ from run to run.  The moments are added as 64-bit integers instead; integer addition is associative, so every
+// run produces the same bits.  Slot k of Gaussian i counts in units of 1 / fix_scale(k, radius_i, M) with
+// M = max |dL/dpixel| of the launch: |slot k| <= c * M * (radius + 1)^fix_exp(k) for a small constant c (pixels covered
+// ~ radius^2, |dx|, |dy| <= radius), so the unit 2^-50 * M * (radius + 1)^fix_exp(k) leaves 13 bits of headroom above
+// that bound and ~50 bits of resolution below it -- finer than the float each contribution starts from.
+// Slots: [S w dx, S w dy, S w dx^2, S w dx dy, S w dy^2, S w (tracking: dL/db), dL/dr, dL/dg, dL/db].
+constexpr int kDaccSlots = 9;
+__host__ __device__ constexpr int fix_exp(int k) { return k < 2 ? 3 : (k < 5 ? 4 : 2); }
+#if defined(__CUDACC__)
+// 2^50 / M (M floored at 1e-20 so that the scale stays a finite float)
+__device__ __forceinline__ float fix_inv_m(const uint32_t* dscale) {
+  return __fdiv_rn(0x1p50f, fmaxf(__uint_as_float(*dscale), 1e-20f));
+}
+// integer steps per unit of slot k for a Gaussian of the given radius.  Encoder and decoder evaluate the same expression
+// (MUFU.RCP is deterministic), so the approximate reciprocal costs nothing in reproducibility.
+__device__ __forceinline__ float fix_scale(int k, float radius, float inv_m) {
+  float ri;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(ri) : "f"(radius + 1.f));
+  const int e = fix_exp(k);
+  float s = __fmul_rn(__fmul_rn(inv_m, ri), ri);
+  if (e >= 3) s = __fmul_rn(s, ri);
+  if (e >= 4) s = __fmul_rn(s, ri);
+  return s;
+}
+__device__ __forceinline__ unsigned long long fix_encode(float x, float scale) {
+  return (unsigned long long)__float2ll_rn(__fmul_rn(x, scale));
+}
+// unit = 1 / fix_scale(...) in double, computed once per Gaussian and exponent
+__device__ __forceinline__ float fix_decode(unsigned long long a, double unit) { return (float)((double)(long long)a * unit); }
+#endif
+
 // ---- geom: P-sized scratch + per-tile counters (caller-owned, gsb_geom_bytes) -------------
 struct GeomView {
   CamConst* cam;
@@ -67,7 +102,8 @@ struct GeomView {
   float4* brec;        // [P] binning record: depth, rect x (rx0 | rx1<<16), rect y (ry0 | ry1<<16), keep mask (bits)
   uint32_t* tiles;     // tile instances per Gaussian (after culling)
   uint8_t* clamped;
-  float4* dacc;        // [3P] backward accumulators
+  unsigned long long* dacc;   // [kDaccSlots * P] backward accumulators, fixed point (see fix_scale)
+  uint32_t* dscale;    // [1] max |dL/dpixel| of the current backward (float bits), the unit of the fixed point
   float* pose_part;    // [nblocks*16]
   float* pose_acc;     // [16]
   uint32_t* status;    // [kStWords]
@@ -92,7 +128,8 @@ static inline GeomView geom_view(void* base, int P) {
   v.brec = (float4*)take(Pp * 16);
   v.tiles = (uint32_t*)take(Pp * 4);
   v.clamped = (uint8_t*)take(Pp);
-  v.dacc = (float4*)take(Pp * 48);
+  v.dacc = (unsigned long long*)take(Pp * kDaccSlots * 8);
+  v.dscale = (uint32_t*)take(4);
   size_t nb = (Pp + kPT - 1) / kPT;
   v.pose_part = (float*)take(nb * 16 * 4);
   v.pose_acc = (float*)take(16 * 4);
@@ -158,5 +195,6 @@ int gsb_launch_binning(int P, const gsb::GeomView& gv, const gsb::BinView& bv, i
 int gsb_launch_blend_fwd(const gsb::GeomView& gv, const gsb::BinView& bv, const gsb::ImgView& iv, const float* bg, int W, int H,
                          float* out_color, cudaStream_t st);
 // pose_only: 8-value accumulator layout (dacc[5] = dL/db, no dL/dopacity), see k_blend_bwd2
+// computes max |dL_dout| into gv.dscale (zeroed by the caller, as is gv.dacc), then the blend backward into gv.dacc
 int gsb_launch_blend_bwd(const gsb::GeomView& gv, const gsb::BinView& bv, const gsb::ImgView& iv, const float* bg, int W, int H,
-                         const float* dL_dout, float* dacc, bool pose_only, cudaStream_t st);
+                         const float* dL_dout, bool pose_only, cudaStream_t st);

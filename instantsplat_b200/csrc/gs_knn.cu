@@ -1,6 +1,6 @@
-// simple_knn._C.distCUDA2 replacement for sm_100a (SURVEY.md section 8 row f1): mean squared distance to the
+// simple_knn._C.distCUDA2 replacement for sm_90a (SURVEY.md section 8 row f1): mean squared distance to the
 // 3 nearest neighbours of every point, used ONCE at initialisation to set the Gaussians' log-scales
-// (/root/reference/scene/gaussian_model.py:20,156-160).  The reference's module (gitlab.inria.fr/bkerbl/simple-knn
+// (scene/gaussian_model.py:20,156-160).  The reference's module (gitlab.inria.fr/bkerbl/simple-knn
 // @ 86710c2) is an empty submodule; its published behaviour is an exact 3-NN (Morton order + box pruning).
 //
 // Here: uniform grid hash (cell ids sorted with cub), then one thread per point searches growing cubes of cells
@@ -16,6 +16,7 @@
 
 void gsb_set_error(const char* s);
 void gsb_count_launch(int n);
+int gsb_sm_count();
 
 namespace {
 
@@ -213,7 +214,8 @@ extern "C" GSB_API int gsb_knn_mean_dist2(int32_t P, const float* points, float*
   if (e == cudaSuccess) {
     const int nb = (P + 255) / 256;
     gsb_count_launch(6);
-    k_bbox<<<nb < 1184 ? nb : 1184, 256, 0, st>>>(P, points, s.bbox);
+    const int max_blocks = 8 * gsb_sm_count();
+    k_bbox<<<nb < max_blocks ? nb : max_blocks, 256, 0, st>>>(P, points, s.bbox);
     k_make_grid<<<1, 32, 0, st>>>(s.bbox, n, s.grid);
     k_cell_ids<<<nb, 256, 0, st>>>(P, points, s.grid, s.cid, s.idx);
     int bits = 1;

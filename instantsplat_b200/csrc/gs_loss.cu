@@ -1,10 +1,10 @@
-// Fused SSIM / L1 loss kernels for sm_100a (C ABI in include/gsb200.h).
+// Fused SSIM / L1 loss kernels for sm_90a (C ABI in include/gsb200.h).
 //
-// Replaces fused_ssim.fused_ssim (/root/reference/train.py:39-43,172-173; an empty submodule,
+// Replaces fused_ssim.fused_ssim (train.py:39-43,172-173; an empty submodule,
 // rahul-goel/fused-ssim @ a7c48d6) whose semantics are those of the reference's PyTorch fallback
-// /root/reference/utils/loss_utils.py:55-85: 11x11 Gaussian window sigma 1.5, zero "same"
+// utils/loss_utils.py:55-85: 11x11 Gaussian window sigma 1.5, zero "same"
 // padding, C1 = 0.01^2, C2 = 0.03^2, per-channel (depthwise), mean over all elements -- plus
-// l1_loss (/root/reference/utils/loss_utils.py:39-40) and the combine of train.py:176.
+// l1_loss (utils/loss_utils.py:39-40) and the combine of train.py:176.
 //
 // One CTA = one 32x16 output tile of one channel: the (32+10)x(16+10) halo of both images is staged
 // in shared memory once and the 11-tap window is applied separably with register tiling (4 outputs
@@ -15,6 +15,10 @@
 #include <stdio.h>
 
 #include "../../include/gsb200.h"
+#include "gs_math.cuh"
+
+using gsb::fma2;
+using gsb::mul2;
 
 void gsb_set_error(const char* s);
 void gsb_count_launch(int n);
@@ -108,9 +112,8 @@ __device__ __forceinline__ void halo_store1(const HaloRegs& p, float (*dst)[EWP]
 }
 __device__ __forceinline__ float2 bcast(float w) { return make_float2(w, w); }
 
-// Register-tiled separable 11-tap filter, packed f32x2 arithmetic (Blackwell FFMA2): the five windowed statistics
-// are carried as {E[a], E[b]}, {E[a^2], E[b^2]} (two packed accumulators) and E[ab] (scalar), i.e. 3 FMA-class
-// instructions per tap and output instead of 5.  Horizontal: thread -> (row, 4 adjacent columns), inputs fetched
+// Register-tiled separable 11-tap filter: the five windowed statistics are carried as {E[a], E[b]}, {E[a^2], E[b^2]}
+// (two float2 accumulators) and E[ab] (scalar).  Horizontal: thread -> (row, 4 adjacent columns), inputs fetched
 // with seven 128-bit shared loads.  Vertical: thread -> (column, 2 adjacent rows).
 // img planes [BC][H][W].  maps (optional) [3][BC][H][W].  sums[0] += sum|a-b| (if do_l1), sums[1] += sum ssim.
 __global__ void __launch_bounds__(256, 4)
@@ -143,15 +146,15 @@ k_ssim_fwd(int H, int W, const float* __restrict__ img1, const float* __restrict
       for (int h = 0; h < 2; ++h) {
         const int i = 2 * q + h;
         const float2 ab = h ? make_float2(v.z, v.w) : make_float2(v.x, v.y);
-        const float2 sq = __fmul2_rn(ab, ab);
+        const float2 sq = mul2(ab, ab);
         const float x = ab.x * ab.y;
 #pragma unroll
         for (int o = 0; o < 4; ++o) {
           const int t = i - o;
           if (t >= 0 && t < 11) {
             const float w = c_win[t];
-            a1[o] = __ffma2_rn(bcast(w), ab, a1[o]);
-            a2[o] = __ffma2_rn(bcast(w), sq, a2[o]);
+            a1[o] = fma2(bcast(w), ab, a1[o]);
+            a2[o] = fma2(bcast(w), sq, a2[o]);
             a3[o] = fmaf(w, x, a3[o]);
           }
         }
@@ -175,8 +178,8 @@ k_ssim_fwd(int H, int W, const float* __restrict__ img1, const float* __restrict
       const int t = i - o;
       if (t >= 0 && t < 11) {
         const float w = c_win[t];
-        m[o] = __ffma2_rn(bcast(w), v1, m[o]);
-        e[o] = __ffma2_rn(bcast(w), v2, e[o]);
+        m[o] = fma2(bcast(w), v1, m[o]);
+        e[o] = fma2(bcast(w), v2, e[o]);
         e12[o] = fmaf(w, v3, e12[o]);
       }
     }
@@ -212,7 +215,7 @@ k_ssim_fwd(int H, int W, const float* __restrict__ img1, const float* __restrict
 }
 
 // out = ssim_scale * (conv(m_mu) + 2 x conv(m_s1) + y conv(m_s12)) [* *dyn_scale] + l1_scale * sign(x-y)
-// The first two maps travel as one packed float2 through both filter passes (2 FMA-class instructions per tap).
+// The first two maps travel as one float2 through both filter passes.
 __global__ void __launch_bounds__(256, 5)
 k_ssim_bwd(int H, int W, const float* __restrict__ img1, const float* __restrict__ img2,
            const float* __restrict__ maps, size_t plane_total, float ssim_scale,
@@ -257,7 +260,7 @@ k_ssim_bwd(int H, int W, const float* __restrict__ img1, const float* __restrict
           const int t = i - o;
           if (t >= 0 && t < 11) {
             const float w = c_win[t];
-            a12[o] = __ffma2_rn(bcast(w), p, a12[o]);
+            a12[o] = fma2(bcast(w), p, a12[o]);
             a3[o] = fmaf(w, m3[i], a3[o]);
           }
         }
@@ -281,7 +284,7 @@ k_ssim_bwd(int H, int W, const float* __restrict__ img1, const float* __restrict
       const int t = i - o;
       if (t >= 0 && t < 11) {
         const float w = c_win[t];
-        g12[o] = __ffma2_rn(bcast(w), v12, g12[o]);
+        g12[o] = fma2(bcast(w), v12, g12[o]);
         g3[o] = fmaf(w, v3, g3[o]);
       }
     }

@@ -1,13 +1,13 @@
-// Per-Gaussian and per-pair arithmetic of the B200 rasterizer, written once as
-// __host__ __device__ inline functions so the same code runs inside the sm_100a kernels
+// Per-Gaussian and per-pair arithmetic of the rasterizer, written once as
+// __host__ __device__ inline functions so the same code runs inside the sm_90a kernels
 // (gs_raster.cu) and inside the CPU math harness tests compile with g++ (tests/host_math.cpp).
 //
 // Behaviour follows SURVEY.md Appendix A (the published algorithm of
-// graphdeco-inria/diff-gaussian-rasterization @ 59f5f77, an empty submodule in /root/reference),
-// anchored on the reference call site /root/reference/gaussian_renderer/__init__.py:60-135.
-// The InstantSplat pose pre-transform (/root/reference/gaussian_renderer/__init__.py:81-89,
-// /root/reference/utils/pose_utils.py:10-55,86-104) and the parameter activations
-// (/root/reference/scene/gaussian_model.py:101-121) are fused in.
+// graphdeco-inria/diff-gaussian-rasterization @ 59f5f77, an empty submodule in the reference checkout),
+// anchored on the reference call site gaussian_renderer/__init__.py:60-135.
+// The InstantSplat pose pre-transform (gaussian_renderer/__init__.py:81-89,
+// utils/pose_utils.py:10-55,86-104) and the parameter activations
+// (scene/gaussian_model.py:101-121) are fused in.
 #pragma once
 #include <math.h>
 #include <stdint.h>
@@ -70,7 +70,7 @@ GS_HD void quat_to_R_bwd(float r, float x, float y, float z, const float* dR, fl
 }
 
 // Fill the pose part of CamConst from pose = [qw,qx,qy,qz,tx,ty,tz]
-// (/root/reference/utils/pose_utils.py:34-55 normalises; quadmultiply :86-104 does not).
+// (utils/pose_utils.py:34-55 normalises; quadmultiply :86-104 does not).
 GS_HD void pose_to_const(const float* pose, CamConst& c) {
   float n = sqrtf(pose[0] * pose[0] + pose[1] * pose[1] + pose[2] * pose[2] + pose[3] * pose[3]);
   quat_to_R(pose[0] / n, pose[1] / n, pose[2] / n, pose[3] / n, c.Rc);
@@ -532,5 +532,16 @@ GS_HD void project_bwd(const CamConst& c, const GaussIn& in, const Proj& p, cons
     g.dq[0] = dq[0]; g.dq[1] = dq[1]; g.dq[2] = dq[2]; g.dq[3] = dq[3];
   }
 }
+
+#if defined(__CUDACC__)
+// Lane-wise float2 arithmetic, rounded like the scalar __f*_rn intrinsics (never contracted), used where the blend and
+// loss kernels carry two pixels or two statistics per register pair.  sm_90 has no packed FP32x2 instructions, so each
+// call issues two FFMA / FMUL / FADD.
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+#endif
 
 }  // namespace gsb

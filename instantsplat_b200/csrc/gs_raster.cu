@@ -1,6 +1,6 @@
-// B200 (sm_100a) differentiable Gaussian rasterizer: per-Gaussian kernels + C ABI (include/gsb200.h).
+// H100 (sm_90a) differentiable Gaussian rasterizer: per-Gaussian kernels + C ABI (include/gsb200.h).
 //
-// Pipeline (one view), every kernel hand-written for sm_100a, no library sort/scan, no host round trip:
+// Pipeline (one view), every kernel hand-written for sm_90a, no library sort/scan, no host round trip:
 //   k_setup_cam        camera/pose constants -> one CamConst in HBM (read by every block)
 //   k_preprocess       fused pose transform + activations + EWA projection + SH->RGB, 128-bit
 //                      coalesced loads staged through shared memory; writes packed splat records and
@@ -8,12 +8,12 @@
 //   k_tile_scan        (gs_bin.cu) exclusive scan of the per-tile counts -> segment offsets, R on device
 //   k_scatter          (gs_bin.cu) (depth | id) keys appended to the tiles' segments
 //   k_tile_sort        (gs_bin.cu) per-tile shared-memory sort + gather into contiguous per-tile slabs
-//   k_blend_fwd2       (gs_blend.cu) one CTA per 16x16 tile, TMA-staged slab chunks, packed f32x2 math
+//   k_blend_fwd2       (gs_blend.cu) one CTA per 16x16 tile, TMA-staged slab chunks, two pixels per lane
 //   k_blend_bwd2       (gs_blend.cu) back-to-front replay, 9 gradients per (warp, Gaussian) reduced in-warp
 //   k_preprocess_bwd   analytic backward to the model's own tensors + in-kernel pose-gradient
 //                      reduction; k_pose_finalize chains it to dL/dP[7]
 //
-// Reference behaviour: SURVEY.md Appendix A; call site /root/reference/gaussian_renderer/__init__.py:60-135.
+// Reference behaviour: SURVEY.md Appendix A; call site gaussian_renderer/__init__.py:60-135.
 #include <string.h>
 
 #include "gs_internal.cuh"
@@ -85,7 +85,18 @@ static std::atomic<int> g_blend_version{2};
 static std::atomic<int> g_stage_bulk{1};   // 1: slabs staged with cp.async.bulk (TMA) + mbarrier, 0: cooperative loads
 int gsb_option_blend_version() { return g_blend_version.load(std::memory_order_relaxed); }
 int gsb_option_stage_bulk() { return g_stage_bulk.load(std::memory_order_relaxed); }
-// option "blend_version": 1 = one pixel per lane (8 warps / tile; cross-check), 2 = two pixels per lane + packed f32x2 (default)
+// SM count of the current device, cached per device: sizes the persistent and grid-stride launches (132 on an H100 SXM)
+int gsb_sm_count() {
+  static std::atomic<int> sms[64];
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+  n = sms[dev].load(std::memory_order_relaxed);
+  if (n > 0) return n;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
+  sms[dev] = n;
+  return n;
+}
+// option "blend_version": 1 = one pixel per lane (8 warps / tile; cross-check), 2 = two pixels per lane (default)
 extern "C" GSB_API int gsb_set_option(const char* name, int value) {
   if (name && strcmp(name, "blend_version") == 0 && value >= 1 && value <= 2) { g_blend_version = value; return GSB_OK; }
   if (name && strcmp(name, "stage_bulk") == 0 && (value == 0 || value == 1)) { g_stage_bulk = value; return GSB_OK; }
@@ -273,7 +284,7 @@ __device__ __forceinline__ void load_block_inputs(const InPtrs& in, int first, i
 // The same full-CTA fast path with the copies done by the TMA unit: one thread arms an mbarrier with the byte count and
 // issues one bulk copy per input array (cp.async.bulk.shared.global, SASS UBLKCP); nothing passes through registers or
 // allocates L1 lines (with register staging, the 180 KB a resident set of CTAs keeps in flight is bounded by the L1
-// carve-out: giving shared memory the whole unified storage made both per-Gaussian kernels 8-13 % slower).
+// carve-out, so giving shared memory the whole unified storage does not help).
 __device__ __forceinline__ bool block_inputs_bulk_ok(const InPtrs& in, int nv, bool use_sh, int M) {
   return in.vec_ok != 0 && nv == kPT && in.scales && in.rots && (!use_sh || (!in.sh_packed && M == 16));
 }
@@ -476,8 +487,18 @@ k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out
   float* row_rest = sm + kSmSh + sr.rest_off + sr.rest_stride * t;
   bool has = false;
   if (t < nv) {
-    float4 d0 = gv.dacc[3 * (size_t)i], d1 = gv.dacc[3 * (size_t)i + 1], d2 = gv.dacc[3 * (size_t)i + 2];
-    float ds[9] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w, d2.x};
+    // the record (and its radius) is only written for Gaussians that cover a tile; the others have no moments
+    float ds[kDaccSlots];
+#pragma unroll
+    for (int k = 0; k < kDaccSlots; ++k) ds[k] = 0.f;
+    if (gv.tiles[i] > 0) {
+      const unsigned long long* acc = gv.dacc + (size_t)i * kDaccSlots;
+      const float radius = gv.rec[3 * (size_t)i + 2].w, inv_m = fix_inv_m(gv.dscale);
+      const double unit[3] = {1.0 / (double)fix_scale(5, radius, inv_m), 1.0 / (double)fix_scale(0, radius, inv_m),
+                              1.0 / (double)fix_scale(2, radius, inv_m)};      // exponents 2, 3, 4
+#pragma unroll
+      for (int k = 0; k < kDaccSlots; ++k) ds[k] = fix_decode(acc[k], unit[fix_exp(k) - 2]);
+    }
     if (pose_only_layout) { ds[8] = ds[5]; ds[5] = 0.f; }     // tracking mode: dacc[5] carries dL/db, no dL/dopacity
     bool any = false;
 #pragma unroll
@@ -742,13 +763,14 @@ extern "C" GSB_API int gsb_backward(const GsbCamera* cam, const GsbGaussians* g,
     if (grads->dL_dpose) GSB_CUDA(cudaMemsetAsync(grads->dL_dpose, 0, 7 * 4, st));
     return GSB_OK;
   }
-  GSB_CUDA(cudaMemsetAsync(gv.dacc, 0, (size_t)P * 48, st));
+  GSB_CUDA(cudaMemsetAsync(gv.dacc, 0, (size_t)P * kDaccSlots * 8, st));
+  GSB_CUDA(cudaMemsetAsync(gv.dscale, 0, 4, st));
   // tracking mode (render.py:99-170): only dL/dpose is wanted -> the blend backward reduces 8 values instead of 9
   const bool pose_only = g->pose && grads->dL_dpose && !grads->dL_dmeans3D && !grads->dL_dmeans2D && !grads->dL_dscales &&
                          !grads->dL_drotations && !grads->dL_dopacities && !grads->dL_dsh_dc && !grads->dL_dsh_rest &&
                          !grads->dL_dcolors && !grads->dL_dcov3D && gsb_option_blend_version() == 2 &&
                          gsb_option_stage_bulk() == 1;
-  rc = gsb_launch_blend_bwd(gv, bv, iv, cam->bg, W, H, dL_dout, (float*)gv.dacc, pose_only, st);
+  rc = gsb_launch_blend_bwd(gv, bv, iv, cam->bg, W, H, dL_dout, pose_only, st);
   if (rc) return rc;
   OutPtrs out;
   out.dmeans = grads->dL_dmeans3D; out.dmeans2D = grads->dL_dmeans2D; out.dscales = grads->dL_dscales;

@@ -1,5 +1,5 @@
 // Pose-only "tracking" mode (SURVEY.md section 8 row f2): the test-view pose optimisation of
-// /root/reference/render.py:99-170 -- Gaussians frozen, 500 Adam iterations on the 7 pose parameters of one view
+// render.py:99-170 -- Gaussians frozen, 500 Adam iterations on the 7 pose parameters of one view
 // under a masked L1 loss -- as device-resident steps, so that the whole loop runs without a single host sync:
 //
 //   gsb_l1_mask_fwd_bwd   loss and dL/dimage of utils/loss_utils.py:17-23 (l1_loss_mask) with the mask of
@@ -94,7 +94,8 @@ extern "C" GSB_API int gsb_l1_mask_fwd_bwd(int32_t C, int32_t H, int32_t W, cons
   cudaStream_t st = (cudaStream_t)stream_;
   GSB_REQUIRE(C > 0 && H > 0 && W > 0 && img && gt && sums && dL_dimg, "gsb_l1_mask_fwd_bwd: bad argument");
   const size_t n = (size_t)C * H * W;
-  const int blocks = (int)((n / 4 + kLT - 1) / kLT < 148 * 8 ? (n / 4 + kLT - 1) / kLT + 1 : 148 * 8);
+  const int max_blocks = 8 * gsb_sm_count();
+  const int blocks = (int)((n / 4 + kLT - 1) / kLT < (size_t)max_blocks ? (n / 4 + kLT - 1) / kLT + 1 : max_blocks);
   ProfScope ps(GSB_K_LOSS_FWD, st);
   k_l1_mask<<<blocks, kLT, 0, st>>>(n, img, gt, threshold, sums, dL_dimg);
   GSB_CUDA(cudaGetLastError());

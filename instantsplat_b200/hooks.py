@@ -4,8 +4,8 @@ The native packages (`diff_gaussian_rasterization`, `fused_ssim`, `simple_knn`) 
 <repo>/shims on PYTHONPATH.  Two replacements live INSIDE the reference's own packages and cannot be shadowed by a
 path entry:
 
-  * `scene.per_point_adam`  (imported by /root/reference/scene/gaussian_model.py:26) -> the fused sm_100a optimizer;
-  * `gaussian_renderer.render` (imported by /root/reference/train.py:24, render.py:27) -> the fused render body.
+  * `scene.per_point_adam`  (imported by scene/gaussian_model.py:26) -> the fused sm_90a optimizer;
+  * `gaussian_renderer.render` (imported by train.py:24, render.py:27) -> the fused render body.
 
 `install()` registers a meta-path finder that serves `scene.per_point_adam` from `instantsplat_b200.per_point_adam`
 and, when GSB_FUSED_RENDER=1 (default), swaps `gaussian_renderer.render` for `instantsplat_b200.renderer.render` right
@@ -14,7 +14,7 @@ after the reference's module has been executed (its other exports -- `network_gu
 
     PYTHONPATH=<repo>/shims:<repo> python train.py -s <scene> -m <out> --pp_optimizer --optim_pose ...
 
-runs the unchanged train.py on the B200 kernels.  GSB_HOOKS=0 disables the hook, GSB_FUSED_RENDER=0 keeps the
+runs the unchanged train.py on the H100 kernels.  GSB_HOOKS=0 disables the hook, GSB_FUSED_RENDER=0 keeps the
 reference's own render() body (PyTorch pose pre-transform -> GaussianRasterizer shim).
 """
 import importlib

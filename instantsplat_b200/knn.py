@@ -1,4 +1,4 @@
-"""`simple_knn._C.distCUDA2` replacement (/root/reference/scene/gaussian_model.py:20,156; SURVEY.md section 8 row
+"""`simple_knn._C.distCUDA2` replacement (scene/gaussian_model.py:20,156; SURVEY.md section 8 row
 f1: runs once at initialisation, not on the per-iteration path).
 
 distCUDA2(points [P,3]) -> [P] mean squared distance to the 3 nearest neighbours, computed exactly by the grid-hash

@@ -1,13 +1,13 @@
 """Host-side mirror of the part of the reference's `GaussianModel` that the training hot path touches
-(/root/reference/scene/gaussian_model.py): parameter tensors and their activations (:101-121), the pose table
+(scene/gaussian_model.py): parameter tensors and their activations (:101-121), the pose table
 (:126-136), `oneupSHdegree` (:142-144), `create_from_pcd` (:146-172, with `distCUDA2` served by libgsb200.so),
 `training_setup_pp` (:203-232), `update_learning_rate` (:234-243) and the optimizer-state surgery behind
 densify / prune / opacity reset (:280-283, :328-478; SURVEY.md section 8 row f4).
 
 Same attribute and method names, argument meaning and param-group layout as the reference, so that the body of
-/root/reference/train.py:140-211 runs on it verbatim (tests/test_reference_loop.py, bench.py `dropin_*`).  The
-GPU box has no /root/reference, hence a mirror rather than an import; tests/test_reference_shims_cpu.py runs the
-REAL reference modules against the same interfaces on the CPU where the reference tree exists.
+train.py:140-211 runs on it verbatim (tests/test_reference_loop.py, bench.py `dropin_*`).  The
+reference tree is not a dependency, hence a mirror rather than an import; tests/test_reference_shims_cpu.py checks
+the mirror on the CPU against what the REAL reference modules computed (tests/golden/ref_loop.npz).
 """
 from __future__ import annotations
 
@@ -29,7 +29,7 @@ def inverse_sigmoid(x):
 
 
 def optimization_defaults(**over):
-    """/root/reference/arguments/__init__.py:73-94 (OptimizationParams defaults; InstantSplat's scripts pass
+    """arguments/__init__.py:73-94 (OptimizationParams defaults; InstantSplat's scripts pass
     --iterations 1000 --pp_optimizer --optim_pose)."""
     d = dict(iterations=30_000, position_lr_init=0.00016, position_lr_final=0.0000016, position_lr_delay_mult=0.01,
              position_lr_max_steps=30_000, feature_lr=0.0025, opacity_lr=0.05, scaling_lr=0.005, rotation_lr=0.001,
@@ -292,7 +292,7 @@ class GaussianModel:
 
 def w2c_to_pose(RT: torch.Tensor) -> torch.Tensor:
     """4x4 world-to-camera -> (qw,qx,qy,qz,tx,ty,tz); rotation -> quaternion by the trace method
-    (/root/reference/utils/pose_utils.py:183-240 get_tensor_from_camera / rotation2quad)."""
+    (utils/pose_utils.py:183-240 get_tensor_from_camera / rotation2quad)."""
     R, t = RT[:3, :3].double(), RT[:3, 3]
     tr = float(R[0, 0] + R[1, 1] + R[2, 2])
     if tr > 0:
@@ -324,7 +324,7 @@ class SimpleGaussianModel(GaussianModel):
 
 
 class PipelineDefaults:
-    """/root/reference/arguments/__init__.py:66-71"""
+    """arguments/__init__.py:66-71"""
     convert_SHs_python = False
     compute_cov3D_python = False
     debug = False

@@ -1,8 +1,8 @@
 """Drop-in for `scene.per_point_adam.PerPointAdam` (boundary B4):
-/root/reference/scene/per_point_adam.py:17-98.  Same constructor, param-group keys
+scene/per_point_adam.py:17-98.  Same constructor, param-group keys
 (`params, lr, betas, eps, weight_decay, per_point_lr, name`), state layout
 (`state[p] = {step, exp_avg, exp_avg_sq}`) and error behaviour, but `step()` is ONE launch of the
-fused sm_100a kernel (gs_adam.cu) over every tensor, with no host synchronisation."""
+fused sm_90a kernel (gs_adam.cu) over every tensor, with no host synchronisation."""
 from __future__ import annotations
 
 import ctypes
@@ -48,7 +48,7 @@ def _launch_adam_on_device(L, entries, flags, skip_ptr, step_sizes_dev):
 
 def _validated_multiplier(param: torch.Tensor, mult):
     """Type / device / shape checks of the optional per-row learning-rate multiplier; same exception types and
-    conditions as the reference optimizer (/root/reference/scene/per_point_adam.py:85-92)."""
+    conditions as the reference optimizer (scene/per_point_adam.py:85-92)."""
     if mult is None:
         return None, 1
     if not isinstance(mult, torch.Tensor):
@@ -88,7 +88,7 @@ class PerPointAdam(Optimizer):
                 if g.is_sparse:
                     raise RuntimeError("PerPointAdam does not support sparse gradients")
                 if not p.is_cuda:
-                    raise _lib.GsbError("PerPointAdam (B200) needs CUDA parameters; there is no CPU path")
+                    raise _lib.GsbError("PerPointAdam needs CUDA parameters; there is no CPU path")
                 st = self.state[p]
                 if not st:                                   # lazy state, same keys as the reference
                     st["step"] = 0
@@ -100,7 +100,7 @@ class PerPointAdam(Optimizer):
                 step_size = group["lr"] * ((1 - b2 ** t) ** 0.5 / (1 - b1 ** t))
                 mult, row_len = _validated_multiplier(p, group.get("per_point_lr"))
                 if not (p.is_contiguous() and g.is_contiguous() and p.dtype == torch.float32):
-                    raise _lib.GsbError("PerPointAdam (B200) needs contiguous fp32 parameters and gradients")
+                    raise _lib.GsbError("PerPointAdam needs contiguous fp32 parameters and gradients")
                 work.append(dict(param=p, grad=g, exp_avg=st["exp_avg"], exp_avg_sq=st["exp_avg_sq"], per_point_lr=mult,
                                  step_size=step_size, beta1=b1, beta2=b2, eps=group["eps"],
                                  weight_decay=group["weight_decay"], row_len=row_len))

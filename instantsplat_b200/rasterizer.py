@@ -1,7 +1,7 @@
 """Drop-in for the `diff_gaussian_rasterization` package (boundary B2 of SURVEY.md section 8b) on top
 of libgsb200.so, plus the fused InstantSplat entry (`rasterize_fused`) used by `render()`.
 
-Mirrors the interface the reference calls at /root/reference/gaussian_renderer/__init__.py:14-17,
+Mirrors the interface the reference calls at gaussian_renderer/__init__.py:14-17,
 60-78,126-135 (and the vanilla-3DGS form at gaussian_renderer/__init__3dgs.py:36-51,85-93):
 same names, argument meaning and error behaviour.
 """
@@ -210,7 +210,7 @@ def _forward(settings, means3D, scales, rotations, opacities, sh_dc, sh_rest, sh
 def _backward(st: _State, dL_dout, want, dev):
     """want: None (everything) or a set of names to compute; gradients that are not wanted are neither
     allocated nor written by the kernels (e.g. the pose-only test-view optimisation of
-    /root/reference/render.py:99-170 passes {"pose"}).  Returns dict of dense grad tensors."""
+    render.py:99-170 passes {"pose"}).  Returns dict of dense grad tensors."""
     L = _lib.lib()
     P, M = st.P, st.M
     _verify(st, dev)
@@ -314,7 +314,7 @@ def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales,
 
 class _RasterizeFused(torch.autograd.Function):
     """InstantSplat path with everything fused: raw model tensors + camera pose in, image out.
-    Replaces /root/reference/gaussian_renderer/__init__.py:81-135 and its autograd chain."""
+    Replaces gaussian_renderer/__init__.py:81-135 and its autograd chain."""
 
     @staticmethod
     def forward(ctx, xyz, rotation, scaling, opacity, f_dc, f_rest, pose, means2D, raster_settings):

@@ -1,4 +1,4 @@
-"""Drop-in for `gaussian_renderer.render` (boundary B1): /root/reference/gaussian_renderer/__init__.py:23-144.
+"""Drop-in for `gaussian_renderer.render` (boundary B1): gaussian_renderer/__init__.py:23-144.
 
 Same signature and result dict.  With the default pipeline flags (no compute_cov3D_python /
 convert_SHs_python / override_color) the whole body -- pose pre-transform (:81-89), activations,
@@ -14,7 +14,7 @@ from .rasterizer import GaussianRasterizationSettings, GaussianRasterizer, raste
 
 # FUSED = True : the whole body (pose pre-transform, activations, feature cat, rasterizer) is ONE call into the library.
 # FUSED = False: the reference's own body is restated op for op (PyTorch pose pre-transform -> GaussianRasterizer), i.e.
-#                what an UNCHANGED /root/reference/gaussian_renderer/__init__.py does on top of the rasterizer shim;
+#                what an UNCHANGED gaussian_renderer/__init__.py does on top of the rasterizer shim;
 #                bench.py times it as `dropin_unchanged`.  Env GSB_FUSED_RENDER=0 selects it process-wide.
 import os as _os
 
@@ -33,7 +33,7 @@ def _identity_consts(device):
 
 
 def get_camera_from_tensor(pose):
-    """/root/reference/utils/pose_utils.py:57-84 (used only by the non-fused branches)."""
+    """utils/pose_utils.py:57-84 (used only by the non-fused branches)."""
     q = pose[:4] / torch.sqrt((pose[:4] * pose[:4]).sum())
     r, x, y, z = q[0], q[1], q[2], q[3]
     R = torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y - r * z), 2 * (x * z + r * y),
@@ -45,7 +45,7 @@ def get_camera_from_tensor(pose):
 
 
 def quadmultiply(q1, q2):
-    """/root/reference/utils/pose_utils.py:86-104."""
+    """utils/pose_utils.py:86-104."""
     w1, x1, y1, z1 = q1.unbind(-1)
     w2, x2, y2, z2 = q2.unbind(-1)
     return torch.stack([w1 * w2 - x1 * x2 - y1 * y2 - z1 * z2, w1 * x2 + x1 * w2 + y1 * z2 - z1 * y2,

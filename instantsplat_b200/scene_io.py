@@ -4,14 +4,14 @@ What the reference's training stage reads and writes, so a scene produced here c
 `train.py` and its outputs can be loaded back:
 
 * `sparse_<n>/0/cameras.txt` (PINHOLE only) and `images.txt` (two lines per image), as parsed by
-  /root/reference/scene/colmap_loader.py:159-182,248-275 and written by
-  /root/reference/utils/sfm_utils.py:202-315;
-* `points3D.ply`: x,y,z f4 | nx,ny,nz f4 | red,green,blue u1 (/root/reference/scene/dataset_readers.py:315-369);
-* `confidence_dsp.npy` [P,1] (/root/reference/train.py:63-96);
+  scene/colmap_loader.py:159-182,248-275 and written by
+  utils/sfm_utils.py:202-315;
+* `points3D.ply`: x,y,z f4 | nx,ny,nz f4 | red,green,blue u1 (scene/dataset_readers.py:315-369);
+* `confidence_dsp.npy` [P,1] (train.py:63-96);
 * the trained model `point_cloud.ply`: x,y,z,nx,ny,nz,f_dc_0..2,f_rest_0..44,opacity,scale_0..2,rot_0..3, all f4,
-  SH stored channel-major (/root/reference/scene/gaussian_model.py:247-278);
+  SH stored channel-major (scene/gaussian_model.py:247-278);
 * `pose_optimized.npy` [n,4,4] world-to-camera matrices ordered by COLMAP image id
-  (/root/reference/train.py:46-60).
+  (train.py:46-60).
 
 PLY files are written/read directly (binary little endian) -- `plyfile` is not a dependency.
 """
@@ -35,7 +35,7 @@ def qvec2rotmat(q: np.ndarray) -> np.ndarray:
 
 def pose7_to_matrix(pose: np.ndarray) -> np.ndarray:
     """[qw,qx,qy,qz,tx,ty,tz] -> 4x4 world-to-camera; the quaternion is normalised first, like
-    get_camera_from_tensor (/root/reference/utils/pose_utils.py:57-84)."""
+    get_camera_from_tensor (utils/pose_utils.py:57-84)."""
     q = np.asarray(pose[:4], dtype=np.float64)
     q = q / np.linalg.norm(q)
     M = np.eye(4)
@@ -158,7 +158,7 @@ def read_points3d_ply(path: str):
 
 
 def gaussian_ply_fields(n_rest: int = 45) -> List[str]:
-    """construct_list_of_attributes (/root/reference/scene/gaussian_model.py:247-259)."""
+    """construct_list_of_attributes (scene/gaussian_model.py:247-259)."""
     return (["x", "y", "z", "nx", "ny", "nz"] + [f"f_dc_{i}" for i in range(3)] + [f"f_rest_{i}" for i in range(n_rest)]
             + ["opacity"] + [f"scale_{i}" for i in range(3)] + [f"rot_{i}" for i in range(4)])
 

@@ -3,19 +3,37 @@
 Everything is generated on the CPU with a seeded ``torch.Generator`` (seed = 1000 + config index)
 and moved to the device by the caller, so tests, the oracle and the CUDA path see identical inputs.
 
-Shapes follow the reference's parameter tensors (/root/reference/scene/gaussian_model.py:146-172):
+Shapes follow the reference's parameter tensors (scene/gaussian_model.py:146-172):
 ``xyz [P,3]``, ``f_dc [P,1,3]``, ``f_rest [P,15,3]``, ``opacity [P,1]`` (logit), ``scaling [P,3]``
 (log), ``rotation [P,4]`` (raw quaternion, real first), pose table ``poses [n_views,7]`` =
 [qw,qx,qy,qz,tx,ty,tz] of the world-to-camera transform
-(/root/reference/scene/gaussian_model.py:126-136).
+(scene/gaussian_model.py:126-136).
 """
 from __future__ import annotations
 
+import functools
 import math
 from dataclasses import dataclass, field
 from typing import Dict, List
 
 import torch
+
+
+def _single_threaded(fn):
+    """Run a generator on one CPU thread.  PyTorch splits large elementwise CPU ops into per-thread chunks, and a chunk's
+    vectorised body and its tail round sin / cos / log / randn differently, so a multi-threaded generator's output
+    depends on the core count.  Training amplifies such last-bit differences, so the same arguments would give different
+    results on machines with different core counts.  On one thread the output is the same on every CPU with AVX2 or
+    AVX-512."""
+    @functools.wraps(fn)
+    def run(*args, **kwargs):
+        n = torch.get_num_threads()
+        torch.set_num_threads(1)
+        try:
+            return fn(*args, **kwargs)
+        finally:
+            torch.set_num_threads(n)
+    return run
 
 
 @dataclass
@@ -49,6 +67,7 @@ def _rotmat_to_quat(R: torch.Tensor) -> torch.Tensor:
     return torch.tensor([w, x, y, z], dtype=torch.float32)
 
 
+@_single_threaded
 def random_scene(P: int = 10_000, width: int = 256, height: int = 256, seed: int = 1001,
                  sh_degree: int = 3, fovx_deg: float = 60.0) -> Scene:
     """cfg1: camera-frame random Gaussians, one perturbed-identity pose."""
@@ -69,13 +88,14 @@ def random_scene(P: int = 10_000, width: int = 256, height: int = 256, seed: int
                  sh_degree, name=f"random{P}")
 
 
+@_single_threaded
 def surface_scene(P: int, n_views: int, width: int, height: int, seed: int, sh_degree: int = 3,
                   fovx_deg: float = 60.0, opacity_mode: str = "mid", sh_rest_std: float = 0.05
                   ) -> Scene:
     """cfg2-5: what init_geo.py produces -- per view, a regular pixel grid of P/n_views points
     unprojected with a smooth random depth in [2,6]; cameras on a small arc looking at the scene.
     Scale = log(grid spacing in world units) (the kNN init rule of
-    /root/reference/scene/gaussian_model.py:156-160 for a regular grid); quat = (1,0,0,0);
+    scene/gaussian_model.py:156-160 for a regular grid); quat = (1,0,0,0);
     opacity 0.1 ("init") or logit ~ N(0,1.5^2) ("mid"); colours from a procedural texture.
     """
     g = torch.Generator().manual_seed(seed)
@@ -150,6 +170,7 @@ def make_config(idx: int, scale: float = 1.0) -> Scene:
     raise ValueError(idx)
 
 
+@_single_threaded
 def perturbed_copy(scene: Scene, seed: int = 7, sigma: float = 0.02) -> Dict[str, torch.Tensor]:
     """Parameters of a perturbed copy (used to render non-trivial ground-truth images)."""
     g = torch.Generator().manual_seed(seed)

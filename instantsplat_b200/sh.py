@@ -1,5 +1,5 @@
 """The reference's optional Python SH branch (pipe.convert_SHs_python,
-/root/reference/gaussian_renderer/__init__.py:108-119; polynomial /root/reference/utils/sh_utils.py:57-112).
+gaussian_renderer/__init__.py:108-119; polynomial utils/sh_utils.py:57-112).
 Not on the default path; kept so `render()` accepts the same pipe flags."""
 import torch
 

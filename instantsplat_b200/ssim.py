@@ -1,5 +1,5 @@
-"""Drop-in for `fused_ssim.fused_ssim` (boundary B3): /root/reference/train.py:39-43,172-173.
-Semantics = the reference's PyTorch fallback /root/reference/utils/loss_utils.py:55-85
+"""Drop-in for `fused_ssim.fused_ssim` (boundary B3): train.py:39-43,172-173.
+Semantics = the reference's PyTorch fallback utils/loss_utils.py:55-85
 (11x11 sigma-1.5 window, zero 'same' padding, C1=1e-4, C2=9e-4, mean over all elements).
 Also the fused L1+DSSIM training loss of train.py:171-176 (`fused_training_loss`)."""
 from __future__ import annotations

@@ -1,5 +1,5 @@
 """Pose-only "tracking" mode (SURVEY.md section 8 row f2): the test-view pose optimisation of
-/root/reference/render.py:99-170 as a device-resident loop.
+render.py:99-170 as a device-resident loop.
 
 Reference semantics, per test view:
   * Gaussians frozen (render.py:106-111); the 7 pose parameters start from the view's W2C (:115);

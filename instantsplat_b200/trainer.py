@@ -1,4 +1,4 @@
-"""The joint pose + Gaussian optimisation inner loop of /root/reference/train.py:124-211, B200-first.
+"""The joint pose + Gaussian optimisation inner loop of train.py:124-211, H100-first.
 
 One `JointTrainer.step(view)` = update_learning_rate -> render (fused pose transform + rasterizer)
 -> L1 + DSSIM loss -> backward -> (multi-GPU: NCCL sum of the flat per-Gaussian gradient buffer)
@@ -34,7 +34,7 @@ SEGMENTS = (("xyz", 3), ("f_dc", 3), ("f_rest", 45), ("opacity", 1), ("scaling",
 
 
 def get_expon_lr_func(lr_init, lr_final, lr_delay_steps=0, lr_delay_mult=1.0, max_steps=1000000):
-    """/root/reference/utils/general_utils.py:29-62 (host-side, fp64 numpy, unchanged semantics)."""
+    """utils/general_utils.py:29-62 (host-side, fp64 numpy, unchanged semantics)."""
 
     def helper(step):
         if step < 0 or (lr_init == 0.0 and lr_final == 0.0):
@@ -51,7 +51,7 @@ def get_expon_lr_func(lr_init, lr_final, lr_delay_steps=0, lr_delay_mult=1.0, ma
 
 
 class OptimConfig:
-    """/root/reference/arguments/__init__.py:73-94 defaults."""
+    """arguments/__init__.py:73-94 defaults."""
     iterations = 30_000
     position_lr_init = 0.00016
     position_lr_final = 0.0000016
@@ -347,7 +347,7 @@ class JointTrainer:
 
     def optimizer_step(self, grad_scale: Optional[float] = None, _advance: bool = True, _dev_steps: bool = False) -> None:
         """PerPointAdam.step over the 6 Gaussian tensors + the pose table in one launch
-        (param groups and LRs of /root/reference/scene/gaussian_model.py:203-243)."""
+        (param groups and LRs of scene/gaussian_model.py:203-243)."""
         c = self.cfg
         if _advance:
             self.opt_step += 1
@@ -553,7 +553,7 @@ class JointTrainer:
             assert self._settle()
 
     # ---- densify / prune / opacity reset on the flat buffers (SURVEY.md section 8 row f4) -----------------------
-    # Semantics of /root/reference/scene/gaussian_model.py: prune_points (:359-374) keeps the surviving rows of every
+    # Semantics of scene/gaussian_model.py: prune_points (:359-374) keeps the surviving rows of every
     # parameter AND of both Adam moments; densification_postfix (:399-418) appends rows with zero moments;
     # reset_opacity (:280-283) clamps the opacity to 0.01 (in logit space) and zeroes that tensor's moments.  The
     # optimizer's step counter is untouched by all three, as in the reference (state["step"] survives the surgery).

@@ -6,25 +6,25 @@ fails loudly when the CUDA library is missing.
 
 What it restates (pure PyTorch, CPU, differentiable through autograd, fp32 or fp64):
 
-* pose pre-transform              /root/reference/gaussian_renderer/__init__.py:81-92,
-                                  /root/reference/utils/pose_utils.py:10-55,57-84,86-104
-* projection matrix               /root/reference/utils/graphics_utils.py:71-91
-* SH -> RGB                       /root/reference/utils/sh_utils.py:57-112 (+0.5 / clamp:
-                                  /root/reference/gaussian_renderer/__init__.py:119)
+* pose pre-transform              gaussian_renderer/__init__.py:81-92,
+                                  utils/pose_utils.py:10-55,57-84,86-104
+* projection matrix               utils/graphics_utils.py:71-91
+* SH -> RGB                       utils/sh_utils.py:57-112 (+0.5 / clamp:
+                                  gaussian_renderer/__init__.py:119)
 * EWA projection, tile rect, (tile, depth) order, front-to-back blend and the analytic
   backward's deviations from naive autograd: SURVEY.md Appendix A.  The arithmetic lives in
   graphdeco-inria/diff-gaussian-rasterization @ 59f5f77e3ddbac3ed9db93ec2cfe99ed6c5d121d,
-  which is an EMPTY submodule in /root/reference, so this part is a restatement of the
+  which is an EMPTY submodule in the reference checkout, so this part is a restatement of the
   published algorithm anchored on the reference's call site
-  (/root/reference/gaussian_renderer/__init__.py:60-78,126-135).
-* L1 / SSIM loss                  /root/reference/utils/loss_utils.py:39-40,45-85 ;
-                                  combine /root/reference/train.py:176
-* per-point Adam                  /root/reference/scene/per_point_adam.py:34-98
+  (gaussian_renderer/__init__.py:60-78,126-135).
+* L1 / SSIM loss                  utils/loss_utils.py:39-40,45-85 ;
+                                  combine train.py:176
+* per-point Adam                  scene/per_point_adam.py:34-98
 
 PARITY PINNING STATUS
   pinned   : eval_sh, ssim, l1_loss, get_camera_from_tensor, quadmultiply, getProjectionMatrix,
              PerPointAdam -- checked against the reference's own Python modules imported from
-             /root/reference (oracle/make_golden.py; vectors in tests/golden/).
+             an InstantSplat checkout (oracle/make_golden.py; vectors in tests/golden/).
   unpinned : the rasterizer proper (EWA / binning / blend / backward).  The reference holds no
              source, tests or golden vectors for it ("parity unpinned" -- see DESIGN.md); it is
              cross-checked only by fp64 finite differences and internal consistency.
@@ -42,7 +42,7 @@ BLOCK = 16
 ALPHA_MIN = 1.0 / 255.0
 T_EPS = 1e-4
 
-# /root/reference/utils/sh_utils.py:24-52
+# utils/sh_utils.py:24-52
 SH_C0 = 0.28209479177387814
 SH_C1 = 0.4886025119029199
 SH_C2 = (1.0925484305920792, -1.0925484305920792, 0.31539156525252005,
@@ -55,7 +55,7 @@ SH_C3 = (-0.5900435899266435, 2.890611442640554, -0.4570457994644658, 0.37317633
 # camera / pose helpers
 # ----------------------------------------------------------------------------------------------
 def projection_matrix(znear: float, zfar: float, fovx: float, fovy: float, dtype=torch.float32):
-    """/root/reference/utils/graphics_utils.py:71-91 (returned NOT transposed)."""
+    """utils/graphics_utils.py:71-91 (returned NOT transposed)."""
     ty = math.tan(fovy / 2)
     tx = math.tan(fovx / 2)
     top, right = ty * znear, tx * znear
@@ -73,10 +73,10 @@ def projection_matrix(znear: float, zfar: float, fovx: float, fovy: float, dtype
 
 @dataclass
 class Camera:
-    """Rasterizer settings, /root/reference/gaussian_renderer/__init__.py:60-76.
+    """Rasterizer settings, gaussian_renderer/__init__.py:60-76.
 
     ``viewmatrix`` / ``projmatrix`` are stored TRANSPOSED (row-vector convention,
-    /root/reference/scene/cameras.py:54-56): p_view = [p,1] @ viewmatrix.
+    scene/cameras.py:54-56): p_view = [p,1] @ viewmatrix.
     """
     width: int
     height: int
@@ -93,7 +93,7 @@ class Camera:
     def instantsplat(width, height, fovx, fovy, bg=None, sh_degree=3, dtype=torch.float32,
                      znear=0.01, zfar=100.0):
         """Identity view, projmatrix = I @ P^T, campos = 0
-        (/root/reference/gaussian_renderer/__init__.py:55-59)."""
+        (gaussian_renderer/__init__.py:55-59)."""
         Pm = projection_matrix(znear, zfar, fovx, fovy, dtype).t().contiguous()
         if bg is None:
             bg = torch.zeros(3, dtype=dtype)
@@ -109,7 +109,7 @@ class Camera:
 
 
 def quad2rotation(q: torch.Tensor) -> torch.Tensor:
-    """/root/reference/utils/pose_utils.py:34-55 -- normalises q.  q: [4] -> [3,3]."""
+    """utils/pose_utils.py:34-55 -- normalises q.  q: [4] -> [3,3]."""
     q = q / torch.sqrt((q * q).sum())
     r, x, y, z = q[0], q[1], q[2], q[3]
     return torch.stack([
@@ -119,7 +119,7 @@ def quad2rotation(q: torch.Tensor) -> torch.Tensor:
 
 
 def pose_to_w2c(pose: torch.Tensor) -> torch.Tensor:
-    """/root/reference/utils/pose_utils.py:57-84.  pose = [qw,qx,qy,qz,tx,ty,tz] -> 4x4."""
+    """utils/pose_utils.py:57-84.  pose = [qw,qx,qy,qz,tx,ty,tz] -> 4x4."""
     R = quad2rotation(pose[:4])
     top = torch.cat([R, pose[4:7].reshape(3, 1)], dim=1)
     bottom = torch.tensor([[0.0, 0.0, 0.0, 1.0]], dtype=pose.dtype, device=pose.device)
@@ -127,7 +127,7 @@ def pose_to_w2c(pose: torch.Tensor) -> torch.Tensor:
 
 
 def quadmultiply(q1: torch.Tensor, q2: torch.Tensor) -> torch.Tensor:
-    """/root/reference/utils/pose_utils.py:86-104 (Hamilton product, real first, no normalise)."""
+    """utils/pose_utils.py:86-104 (Hamilton product, real first, no normalise)."""
     w1, x1, y1, z1 = q1.unbind(-1)
     w2, x2, y2, z2 = q2.unbind(-1)
     return torch.stack([
@@ -138,7 +138,7 @@ def quadmultiply(q1: torch.Tensor, q2: torch.Tensor) -> torch.Tensor:
 
 
 def pose_pretransform(xyz: torch.Tensor, rot: torch.Tensor, pose: torch.Tensor):
-    """/root/reference/gaussian_renderer/__init__.py:81-89."""
+    """gaussian_renderer/__init__.py:81-89."""
     w2c = pose_to_w2c(pose)
     homo = torch.cat([xyz, torch.ones(xyz.shape[0], 1, dtype=xyz.dtype, device=xyz.device)], dim=1)
     means = (w2c @ homo.t()).t()[:, :3]
@@ -151,7 +151,7 @@ def pose_pretransform(xyz: torch.Tensor, rot: torch.Tensor, pose: torch.Tensor):
 # ----------------------------------------------------------------------------------------------
 def eval_sh(deg: int, sh: torch.Tensor, dirs: torch.Tensor) -> torch.Tensor:
     """sh: [P, M, 3] (coefficient-major, the rasterizer's layout), dirs [P,3] unit -> [P,3].
-    Polynomial of /root/reference/utils/sh_utils.py:57-112."""
+    Polynomial of utils/sh_utils.py:57-112."""
     res = SH_C0 * sh[:, 0]
     if deg > 0:
         x, y, z = dirs[:, 0:1], dirs[:, 1:2], dirs[:, 2:3]
@@ -416,8 +416,8 @@ def rasterize(means3D, scales, rotations, opacities, shs, cam: Camera, means2D=N
 def render_instantsplat(xyz, rotation, scaling, opacity, f_dc, f_rest, pose, cam: Camera,
                         means2D=None, tiles=None, return_aux=False, **blend_kw):
     """The ``render()`` boundary (B1) on RAW parameters
-    (/root/reference/gaussian_renderer/__init__.py:23-144 with the default pipe flags;
-    activations /root/reference/scene/gaussian_model.py:101-121)."""
+    (gaussian_renderer/__init__.py:23-144 with the default pipe flags;
+    activations scene/gaussian_model.py:101-121)."""
     means, rots = pose_pretransform(xyz, rotation, pose)
     shs = torch.cat([f_dc, f_rest], dim=1)
     return rasterize(means, torch.exp(scaling), rots, torch.sigmoid(opacity), shs, cam,
@@ -428,19 +428,19 @@ def render_instantsplat(xyz, rotation, scaling, opacity, f_dc, f_rest, pose, cam
 # loss  (A.4)
 # ----------------------------------------------------------------------------------------------
 def l1_loss(a, b):
-    """/root/reference/utils/loss_utils.py:39-40."""
+    """utils/loss_utils.py:39-40."""
     return (a - b).abs().mean()
 
 
 def gaussian_window(window_size=11, sigma=1.5, dtype=torch.float32):
-    """/root/reference/utils/loss_utils.py:45-47 (built in fp32 like the reference)."""
+    """utils/loss_utils.py:45-47 (built in fp32 like the reference)."""
     g = torch.tensor([math.exp(-(x - window_size // 2) ** 2 / float(2 * sigma ** 2))
                       for x in range(window_size)], dtype=torch.float32)
     return (g / g.sum()).to(dtype)
 
 
 def ssim_map(img1, img2, window_size=11):
-    """/root/reference/utils/loss_utils.py:65-85; img [C,H,W] or [B,C,H,W]; zero 'same' padding."""
+    """utils/loss_utils.py:65-85; img [C,H,W] or [B,C,H,W]; zero 'same' padding."""
     squeeze = img1.dim() == 3
     if squeeze:
         img1, img2 = img1[None], img2[None]
@@ -464,12 +464,12 @@ def ssim(img1, img2):
 
 
 def training_loss(image, gt, lambda_dssim=0.2):
-    """/root/reference/train.py:171-176."""
+    """train.py:171-176."""
     return (1.0 - lambda_dssim) * l1_loss(image, gt) + lambda_dssim * (1.0 - ssim(image, gt))
 
 
 # ----------------------------------------------------------------------------------------------
-# per-point Adam  (/root/reference/scene/per_point_adam.py:34-98)
+# per-point Adam  (scene/per_point_adam.py:34-98)
 # ----------------------------------------------------------------------------------------------
 def per_point_adam_step(p, grad, exp_avg, exp_avg_sq, step, lr, beta1=0.9, beta2=0.999,
                         eps=1e-15, weight_decay=0.0, per_point_lr=None):

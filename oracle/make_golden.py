@@ -1,18 +1,17 @@
 """Generate tests/golden/*.npz by importing the REFERENCE's own Python modules.
 
-Runs only in the authoring container (needs /root/reference, which does not exist on the GPU
-box).  The vectors it writes are committed; tests/test_oracle_golden.py checks the oracle
+Needs an InstantSplat checkout.  The vectors it writes are committed; tests/test_oracle_golden.py checks the oracle
 (oracle/gs_oracle.py) against them on CPU, and the `-m gpu` tests check the CUDA kernels
 against the same vectors.
 
-    python oracle/make_golden.py
+    python oracle/make_golden.py <path to the InstantSplat checkout>
 
 Reference modules used (imported by file path because `scene/__init__.py` pulls in plyfile):
-    /root/reference/utils/sh_utils.py        eval_sh
-    /root/reference/utils/loss_utils.py      ssim, l1_loss
-    /root/reference/utils/pose_utils.py      get_camera_from_tensor, quadmultiply
-    /root/reference/utils/graphics_utils.py  getProjectionMatrix
-    /root/reference/scene/per_point_adam.py  PerPointAdam
+    utils/sh_utils.py        eval_sh
+    utils/loss_utils.py      ssim, l1_loss
+    utils/pose_utils.py      get_camera_from_tensor, quadmultiply
+    utils/graphics_utils.py  getProjectionMatrix
+    scene/per_point_adam.py  PerPointAdam
 The rasterizer itself (diff-gaussian-rasterization) is an empty submodule: no vectors can be
 generated for it from the reference ("parity unpinned"); `raster_tiny.npz` holds the ORACLE's
 own fp64 outputs as a regression pin and is labelled as such.
@@ -24,7 +23,7 @@ import sys
 import numpy as np
 import torch
 
-REF = "/root/reference"
+REF = None                                       # the InstantSplat checkout (command line)
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 OUT = os.path.join(ROOT, "tests", "golden")
@@ -75,7 +74,7 @@ def main():
     q2 = torch.randn(32, 4, generator=g)
     qm = pose_utils.quadmultiply(poses[0, :4], q2)
     xyz = torch.randn(32, 3, generator=g)
-    # the 4 lines of /root/reference/gaussian_renderer/__init__.py:83-88 driven by the
+    # the 4 lines of gaussian_renderer/__init__.py:83-88 driven by the
     # reference's own get_camera_from_tensor
     homo = torch.cat((xyz, torch.ones(32, 1)), dim=1)
     trans = (w2c[0] @ homo.T).T[:, :3]
@@ -138,7 +137,7 @@ def main():
         rec["g_" + k] = P64[k].grad.numpy()
     np.savez_compressed(os.path.join(OUT, "raster_tiny.npz"), **rec)
     # ---- scene file formats (row f3): files written by instantsplat_b200.scene_io, parsed by the REFERENCE's
-    # own COLMAP text readers (/root/reference/scene/colmap_loader.py:159-182,248-275)
+    # own COLMAP text readers (scene/colmap_loader.py:159-182,248-275)
     import tempfile
     from instantsplat_b200 import scene_io
     from instantsplat_b200.scenes import surface_scene
@@ -159,4 +158,7 @@ def main():
 
 
 if __name__ == "__main__":
+    if len(sys.argv) != 2:
+        sys.exit(__doc__)
+    REF = sys.argv[1]
     main()

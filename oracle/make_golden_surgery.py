@@ -3,11 +3,11 @@ optimizer-state surgery behind densify / prune / opacity reset (SURVEY.md sectio
 `prune_points` (:359-374), `densification_postfix` (:399-418), `reset_opacity` (:280-283) -- interleaved with
 `update_learning_rate` + `PerPointAdam.step` on seeded gradients.
 
-Runs only where /root/reference exists (CPU; `.cuda()` / device="cuda" are neutralised, the native packages are the
+Needs an InstantSplat checkout (CPU; `.cuda()` / device="cuda" are neutralised, the native packages are the
 oracle-backed stand-ins of tests/cpu_standins).  The GPU tests replay the same script on `JointTrainer` and on the
 mirror `instantsplat_b200.model.GaussianModel` and must land on these vectors.
 
-    python oracle/make_golden_surgery.py
+    python oracle/make_golden_surgery.py <path to the InstantSplat checkout>
 """
 import importlib.abc
 import importlib.util
@@ -16,7 +16,9 @@ import sys
 import types
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+if len(sys.argv) != 2:
+    sys.exit(__doc__)
+REF = sys.argv[1]
 for p in (os.path.join(ROOT, "tests", "cpu_standins"), os.path.join(ROOT, "tests", "stubs"), ROOT):
     sys.path.insert(0, p)
 sys.path.append(REF)

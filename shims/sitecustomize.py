@@ -1,5 +1,5 @@
 """Picked up automatically by Python when <repo>/shims is on PYTHONPATH: installs the import hook that swaps the
-reference's in-package pieces (`scene.per_point_adam`, `gaussian_renderer.render`) for the B200 ones without editing
+reference's in-package pieces (`scene.per_point_adam`, `gaussian_renderer.render`) for the fused ones without editing
 the reference (instantsplat_b200/hooks.py).  The hook module is loaded by file path so that start-up does not import
 torch; the heavy imports happen only when the reference actually imports the hooked modules."""
 import importlib.util

@@ -11,8 +11,7 @@ Protocol (BASELINE.json north_star: render <= 1e-4 max abs per pixel, gradients 
    pixels in BOTH arms, so a legitimate flip cannot leak into the comparison; the tolerance stays 1e-3 for every
    tensor (no relaxation when a pixel flips).  When the weights are the real training-loss gradient dL/dimage
    (L1 + D-SSIM), the CUDA loss kernels' dL/dimage is compared with the oracle's as well.
-3. Every case appends its numbers to a report that conftest.py writes to gpurun_out/parity_r02.json at the end
-   of the session (committed under profiles/ after a GPU run).
+3. Every case appends its numbers to a report that conftest.py writes at the end of the session.
 """
 import math
 
@@ -45,7 +44,7 @@ def settings_for(sc, deg, bg, debug=False):
 
 def flip_budget(npix):
     """How many compared pixels may exceed 1e-4 (all of them oracle-flagged): 1 in 20 000, at least 2.
-    Measured rates are recorded in profiles/parity_r02.json."""
+    Measured rates are recorded in the session's parity report."""
     return max(2, int(5e-5 * npix))
 
 

@@ -1,4 +1,4 @@
-"""CPU stand-in for `fused_ssim` (tests only): the oracle's restatement of /root/reference/utils/loss_utils.py:55-85."""
+"""CPU stand-in for `fused_ssim` (tests only): the oracle's restatement of utils/loss_utils.py:55-85."""
 from oracle import gs_oracle as O
 
 

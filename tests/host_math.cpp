@@ -1,5 +1,5 @@
 // CPU harness around instantsplat_b200/csrc/gs_math.cuh: runs the SAME per-Gaussian forward /
-// backward arithmetic the sm_100a kernels inline, on the host, so the algebra can be checked
+// backward arithmetic the sm_90a kernels inline, on the host, so the algebra can be checked
 // against the oracle without a GPU (tests/test_host_math.py).  Test utility only -- it is not
 // part of the product library and is never loaded by instantsplat_b200.
 #include <cstring>

@@ -1,5 +1,5 @@
 """Test-only stand-in for the `plyfile` PyPI package (not installed in this image): lets
-/root/reference/scene/gaussian_model.py be IMPORTED by tests/test_reference_shims_cpu.py.  Nothing on the tested path
+scene/gaussian_model.py be IMPORTED by tests/test_reference_shims_cpu.py.  Nothing on the tested path
 reads or writes PLY files through it."""
 
 

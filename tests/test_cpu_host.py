@@ -179,3 +179,22 @@ def test_debug_mode_writes_snapshot_of_failing_call(tmp_path, monkeypatch):
                                  colors_precomp=torch.ones(5, 3), scales=torch.ones(5, 3), rotations=torch.ones(5, 4))
     dump = torch.load(tmp_path / "snapshot_fw.dump", weights_only=False)
     assert tuple(dump[0].shape) == (5, 4) and dump[-1][0] == 32
+
+
+def test_scene_generation_does_not_depend_on_the_thread_count():
+    """The synthetic scenes are the benchmark's and the tests' inputs: they must be bit-identical whatever the core
+    count (large elementwise CPU ops are split into per-thread chunks that round transcendental functions differently)."""
+    from instantsplat_b200.scenes import perturbed_copy, surface_scene
+    n = torch.get_num_threads()
+    out = []
+    try:
+        for threads in (1, 4, 7):
+            torch.set_num_threads(threads)
+            sc = surface_scene(300_000, 3, 320, 180, seed=11, sh_degree=3)
+            out.append([sc.poses, sc.per_point_lr] + [sc.params[k] for k in sorted(sc.params)] +
+                       [v for _, v in sorted(perturbed_copy(sc, sigma=0.05).items())])
+    finally:
+        torch.set_num_threads(n)
+    assert torch.get_num_threads() == n
+    for a, b, c in zip(*out):
+        assert torch.equal(a, b) and torch.equal(a, c)

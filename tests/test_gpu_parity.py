@@ -70,7 +70,7 @@ def masked_weights(shape, amb, seed):
 def test_library_loads_and_reports_device():
     import instantsplat_b200 as I
     assert I.lib().gsb_abi_version() == 2
-    assert torch.cuda.get_device_capability()[0] >= 10, "these kernels are built for sm_100a only"
+    assert torch.cuda.get_device_capability() == (9, 0), "these kernels are built for sm_90a only"
 
 
 @pytest.mark.parametrize("deg", [0, 3])
@@ -267,7 +267,7 @@ def test_sync_free_capacity_overflow_is_repaired():
 
 
 def test_blend_kernel_versions_agree():
-    """v1 (one pixel per lane) and v2 (two pixels, packed f32x2) blend kernels, with and without TMA bulk
+    """v1 (one pixel per lane) and v2 (two pixels per lane) blend kernels, with and without TMA bulk
     staging, on a scene whose image size is not a multiple of the tile size."""
     import instantsplat_b200 as I
     L = I.lib()
@@ -496,7 +496,7 @@ def test_per_point_adam_large_unaligned():
 
 # ----------------------------------------------------------------------------------------------
 class _FakeGaussians:
-    """The attributes render() reads from GaussianModel (/root/reference/scene/gaussian_model.py:101-136)."""
+    """The attributes render() reads from GaussianModel (scene/gaussian_model.py:101-136)."""
 
     def __init__(self, sc, deg):
         p = {k: torch.nn.Parameter(v.to(DEV).clone()) for k, v in sc.params.items()}
@@ -658,7 +658,7 @@ def test_knn_distcuda2_matches_bruteforce():
 
 def test_per_point_adam_state_surgery_prune_and_cat():
     """Row f4: the reference's densify/prune code edits `optimizer.state[p]` and `param_groups[i]["params"]` in place
-    (/root/reference/scene/gaussian_model.py:328-398: _prune_optimizer, cat_tensors_to_optimizer).  The drop-in keeps the
+    (scene/gaussian_model.py:328-398: _prune_optimizer, cat_tensors_to_optimizer).  The drop-in keeps the
     same state layout, so the same surgery works and later steps match the oracle on the resized tensors."""
     import instantsplat_b200 as I
     g = torch.Generator().manual_seed(5)
@@ -735,3 +735,22 @@ def test_dgr_C_surface_matches_module_path():
         assert rel_err(a, b) < 1e-4
     vis = dgr._C.mark_visible(means.detach(), rs.viewmatrix, rs.projmatrix)
     assert torch.equal(vis, means.detach()[:, 2] > 0.2)
+
+
+def test_training_steps_are_bit_reproducible():
+    """Two trainers running the same steps on the same inputs end bit-identical: the blend backward adds its
+    per-Gaussian sums in fixed point, so their value does not depend on the order in which CTAs arrive (with float
+    atomics it did, and Adam amplified the difference over a run)."""
+    import instantsplat_b200 as I
+    sc = surface_scene(30_000, 3, 320, 192, seed=19, sh_degree=3)
+    gts = torch.rand(3, 3, sc.height, sc.width, generator=torch.Generator().manual_seed(6)).to(DEV)
+    out = []
+    for _ in range(2):
+        tr = I.JointTrainer(sc, DEV, gt_images=gts)
+        for s in range(12):
+            tr.step(s % 3)
+        torch.cuda.synchronize()
+        out.append((tr.params.clone(), tr.poses.clone(), tr.color.clone(), tr.loss_value().clone()))
+        del tr
+    for a, b in zip(*out):
+        assert torch.equal(a, b)

@@ -1,5 +1,5 @@
-"""GPU side of "the reference's loop on the drop-ins" (-m gpu).  The GPU box has no /root/reference, so the loop body
-of /root/reference/train.py:140-211 is transcribed here and driven through the repo's mirror of the reference's
+"""GPU side of "the reference's loop on the drop-ins" (-m gpu).  The reference tree is not a dependency, so the loop body
+of train.py:140-211 is transcribed here and driven through the repo's mirror of the reference's
 `GaussianModel` (instantsplat_b200/model.py; tests/test_reference_shims_cpu.py shows on the CPU, with the REAL reference
 modules, that mirror == reference).  Three ways of running the same 20 iterations must give the same losses:
 

@@ -1,5 +1,5 @@
 """Pose-only tracking mode (-m gpu; SURVEY.md section 8 row f2): the device-resident loop of
-instantsplat_b200/tracking.py against a CPU restatement of /root/reference/render.py:113-161 built from the oracle's
+instantsplat_b200/tracking.py against a CPU restatement of render.py:113-161 built from the oracle's
 renderer and torch's own Adam + CosineAnnealingLR (the classes the reference instantiates)."""
 import math
 
