@@ -328,13 +328,15 @@ def build_tile_lists(proj):
 # ----------------------------------------------------------------------------------------------
 # blend  (A.2 step 10, A.3)
 # ----------------------------------------------------------------------------------------------
-def blend(proj, cam: Camera, tiles=None, return_aux=False, alpha_min=ALPHA_MIN, t_eps=T_EPS):
+def blend(proj, cam: Camera, tiles=None, return_aux=False, alpha_min=ALPHA_MIN, t_eps=T_EPS, lists=None):
     """Front-to-back alpha blend per 16x16 tile.  ``tiles``: optional iterable of tile ids to
-    render (others left at bg) -- used for bounded CPU timing samples."""
+    render (others left at bg) -- used for bounded CPU timing samples.  ``lists``: (gids, ranges) to blend
+    instead of ``build_tile_lists(proj)`` -- e.g. the fp32 lists under an fp64 blend, so that a rect bound or a
+    depth order within rounding does not differ from what an fp32 implementation bins."""
     dt = proj["xy"].dtype
     W, H = cam.width, cam.height
     gx, gy = proj["grid"]
-    gids, ranges = build_tile_lists(proj)
+    gids, ranges = build_tile_lists(proj) if lists is None else lists
     bg = cam.bg.to(dt)
     out = bg[:, None, None].expand(3, H, W).clone()
     final_T = torch.ones(H, W, dtype=dt)

@@ -11,7 +11,13 @@ Protocol (BASELINE.json north_star: render <= 1e-4 max abs per pixel, gradients 
    pixels in BOTH arms, so a legitimate flip cannot leak into the comparison; the tolerance stays 1e-3 for every
    tensor (no relaxation when a pixel flips).  When the weights are the real training-loss gradient dL/dimage
    (L1 + D-SSIM), the CUDA loss kernels' dL/dimage is compared with the oracle's as well.
-3. Every case appends its numbers to a report that conftest.py writes at the end of the session.
+3. Every gradient tensor is also compared row by row (one row per Gaussian, `row_err`): the whole-tensor metric
+   divides by the tensor's largest gradient, so it cannot see an error confined to Gaussians with small gradients
+   (deep in a list, behind low transmittance, seen through an edge tile).  The oracle computes the truth in fp64, so
+   the per-row metric does not measure the oracle's own fp32 rounding.
+4. Every forward's tile lists are checked exactly on all tiles (tests/_binning.py `check_lists`), not only on the
+   compared ones.
+5. Every case appends its numbers to a report that conftest.py writes at the end of the session.
 """
 import math
 
@@ -19,16 +25,40 @@ import torch
 
 from oracle import gs_oracle as O
 
+import _binning as BL
+
 DEV = "cuda"
 NAMES = ("xyz", "rotation", "scaling", "opacity", "f_dc", "f_rest")
 IMG_TOL = 1e-4
 GRAD_TOL = 1e-3
+ROW_TAU = 1e-3       # per-row metric: floor of the denominator, relative to the tensor's largest gradient
+# bounds on the 99.9th percentile of the per-row error where it is asserted, set from H100 measurements with a margin
+# (DESIGN.md section 2): random scenes on tile subsets, and the constructed one-tile scenes of test_binning_lists.py
+ROW_TOL = 2e-3
+ROW_TOL_SCENES = 1e-4
 REPORT = []          # list of dicts, one per parity case
 
 
 def rel_err(a, b):
     a, b = a.detach().cpu().double().reshape(-1), b.detach().cpu().double().reshape(-1)
     return float((a - b).abs().max() / (b.abs().max() + 1e-20))
+
+
+def row_err(a, b, tau=ROW_TAU):
+    """Per-Gaussian error of a gradient tensor (rows = first dimension): e_i = max|a_i - b_i| / (max|b_i| +
+    tau * max|b|), over the rows where either arm is non-zero.  -> dict(rows, p50, p99, p999, max); the
+    percentiles take the next higher sample, so an error shared by >= 0.1 % of the rows shows in p999."""
+    import numpy as np
+    a, b = a.detach().cpu().double(), b.detach().cpu().double()
+    a, b = a.reshape(a.shape[0], -1), b.reshape(b.shape[0], -1)
+    d = (a - b).abs().amax(1)
+    m = b.abs().amax(1)
+    live = (m > 0) | (a.abs().amax(1) > 0)
+    e = (d / (m + tau * b.abs().max() + 1e-300))[live].numpy()
+    if e.size == 0:
+        return dict(rows=0, p50=0.0, p99=0.0, p999=0.0, max=0.0)
+    q = np.quantile(e, [0.5, 0.99, 0.999], method="higher")
+    return dict(rows=int(e.size), p50=float(q[0]), p99=float(q[1]), p999=float(q[2]), max=float(e.max()))
 
 
 def settings_for(sc, deg, bg, debug=False):
@@ -73,24 +103,52 @@ def dilate(mask, r):
     return torch.nn.functional.max_pool2d(m, 2 * r + 1, stride=1, padding=r)[0, 0] > 0
 
 
-def compare_fused(name, sc, view, deg, bg, gt=None, tiles=None, names=None, record=True, weight_seed=11):
-    """The InstantSplat path (`rasterize_fused`: raw parameters + pose) against `O.render_instantsplat`.
+def _oracle_arm(sc, view, deg, bg, tiles):
+    """fp64 oracle render of `view` (tiles: optional subset) -> (image, radii, aux, finish) where finish(w)
+    back-propagates sum(w * image) and returns the gradients.  The tile lists (rects, depth order) are those of the
+    fp32 projection, which the kernels share to within the ambiguities the lists checks allow; the blend and its
+    gradients are computed in fp64."""
+    lists = O.build_tile_lists(BL.oracle_proj(sc, view, deg))
+    cam = O.Camera.instantsplat(sc.width, sc.height, sc.fovx, sc.fovy, bg=bg, sh_degree=deg, dtype=torch.float64)
+    po = {k: v.double().clone().requires_grad_(True) for k, v in sc.params.items()}
+    pose_o = sc.poses[view].double().clone().requires_grad_(True)
+    m2o = torch.zeros(sc.P, 3, dtype=torch.float64, requires_grad=True)
+    img_o, radii_o, aux = O.render_instantsplat(po["xyz"], po["rotation"], po["scaling"], po["opacity"], po["f_dc"],
+                                                po["f_rest"], pose_o, cam, means2D=m2o, tiles=tiles, return_aux=True,
+                                                lists=lists)
+
+    def finish(w):
+        (img_o * w.double()).sum().backward()
+        g = {k: po[k].grad for k in po}
+        g["pose"], g["means2D"] = pose_o.grad, m2o.grad
+        return g
+    return img_o, radii_o, aux, finish
+
+
+def compare_fused(name, sc, view, deg, bg, gt=None, tiles=None, names=None, record=True, weight_seed=11,
+                  row_tol=None, oracle_cache=None):
+    """The InstantSplat path (`rasterize_fused`: raw parameters + pose) against `O.render_instantsplat` in fp64.
     gt given (full frame only) -> weights = dL/dimage of the training loss, and the CUDA loss kernels are checked
-    too; otherwise seeded random weights on the compared tiles.  Returns the record."""
+    too; otherwise seeded random weights on the compared tiles.  Every tile list of the CUDA forward is checked
+    (`_binning.check_lists`).  row_tol: bound on the 99.9th percentile of the per-row gradient error of every tensor.
+    oracle_cache: a dict that keeps the oracle arm of a random-weight comparison for the next call on the same scene,
+    view and weights (e.g. the same frame under another blend kernel).  Returns the record."""
     import instantsplat_b200 as I
     if names is None:
         names = NAMES if deg > 0 else tuple(n for n in NAMES if n != "f_rest")
-    cam = O.Camera.instantsplat(sc.width, sc.height, sc.fovx, sc.fovy, bg=bg, sh_degree=deg)
-    po = {k: v.clone().requires_grad_(True) for k, v in sc.params.items()}
-    pose_o = sc.poses[view].clone().requires_grad_(True)
-    m2o = torch.zeros(sc.P, 3, requires_grad=True)
-    img_o, radii_o, aux = O.render_instantsplat(po["xyz"], po["rotation"], po["scaling"], po["opacity"], po["f_dc"],
-                                                po["f_rest"], pose_o, cam, means2D=m2o, tiles=tiles, return_aux=True)
+    if oracle_cache is not None and "img" in oracle_cache:
+        assert gt is None
+        img_o, radii_o, aux, g_o = (oracle_cache[k] for k in ("img", "radii", "aux", "grads"))
+        finish = None
+    else:
+        img_o, radii_o, aux, finish = _oracle_arm(sc, view, deg, bg, tiles)
+    img_o = img_o.detach()
     pc = {k: v.to(DEV).clone().requires_grad_(True) for k, v in sc.params.items()}
     pose_c = sc.poses[view].to(DEV).clone().requires_grad_(True)
     m2c = torch.zeros(sc.P, 3, device=DEV, requires_grad=True)
     img_c, radii_c = I.rasterize_fused(pc["xyz"], pc["rotation"], pc["scaling"], pc["opacity"], pc["f_dc"],
                                        pc["f_rest"], pose_c, m2c, settings_for(sc, deg, bg))
+    lists = BL.check_lists(BL.decode(img_c.grad_fn.st))
     mask = None
     if tiles is not None:
         gx = (sc.width + 15) // 16
@@ -103,18 +161,19 @@ def compare_fused(name, sc, view, deg, bg, gt=None, tiles=None, names=None, reco
     rec = dict(case=name, P=sc.P, width=sc.width, height=sc.height, view=int(view), sh_degree=deg,
                tiles_compared=(len(tiles) if tiles is not None else ((sc.width + 15) // 16) * ((sc.height + 15) // 16)),
                **st)
+    rec["lists"] = lists
     rec["radii_mismatch_frac"] = float((radii_c.cpu() != radii_o).float().mean())
     # ---- weights
     if gt is not None:
         assert tiles is None
-        im_o = img_o.detach().clone().requires_grad_(True)
-        loss_o = O.training_loss(im_o, gt)
+        im_o = img_o.clone().requires_grad_(True)
+        loss_o = O.training_loss(im_o, gt.double())
         loss_o.backward()
         w = im_o.grad.clone()
         im_c = img_c.detach().clone().requires_grad_(True)
         loss_c = I.fused_training_loss(im_c, gt.to(DEV))
         loss_c.backward()
-        err = (img_c.detach().cpu() - img_o.detach()).abs().max(0)[0]
+        err = (img_c.detach().cpu() - img_o).abs().max(0)[0]
         near_flip = dilate(err > IMG_TOL, 5)          # SSIM's 11x11 window spreads a flipped pixel over its neighbours
         keep = (~near_flip)[None].expand_as(w)
         rec["loss_abs_err"] = abs(float(loss_c) - float(loss_o))
@@ -127,19 +186,28 @@ def compare_fused(name, sc, view, deg, bg, gt=None, tiles=None, names=None, reco
         if mask is not None:
             w = w * mask
     w = w * (~amb)[None]                              # flagged pixels carry no weight in EITHER arm
-    (img_o * w).sum().backward()
-    (img_c * w.to(DEV)).sum().backward()
-    ge = {k: rel_err(pc[k].grad, po[k].grad) for k in names}
-    ge["pose"] = rel_err(pose_c.grad, pose_o.grad)
-    ge["means2D"] = rel_err(m2c.grad, m2o.grad)
+    if finish is not None:
+        g_o = finish(w)
+        if oracle_cache is not None and gt is None:
+            oracle_cache.update(img=img_o, radii=radii_o, aux=aux, grads=g_o)
+    (img_c * w.float().to(DEV)).sum().backward()
+    g_c = {k: pc[k].grad for k in pc}
+    g_c["pose"], g_c["means2D"] = pose_c.grad, m2c.grad
+    ge = {k: rel_err(g_c[k], g_o[k]) for k in names + ("pose", "means2D")}
     if "f_rest" not in names:
         assert float(pc["f_rest"].grad.abs().max()) == 0.0
     rec["grad_rel_err"] = ge
     rec["grad_rel_err_max"] = max(ge.values())
+    rows = {k: row_err(g_c[k], g_o[k]) for k in names + ("means2D",)}
+    rec["grad_row_err"] = rows
+    rec["grad_row_err_p999_max"] = max(r["p999"] for r in rows.values())
     if record:
         REPORT.append(rec)
     assert_image(st, name)
     assert rec["radii_mismatch_frac"] < 2e-3, rec
     bad = {k: v for k, v in ge.items() if not v < GRAD_TOL}
     assert not bad, f"{name}: gradient relative errors over {GRAD_TOL}: {bad} (all: {ge})"
+    if row_tol is not None:
+        bad = {k: r for k, r in rows.items() if not r["p999"] <= row_tol}
+        assert not bad, f"{name}: per-Gaussian gradient errors (99.9th percentile) over {row_tol}: {bad}"
     return rec
