@@ -1,0 +1,134 @@
+"""Host side of one forward of libgsb200.so: the status-word format, the scratch buffers of a (device, P, W, H), the
+binning-capacity rule and the camera / Gaussians descriptors.
+
+The library protocol is gsb_preprocess -> (the caller may wait for the instance count R) -> size the binning buffer
+-> gsb_render -> gsb_backward.  When to wait, how much headroom to give and when to grow the buffer is the caller's
+policy (rasterizer.py, trainer.py, tracking.py); this module only owns the mechanism and the formats.
+"""
+from __future__ import annotations
+
+import ctypes
+import math
+
+import torch
+
+from . import _lib
+from ._lib import GsbCamera, GsbGaussians, check
+
+# the status words of a forward (kSt* of csrc/gs_internal.cuh); the library writes them as uint32
+ST_R, ST_OVERFLOW, ST_MAX_LIST, ST_HUGE_TILES, ST_NLARGE, ST_NHUGE, ST_SEQ = range(7)
+ST_WORDS = 8
+
+
+def u32(word) -> int:
+    """A status word (int32 in a torch tensor) as the unsigned value the device wrote."""
+    return int(word) & 0xFFFFFFFF
+
+
+def read_R(words) -> int:
+    """Instance count R from a host or device copy of the status words."""
+    return u32(words[ST_R])
+
+
+def capacity(R: int, headroom: float) -> int:
+    """Binning capacity (instances) for an expected count R: the headroom is the caller's, the floor keeps tiny
+    frames from overflowing on small changes."""
+    return int(R * headroom) + 65536
+
+
+def _p(t):
+    return None if t is None else t.data_ptr()
+
+
+def camera(W, H, tanfovx, tanfovy, sh_degree, sh_coeffs, bg, viewmatrix, projmatrix, campos, scale_modifier=1.0,
+           exact_cull=True) -> GsbCamera:
+    """GsbCamera over contiguous fp32 device tensors; exact_cull: lossless alpha < 1/255 tile culling."""
+    cam = GsbCamera()
+    cam.width, cam.height = int(W), int(H)
+    cam.tanfovx, cam.tanfovy, cam.scale_modifier = float(tanfovx), float(tanfovy), float(scale_modifier)
+    cam.sh_degree, cam.sh_coeffs, cam.exact_cull = int(sh_degree), int(sh_coeffs), 1 if exact_cull else 0
+    cam.bg, cam.viewmatrix, cam.projmatrix, cam.campos = _p(bg), _p(viewmatrix), _p(projmatrix), _p(campos)
+    return cam
+
+
+class IdentityView:
+    """InstantSplat's camera (gaussian_renderer/__init__.py:55-59): identity view matrix, camera at the origin and
+    the projection of (fovx, fovy); the camera pose moves the Gaussians instead.  Holds the tensors GsbCamera points to."""
+
+    def __init__(self, W, H, fovx, fovy, bg, device):
+        from .camera import projection_matrix
+        self.W, self.H = int(W), int(H)
+        self.tanfovx, self.tanfovy = math.tan(fovx * 0.5), math.tan(fovy * 0.5)
+        self.viewmatrix = torch.eye(4, device=device)
+        self.projmatrix = projection_matrix(0.01, 100.0, fovx, fovy).t().contiguous().to(device)
+        self.campos = torch.zeros(3, device=device)
+        self.bg = bg.to(device).float().contiguous()
+
+    def camera(self, sh_degree, sh_coeffs, exact_cull=True) -> GsbCamera:
+        return camera(self.W, self.H, self.tanfovx, self.tanfovy, sh_degree, sh_coeffs, self.bg, self.viewmatrix,
+                      self.projmatrix, self.campos, exact_cull=exact_cull)
+
+
+def gaussians(P, xyz, rotation, scaling, opacity, f_dc, f_rest, pose, raw_params=1, sh_packed=0, colors_precomp=None,
+              cov3D_precomp=None) -> GsbGaussians:
+    """GsbGaussians over contiguous fp32 device tensors (None: not given).  raw_params=1: the model's raw parameters
+    (log scales, unnormalised quaternions, logit opacities) moved by `pose`; raw_params=0: activated values as the
+    upstream rasterizer takes them, sh_packed=1 when all SH coefficients are in f_dc as [P, M, 3]."""
+    g = GsbGaussians()
+    g.P, g.sh_packed, g.raw_params = P, int(sh_packed), int(raw_params)
+    g.means3D, g.rotations, g.scales, g.opacities = _p(xyz), _p(rotation), _p(scaling), _p(opacity)
+    g.sh_dc, g.sh_rest, g.pose = _p(f_dc), _p(f_rest), _p(pose)
+    g.colors_precomp, g.cov3D_precomp = _p(colors_precomp), _p(cov3D_precomp)
+    return g
+
+
+class Frame:
+    """Scratch of forwards at one (device, P, W, H): the geometry buffer (which holds the status words), radii, the
+    image buffer, the rendered colour [3, H, W], and a binning buffer of `cap` instances (0: none yet).
+
+    host_status arguments are the caller's pinned 8-word slots (or None): the library copies the status words there
+    after the phase."""
+
+    def __init__(self, device, P, W, H):
+        L = _lib.lib()
+        self.P, self.W, self.H = P, W, H
+        self.geom = torch.empty(L.gsb_geom_bytes(P), dtype=torch.uint8, device=device)
+        self.radii = torch.empty(P, dtype=torch.int32, device=device)
+        self.image = torch.empty(L.gsb_image_bytes(W, H), dtype=torch.uint8, device=device)
+        self.color = torch.empty(3, H, W, dtype=torch.float32, device=device)
+        self._so = L.gsb_status_device(self.geom.data_ptr(), P) - self.geom.data_ptr()
+        self.binning, self.cap = None, 0
+
+    @property
+    def status(self) -> torch.Tensor:
+        """Device view of the status words (int32)."""
+        return self.geom[self._so:self._so + 4 * ST_WORDS].view(torch.int32)
+
+    def word(self, i: int) -> torch.Tensor:
+        """Device view of status word i (one int32); its data_ptr() is the word's device address."""
+        return self.geom[self._so + 4 * i:self._so + 4 * i + 4].view(torch.int32)
+
+    def alloc_binning(self, cap: int, round_to: int = 1) -> None:
+        """A new binning buffer of `cap` instances, its byte size rounded up to a multiple of round_to."""
+        nbytes = (_lib.lib().gsb_binning_bytes(cap, self.W, self.H) + round_to - 1) // round_to * round_to
+        self.binning = torch.empty(nbytes, dtype=torch.uint8, device=self.geom.device)
+        self.cap = cap
+
+    def preprocess(self, cam, g, host_status=None) -> None:
+        check(_lib.lib().gsb_preprocess(ctypes.byref(cam), ctypes.byref(g), self.geom.data_ptr(), self.geom.numel(),
+                                        self.radii.data_ptr(), _p(host_status), _lib.stream_ptr()), "gsb_preprocess")
+
+    def render(self, cam, host_status=None) -> None:
+        check(_lib.lib().gsb_render(ctypes.byref(cam), self.P, self.geom.data_ptr(), self.binning.data_ptr(),
+                                    self.binning.numel(), self.cap, self.image.data_ptr(), self.color.data_ptr(),
+                                    _p(host_status), _lib.stream_ptr()), "gsb_render")
+
+    def backward(self, cam, g, dL_dimage, grads) -> None:
+        check(_lib.lib().gsb_backward(ctypes.byref(cam), ctypes.byref(g), self.geom.data_ptr(), self.binning.data_ptr(),
+                                      self.cap, self.image.data_ptr(), dL_dimage.data_ptr(), ctypes.byref(grads),
+                                      _lib.stream_ptr()), "gsb_backward")
+
+    def blend_stats(self, cam, dL_dimage, stats) -> None:
+        check(_lib.lib().gsb_blend_stats(ctypes.byref(cam), self.P, self.geom.data_ptr(), self.binning.data_ptr(),
+                                         self.cap, self.image.data_ptr(), self.color.data_ptr(), dL_dimage.data_ptr(),
+                                         stats.data_ptr(), _lib.stream_ptr()), "gsb_blend_stats")

@@ -7,18 +7,15 @@ same names, argument meaning and error behaviour.
 """
 from __future__ import annotations
 
-import ctypes
 import warnings
-import weakref
 from typing import NamedTuple, Optional
 
 import torch
 import torch.nn as nn
 
 from . import _lib
-from ._lib import GsbCamera, GsbGaussians, GsbGrads, check, f32c, ptr
-
-_vp = ctypes.c_void_p
+from ._lib import GsbGrads, check, f32c, ptr
+from .frame import ST_WORDS, Frame, camera, capacity, gaussians, read_R
 
 
 class GaussianRasterizationSettings(NamedTuple):
@@ -40,26 +37,22 @@ EXACT_CULL = True   # lossless alpha<1/255 tile culling (set False for the refer
 
 # The instance count R (number of (Gaussian, tile) pairs) never has to reach the host BEFORE the render phase is
 # launched: the kernels read it from device memory, the host only chooses the CAPACITY of the binning buffer.
-# SYNC_FREE = True sizes it from the counts seen for the same (device, P, W, H) with 50 % headroom, enqueues binning
-# and blend, and only then waits for the status words of the PREPROCESS phase (an event right behind the tile scan):
+# A forward sizes it from the counts seen for the same (device, P, W, H) with 50 % headroom, enqueues binning and
+# blend, and only then waits for the status words of the PREPROCESS phase (an event right behind the tile scan):
 # while the host waits, the GPU has the whole render phase queued, so it never idles -- unlike the reference's
 # blocking cudaMemcpy of num_rendered, which stalls the GPU until the host has sized its buffers and launched the
 # rest.  If the capacity was exceeded (rare), the render phase is repeated with an exact buffer before the forward
-# returns, so whatever the caller computes from the image is consistent.  LAZY_VERIFY = True postpones the check to
-# the backward / the next forward instead (forward-only loops that never look at R); the very first call of a shape
-# -- and every call when SYNC_FREE is False -- waits for R before launching the render phase and sizes it exactly.
-SYNC_FREE = True
-LAZY_VERIFY = False
+# returns, so whatever the caller computes from the image is consistent.  The first call of a shape, and every call
+# in debug mode, waits for R before launching the render phase and sizes it exactly.
 HEADROOM = 1.5
 _last_R = {}            # (device index, P, W, H) -> last verified instance count
-_pending = {}           # same key -> _State whose capacity check has not been read yet
 
 
 class _StatusRing:
     """Pinned 8-word status slots, recycled round-robin (a slot is long verified before it comes round again)."""
 
     def __init__(self, n=512):
-        self.buf = torch.zeros(n, 8, dtype=torch.int32).pin_memory()
+        self.buf = torch.zeros(n, ST_WORDS, dtype=torch.int32).pin_memory()
         self.n, self.i = n, 0
 
     def take(self) -> torch.Tensor:
@@ -78,142 +71,64 @@ def _status_slot() -> torch.Tensor:
     return _ring.take()
 
 
-class _State:
-    """Everything the backward needs; keeps the torch buffers alive."""
-    __slots__ = ("cam", "g", "geom", "binning", "image", "R", "keep", "P", "M", "packed", "has_pose",
-                 "key", "status", "event", "checked", "color", "bin_bytes", "R_true", "__weakref__")
+class _State(Frame):
+    """One forward: its scratch buffers and everything the backward needs (cam, g, and `keep`, the converted inputs
+    they point to).  R_true: the forward's instance count."""
+
+    @property
+    def R(self) -> int:
+        """The capacity the render phase ran with (the instance count it was sized for)."""
+        return self.cap
 
 
-def _camera(settings: GaussianRasterizationSettings, sh_coeffs: int, keep: list) -> GsbCamera:
-    bg, vm, pm, cp = (f32c(settings.bg), f32c(settings.viewmatrix), f32c(settings.projmatrix),
-                      f32c(settings.campos))
-    keep += [bg, vm, pm, cp]
-    cam = GsbCamera()
-    cam.width, cam.height = int(settings.image_width), int(settings.image_height)
-    cam.tanfovx, cam.tanfovy = float(settings.tanfovx), float(settings.tanfovy)
-    cam.scale_modifier = float(settings.scale_modifier)
-    cam.sh_degree, cam.sh_coeffs = int(settings.sh_degree), int(sh_coeffs)
-    cam.exact_cull = 1 if EXACT_CULL else 0
-    cam.bg, cam.viewmatrix, cam.projmatrix, cam.campos = ptr(bg), ptr(vm), ptr(pm), ptr(cp)
-    return cam
-
-
-def _render_phase(st: _State, cap: int, dev):
-    """Binning + blend into st.color with a binning buffer of `cap` instances (allocation rounded up to 32 MiB so
-    the caching allocator can reuse the block of the previous call)."""
-    L = _lib.lib()
-    H, W = st.cam.height, st.cam.width
-    bin_bytes = (L.gsb_binning_bytes(cap, W, H) + (1 << 25) - 1) >> 25 << 25
-    st.binning = torch.empty(bin_bytes, dtype=torch.uint8, device=dev)
-    st.bin_bytes, st.R = bin_bytes, cap
-    check(L.gsb_render(ctypes.byref(st.cam), st.P, st.geom.data_ptr(), st.binning.data_ptr(), bin_bytes, cap,
-                       st.image.data_ptr(), st.color.data_ptr(), None, _lib.stream_ptr()), "gsb_render")
-    st.checked = False
-
-
-def _note_R(key, R: int) -> None:
-    """Capacity estimate = slowly decaying maximum of the counts seen (different views share a key)."""
-    _last_R[key] = max(R, int(0.98 * _last_R.get(key, 0)))
-
-
-def _verify(st: _State, dev) -> None:
-    """Read the lazily copied status words of st's forward; if the binning buffer was too small, redo the render
-    phase in place with an exactly sized one (image and scratch become exact before anybody differentiates)."""
-    if st.checked:
-        return
-    st.event.synchronize()                 # recorded right behind the tile scan: early in the forward
-    R_true = int(st.status[0]) & 0xFFFFFFFF
-    overflow = R_true > st.R
-    _note_R(st.key, R_true)
-    st.checked, st.R_true = True, R_true
-    _pending.pop(st.key, None)
-    if overflow:
-        warnings.warn(f"instantsplat_b200: instance count {R_true} exceeded the binning capacity {st.R}; "
-                      "the render phase was repeated with an exact buffer", RuntimeWarning)
-        with torch.cuda.device(dev):
-            _render_phase(st, R_true, dev)
-            st.checked = True
-
-
-def _verify_pending(key, dev) -> None:
-    """At the next forward of the same shape: settle the previous call's capacity check (its result has long
-    arrived; the forward's state may already be gone if nobody differentiated it)."""
-    rec = _pending.pop(key, None)
-    if rec is None:
-        return
-    ref, status, event, cap = rec
-    st = ref()
-    if st is not None:
-        _pending[key] = rec
-        _verify(st, dev)
-        return
-    event.synchronize()
-    _note_R(key, int(status[0]) & 0xFFFFFFFF)
-    if (int(status[0]) & 0xFFFFFFFF) > cap:
-        warnings.warn(f"instantsplat_b200: a forward-only call rendered with a truncated binning buffer "
-                      f"({_last_R[key]} instances > capacity {cap}); the capacity has been raised", RuntimeWarning)
+_BIN_ROUND = 1 << 25    # binning allocations rounded up to 32 MiB so the caching allocator can reuse the last block
 
 
 def _forward(settings, means3D, scales, rotations, opacities, sh_dc, sh_rest, sh_packed, M,
              colors_precomp, cov3D_precomp, pose, raw_params):
-    L = _lib.lib()
     dev = means3D.device
     if means3D.dim() != 2 or means3D.shape[1] != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")
     P = means3D.shape[0]
-    st = _State()
-    st.keep = []
-    st.cam = _camera(settings, M, st.keep)
-    g = GsbGaussians()
-    g.P, g.sh_packed, g.raw_params = P, int(sh_packed), int(raw_params)
-    ts = dict(means3D=means3D, scales=scales, rotations=rotations, opacities=opacities, sh_dc=sh_dc,
-              sh_rest=sh_rest, colors_precomp=colors_precomp, cov3D_precomp=cov3D_precomp, pose=pose)
-    for k, v in ts.items():
-        v = f32c(v)
-        st.keep.append(v)
-        setattr(g, k, ptr(v))
-    st.g, st.P, st.M, st.packed, st.has_pose = g, P, M, bool(sh_packed), pose is not None
-    H, W = st.cam.height, st.cam.width
-    st.key = (dev.index, P, W, H)
+    W, H = int(settings.image_width), int(settings.image_height)
+    keep = [f32c(t) for t in (settings.bg, settings.viewmatrix, settings.projmatrix, settings.campos, means3D,
+                              scales, rotations, opacities, sh_dc, sh_rest, colors_precomp, cov3D_precomp, pose)]
+    bg, vm, pm, cp, xyz, sca, rot, op, dc, rest, cpre, cov, pos = keep
+    cam = camera(W, H, settings.tanfovx, settings.tanfovy, settings.sh_degree, M, bg, vm, pm, cp,
+                 settings.scale_modifier, EXACT_CULL)
+    g = gaussians(P, xyz, rot, sca, op, dc, rest, pos, raw_params, sh_packed, cpre, cov)
+    key = (dev.index, P, W, H)
     with torch.cuda.device(dev):
-        _verify_pending(st.key, dev)   # long finished in practice: just reads the pinned words
-        stream = _lib.stream_ptr()
-        geom_bytes = L.gsb_geom_bytes(P)
-        st.geom = torch.empty(geom_bytes, dtype=torch.uint8, device=dev)
-        radii = torch.empty(P, dtype=torch.int32, device=dev)
-        st.image = torch.empty(L.gsb_image_bytes(W, H), dtype=torch.uint8, device=dev)
-        st.color = torch.empty(3, H, W, dtype=torch.float32, device=dev)
-        est = _last_R.get(st.key) if (SYNC_FREE and not settings.debug) else None
-        st.status = _status_slot()
-        check(L.gsb_preprocess(ctypes.byref(st.cam), ctypes.byref(g), st.geom.data_ptr(), geom_bytes,
-                               radii.data_ptr(), st.status.data_ptr(), stream), "gsb_preprocess")
-        st.event = torch.cuda.Event()
-        st.event.record()
+        st = _State(dev, P, W, H)
+        st.cam, st.g, st.keep = cam, g, keep
+        st.M, st.packed, st.has_pose = M, bool(sh_packed), pose is not None
+        est = None if settings.debug else _last_R.get(key)
+        status = _status_slot()
+        st.preprocess(cam, g, status)
+        event = torch.cuda.Event()
+        event.record()
         if est is None:
-            st.event.synchronize()                         # exact sizing: wait for R once
-            cap = int(st.status[0]) & 0xFFFFFFFF
-        else:
-            cap = int(est * HEADROOM) + 65536
-        _render_phase(st, cap, dev)
-        if est is None:
-            _note_R(st.key, cap)
-            st.checked, st.R_true = True, cap
-        elif LAZY_VERIFY:
-            _pending[st.key] = (weakref.ref(st), st.status, st.event, cap)
-        else:
-            _verify(st, dev)             # waits for the preprocess phase only; repeats the render phase on overflow
+            event.synchronize()                            # exact sizing: wait for R once
+        st.alloc_binning(read_R(status) if est is None else capacity(est, HEADROOM), _BIN_ROUND)
+        st.render(cam)
+        event.synchronize()                                # recorded right behind the tile scan: early in the forward
+        st.R_true = R = read_R(status)
+        _last_R[key] = max(R, int(0.98 * _last_R.get(key, 0)))   # decaying maximum: different views share a key
+        if R > st.cap:
+            warnings.warn(f"instantsplat_b200: instance count {R} exceeded the binning capacity {st.cap}; "
+                          "the render phase was repeated with an exact buffer", RuntimeWarning)
+            st.alloc_binning(R, _BIN_ROUND)
+            st.render(cam)
         if settings.debug:
             torch.cuda.synchronize()
-    return st.color, radii, st
+    return st.color, st.radii, st
 
 
 def _backward(st: _State, dL_dout, want, dev):
     """want: None (everything) or a set of names to compute; gradients that are not wanted are neither
     allocated nor written by the kernels (e.g. the pose-only test-view optimisation of
     render.py:99-170 passes {"pose"}).  Returns dict of dense grad tensors."""
-    L = _lib.lib()
     P, M = st.P, st.M
-    _verify(st, dev)
     dL = f32c(dL_dout)
     gr = GsbGrads()
     out = {}
@@ -246,9 +161,7 @@ def _backward(st: _State, dL_dout, want, dev):
         t = torch.empty(7, dtype=torch.float32, device=dev)     # always required by the ABI when pose is fused
         out["pose"] = t
         gr.dL_dpose = t.data_ptr()
-    check(L.gsb_backward(ctypes.byref(st.cam), ctypes.byref(st.g), st.geom.data_ptr(), st.binning.data_ptr(),
-                         st.R, st.image.data_ptr(), dL.data_ptr(), ctypes.byref(gr), _lib.stream_ptr()),
-          "gsb_backward")
+    st.backward(st.cam, st.g, dL, gr)
     return out
 
 

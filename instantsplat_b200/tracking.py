@@ -16,7 +16,6 @@ evaluates the cosine schedule; nothing waits for the GPU until the best pose is 
 """
 from __future__ import annotations
 
-import ctypes
 import math
 from typing import Optional
 
@@ -24,6 +23,7 @@ import torch
 
 from . import _lib
 from ._lib import GsbCamera, GsbGaussians, GsbGrads, check
+from .frame import ST_OVERFLOW, ST_WORDS, Frame, IdentityView, capacity, gaussians, read_R
 
 
 def cosine_lr(base_lr: float, k: int, t_max: int, eta_min: float = 1e-4) -> float:
@@ -43,21 +43,10 @@ class PoseTracker:
         self.P = self.xyz.shape[0]
         self.W, self.H = int(width), int(height)
         self.sh_degree = int(sh_degree)
-        from .camera import projection_matrix
-        self.tanfovx, self.tanfovy = math.tan(fovx * 0.5), math.tan(fovy * 0.5)
-        self.viewmatrix = torch.eye(4, device=self.dev)
-        self.projmatrix = projection_matrix(0.01, 100.0, fovx, fovy).t().contiguous().to(self.dev)
-        self.campos = torch.zeros(3, device=self.dev)
-        self.bg = (torch.zeros(3) if bg is None else bg).to(self.dev).float().contiguous()
-        L = _lib.lib()
-        self.geom_bytes = L.gsb_geom_bytes(self.P)
-        self.geom = torch.empty(self.geom_bytes, dtype=torch.uint8, device=self.dev)
-        self.image_buf = torch.empty(L.gsb_image_bytes(self.W, self.H), dtype=torch.uint8, device=self.dev)
-        self.radii = torch.empty(self.P, dtype=torch.int32, device=self.dev)
-        self.color = torch.empty(3, self.H, self.W, dtype=torch.float32, device=self.dev)
-        self.dL = torch.empty_like(self.color)
-        self.host_status = torch.zeros(8, dtype=torch.int32).pin_memory()
-        self.cap, self.binning, self.bin_bytes = 0, None, 0
+        self.ident = IdentityView(self.W, self.H, fovx, fovy, torch.zeros(3) if bg is None else bg, self.dev)
+        self.frame = Frame(self.dev, self.P, self.W, self.H)
+        self.dL = torch.empty_like(self.frame.color)
+        self.host_status = torch.zeros(ST_WORDS, dtype=torch.int32).pin_memory()
         self.headroom = 1.6            # the pose moves during tracking, and with it the instance count
         self.R_seen = 0
 
@@ -70,44 +59,27 @@ class PoseTracker:
 
     # ------------------------------------------------------------------------------------------
     def _cam(self) -> GsbCamera:
-        cam = GsbCamera()
-        cam.width, cam.height = self.W, self.H
-        cam.tanfovx, cam.tanfovy, cam.scale_modifier = self.tanfovx, self.tanfovy, 1.0
-        cam.sh_degree, cam.sh_coeffs, cam.exact_cull = self.sh_degree, 1 + self.f_rest.shape[1], 1
-        cam.bg, cam.viewmatrix = self.bg.data_ptr(), self.viewmatrix.data_ptr()
-        cam.projmatrix, cam.campos = self.projmatrix.data_ptr(), self.campos.data_ptr()
-        return cam
+        return self.ident.camera(self.sh_degree, 1 + self.f_rest.shape[1])
 
     def _gauss(self, pose: torch.Tensor) -> GsbGaussians:
-        g = GsbGaussians()
-        g.P, g.sh_packed, g.raw_params = self.P, 0, 1
-        g.means3D, g.scales, g.rotations = self.xyz.data_ptr(), self.scaling.data_ptr(), self.rotation.data_ptr()
-        g.opacities, g.sh_dc = self.opacity.data_ptr(), self.f_dc.data_ptr()
-        g.sh_rest = self.f_rest.data_ptr() if self.f_rest.numel() else None
-        g.pose = pose.data_ptr()
-        return g
+        return gaussians(self.P, self.xyz, self.rotation, self.scaling, self.opacity, self.f_dc,
+                         self.f_rest if self.f_rest.numel() else None, pose)
 
     def _forward(self, cam, g, first: bool):
-        L = _lib.lib()
-        st = _lib.stream_ptr()
-        check(L.gsb_preprocess(ctypes.byref(cam), ctypes.byref(g), self.geom.data_ptr(), self.geom_bytes,
-                               self.radii.data_ptr(), self.host_status.data_ptr() if first else None, st), "gsb_preprocess")
+        fr = self.frame
+        fr.preprocess(cam, g, self.host_status if first else None)
         if first:                      # size the binning buffer once, from the real count at the initial pose
             torch.cuda.current_stream().synchronize()
-            R = int(self.host_status[0]) & 0xFFFFFFFF
-            self.R_seen = R
-            if R * self.headroom + 65536 > self.cap:
-                self.cap = int(R * self.headroom) + 65536
-                self.bin_bytes = L.gsb_binning_bytes(self.cap, self.W, self.H)
-                self.binning = torch.empty(self.bin_bytes, dtype=torch.uint8, device=self.dev)
-        check(L.gsb_render(ctypes.byref(cam), self.P, self.geom.data_ptr(), self.binning.data_ptr(), self.bin_bytes,
-                           self.cap, self.image_buf.data_ptr(), self.color.data_ptr(), None, st), "gsb_render")
+            self.R_seen = R = read_R(self.host_status)
+            if capacity(R, self.headroom) > fr.cap:
+                fr.alloc_binning(capacity(R, self.headroom))
+        fr.render(cam)
 
     def render(self, pose: torch.Tensor) -> torch.Tensor:
         with torch.cuda.device(self.dev):
             p = pose.detach().to(self.dev).float().contiguous()
             self._forward(self._cam(), self._gauss(p), True)
-            return self.color.clone()
+            return self.frame.color.clone()
 
     def optimize(self, init_pose: torch.Tensor, gt: torch.Tensor, num_iter: int = 500, lr_T: float = 0.003,
                  lr_q: float = 0.001, weight_decay: float = 1e-4, eta_min: float = 1e-4,
@@ -129,18 +101,15 @@ class PoseTracker:
             cam, g = self._cam(), self._gauss(pose)
             gr = GsbGrads()
             gr.dL_dpose = dpose.data_ptr()
-            status_dev = L.gsb_status_device(self.geom.data_ptr(), self.P)
             ovf = torch.zeros(1, dtype=torch.int32, device=self.dev)
-            so = status_dev - self.geom.data_ptr()
-            status_t = self.geom[so:so + 32].view(torch.int32)
+            ovf_word = self.frame.word(ST_OVERFLOW)
             for k in range(num_iter):
                 self._forward(cam, g, k == 0)
-                ovf |= status_t[1:2]                       # sticky overflow flag, checked once at the end
-                check(L.gsb_l1_mask_fwd_bwd(3, self.H, self.W, self.color.data_ptr(), gt.data_ptr(), float(threshold),
-                                            sums[k].data_ptr(), self.dL.data_ptr(), st), "gsb_l1_mask_fwd_bwd")
-                check(L.gsb_backward(ctypes.byref(cam), ctypes.byref(g), self.geom.data_ptr(), self.binning.data_ptr(),
-                                     self.cap, self.image_buf.data_ptr(), self.dL.data_ptr(), ctypes.byref(gr), st),
-                      "gsb_backward")
+                ovf |= ovf_word                            # sticky overflow flag, checked once at the end
+                check(L.gsb_l1_mask_fwd_bwd(3, self.H, self.W, self.frame.color.data_ptr(), gt.data_ptr(),
+                                            float(threshold), sums[k].data_ptr(), self.dL.data_ptr(), st),
+                      "gsb_l1_mask_fwd_bwd")
+                self.frame.backward(cam, g, self.dL, gr)
                 check(L.gsb_track_step(pose.data_ptr(), dpose.data_ptr(), sums[k].data_ptr(), m.data_ptr(), v.data_ptr(),
                                        best.data_ptr(), trace[k:].data_ptr() if return_trace else None, k + 1,
                                        cosine_lr(lr_q, k, num_iter, eta_min), cosine_lr(lr_T, k, num_iter, eta_min),

@@ -18,15 +18,14 @@ kernel, so all replicas stay bit-identical.  An "iteration" in the reported iter
 """
 from __future__ import annotations
 
-import ctypes
-import math
 from typing import Dict, List, Optional
 
 import numpy as np
 import torch
 
 from . import _lib
-from ._lib import GsbCamera, GsbGaussians, GsbGrads, check
+from ._lib import GsbGaussians, GsbGrads, check
+from .frame import ST_OVERFLOW, ST_SEQ, ST_WORDS, Frame, IdentityView, capacity, gaussians, read_R
 from .per_point_adam import launch_adam
 from .scenes import Scene
 
@@ -140,32 +139,14 @@ class JointTrainer:
             ppl[:P] = scene.per_point_lr.to(self.dev).float().reshape(P)
             self.per_point_lr = ppl
         self.gt = None if gt_images is None else gt_images.to(self.dev).float().contiguous()
-        # ---- camera constants (identity view, reference gaussian_renderer/__init__.py:55-59)
-        from .camera import projection_matrix
-        self.tanfovx, self.tanfovy = math.tan(scene.fovx * 0.5), math.tan(scene.fovy * 0.5)
-        self.viewmatrix = torch.eye(4, device=self.dev)
-        self.projmatrix = projection_matrix(0.01, 100.0, scene.fovx, scene.fovy).t().contiguous().to(self.dev)
-        self.campos = torch.zeros(3, device=self.dev)
-        self.bg = scene.bg.to(self.dev).float().contiguous()
-        # ---- scratch
-        L = _lib.lib()
-        self.geom_bytes = L.gsb_geom_bytes(P)
-        self.geom = torch.empty(self.geom_bytes, dtype=torch.uint8, device=self.dev)
-        self.image_buf = torch.empty(L.gsb_image_bytes(self.W, self.H), dtype=torch.uint8, device=self.dev)
-        self.binning = None
-        self.bin_bytes = 0
-        self.cap = 0                  # instance capacity of the binning buffer (0: not sized yet)
+        self.ident = IdentityView(self.W, self.H, scene.fovx, scene.fovy, scene.bg, self.dev)
+        self.frame = Frame(self.dev, P, self.W, self.H)     # scratch; its binning buffer is sized by the first forward
         self.headroom = 1.5
-        self.radii = torch.empty(P, dtype=torch.int32, device=self.dev)
-        self.color = torch.empty(3, self.H, self.W, dtype=torch.float32, device=self.dev)
         self.dL_dimg = torch.empty_like(self.color)
         self.maps = torch.empty(3, 3, self.H, self.W, dtype=torch.float32, device=self.dev)
         self.sums = torch.zeros(2, dtype=torch.float64, device=self.dev)
-        self.host_status = torch.zeros(2, 8, dtype=torch.int32).pin_memory()   # [0] after preprocess, [1] after render
+        self.host_status = torch.zeros(2, ST_WORDS, dtype=torch.int32).pin_memory()   # [0] after preprocess, [1] after render
         self._ev_pre = torch.cuda.Event()
-        self._status_dev = L.gsb_status_device(self.geom.data_ptr(), P)        # device address of the status words
-        so = self._status_dev - self.geom.data_ptr()
-        self._status_t = self.geom[so:so + 32].view(torch.int32)               # [R, overflow, longest list, ...]
         self._ovf = None
         self.flags = torch.zeros(8, dtype=torch.int32, device=self.dev)
         self._pose_flags = torch.zeros(8, dtype=torch.int32, device=self.dev)
@@ -181,7 +162,7 @@ class JointTrainer:
         self._after_backward = None   # test hook: called (and captured) between the backward and the optimizer step
         self._step_host = torch.zeros(8, dtype=torch.float32).pin_memory()
         self._step_dev = torch.zeros(8, dtype=torch.float32, device=self.dev)
-        self._status_t.zero_()        # the forward serial number lives in these words
+        self.frame.status.zero_()     # the forward serial number lives in these words
         self._fwd_count = 0
         self._polling = False
         self.iteration = 0            # reference iterations = views consumed (by all ranks)
@@ -209,55 +190,39 @@ class JointTrainer:
         from .parallel import shard_views
         return shard_views(self.n_views, self.world_size, self.rank)
 
-    def _cam(self) -> GsbCamera:
-        cam = GsbCamera()
-        cam.width, cam.height = self.W, self.H
-        cam.tanfovx, cam.tanfovy, cam.scale_modifier = self.tanfovx, self.tanfovy, 1.0
-        cam.sh_degree, cam.sh_coeffs = self.active_sh_degree, 16
-        cam.exact_cull = 1 if self.exact_cull else 0
-        cam.bg, cam.viewmatrix = self.bg.data_ptr(), self.viewmatrix.data_ptr()
-        cam.projmatrix, cam.campos = self.projmatrix.data_ptr(), self.campos.data_ptr()
-        return cam
+    @property
+    def color(self) -> torch.Tensor:
+        """The last rendered image [3, H, W]."""
+        return self.frame.color
+
+    @property
+    def cap(self) -> int:
+        """Instance capacity of the binning buffer (0: not sized yet)."""
+        return self.frame.cap
 
     def _gauss(self, view: int) -> GsbGaussians:
-        g = GsbGaussians()
-        g.P, g.sh_packed, g.raw_params = self.P, 0, 1
         p = self.params
-        g.means3D = self.view(p, "xyz").data_ptr()
-        g.scales = self.view(p, "scaling").data_ptr()
-        g.rotations = self.view(p, "rotation").data_ptr()
-        g.opacities = self.view(p, "opacity").data_ptr()
-        g.sh_dc = self.view(p, "f_dc").data_ptr()
-        g.sh_rest = self.view(p, "f_rest").data_ptr()
-        g.pose = self.poses[view].data_ptr()
-        return g
+        return gaussians(self.P, *(self.view(p, n) for n in ("xyz", "rotation", "scaling", "opacity", "f_dc", "f_rest")),
+                         self.poses[view])
 
     # ------------------------------------------------------------------------------------------
     def _size_binning(self, R: int) -> None:
-        L = _lib.lib()
-        self.cap = int(R * self.headroom) + 65536
-        self.bin_bytes = L.gsb_binning_bytes(self.cap, self.W, self.H)
-        self.binning = torch.empty(self.bin_bytes, dtype=torch.uint8, device=self.dev)
+        self.frame.alloc_binning(capacity(R, self.headroom))
 
     def _launch_forward(self, view: int) -> None:
         """Enqueue the forward without ever waiting for the GPU: the instance count R stays on the device; the
         host only provides a capacity (sized from the counts seen so far, +50 %) and reads R back lazily."""
-        L = _lib.lib()
-        st = _lib.stream_ptr()
-        cam, g = self._cam(), self._gauss(view)
+        cam, g = self.ident.camera(self.active_sh_degree, 16, self.exact_cull), self._gauss(view)
         capturing = torch.cuda.is_current_stream_capturing()
-        check(L.gsb_preprocess(ctypes.byref(cam), ctypes.byref(g), self.geom.data_ptr(), self.geom_bytes,
-                               self.radii.data_ptr(), self.host_status[0].data_ptr(), st), "gsb_preprocess")
+        self.frame.preprocess(cam, g, self.host_status[0])
         if not capturing:
             self._fwd_count += 1
             self._polling = False
             self._ev_pre.record()
-            if self.cap == 0:                               # very first forward: size the buffer from the real count
+            if self.cap == 0:                         # very first forward: size the buffer from the real count
                 self._ev_pre.synchronize()
-                self._size_binning(int(self.host_status[0, 0]) & 0xFFFFFFFF)
-        check(L.gsb_render(ctypes.byref(cam), self.P, self.geom.data_ptr(), self.binning.data_ptr(),
-                           self.bin_bytes, self.cap, self.image_buf.data_ptr(), self.color.data_ptr(),
-                           self.host_status[1].data_ptr(), st), "gsb_render")
+                self._size_binning(read_R(self.host_status[0]))
+        self.frame.render(cam, self.host_status[1])
         self._keep = (cam, g)
 
     def _settle(self) -> bool:
@@ -270,19 +235,19 @@ class JointTrainer:
             want = self._fwd_count & 0x7FFFFFFF
             hs = self.host_status
             n = 0
-            while (int(hs[0, 6]) & 0x7FFFFFFF) != want:
+            while (int(hs[0, ST_SEQ]) & 0x7FFFFFFF) != want:
                 n += 1
                 if n > 20_000_000:
                     raise _lib.GsbError("graph replay: the forward's status words never arrived")
         else:
             self._ev_pre.synchronize()
-        R = int(self.host_status[0, 0]) & 0xFFFFFFFF
+        R = read_R(self.host_status[0])
         self.last_R = R
         if R > self.cap:
             self.overflows += 1
             self._size_binning(R)
             return False
-        if R > 0.85 * self.cap:                              # grow ahead of need
+        if R > 0.85 * self.cap:                        # grow ahead of need
             self._size_binning(R)
         return True
 
@@ -313,9 +278,7 @@ class JointTrainer:
         gr.dL_dsh_rest = self.view(gd, "f_rest").data_ptr()
         self.pose_grad.zero_()
         gr.dL_dpose = self.pose_grad[view].data_ptr()
-        check(L.gsb_backward(ctypes.byref(cam), ctypes.byref(g), self.geom.data_ptr(), self.binning.data_ptr(),
-                             self.cap, self.image_buf.data_ptr(), self.dL_dimg.data_ptr(), ctypes.byref(gr), st),
-              "gsb_backward")
+        self.frame.backward(cam, g, self.dL_dimg, gr)
 
     def loss_value(self) -> torch.Tensor:
         n = 3 * self.H * self.W
@@ -325,7 +288,7 @@ class JointTrainer:
     def reduce_grads(self) -> None:
         if self.world_size > 1:
             from .parallel import allreduce_sum_
-            self._pg_buf[-1:].copy_(self._status_t[1:2])
+            self._pg_buf[-1:].copy_(self.frame.word(ST_OVERFLOW))
             allreduce_sum_((self.grads, self._pg_buf), self.pg)
 
     def _step_sizes(self):
@@ -375,7 +338,7 @@ class JointTrainer:
         (multi-GPU: its sum over ranks, so that every replica takes the same decision)."""
         if self.world_size > 1:
             return self._ovf.data_ptr()
-        return self._status_dev + 4
+        return self.frame.word(ST_OVERFLOW).data_ptr()
 
     def _lrs(self):
         c = self.cfg
@@ -412,13 +375,14 @@ class JointTrainer:
             # kernel through peer memory; its flag barrier is also "every rank's gradients are written".  Epoch 0 = the
             # device-resident epoch counter (advanced by this kernel), so the launch is identical every step
             check(L.gsb_peer_exchange(self.world_size, self.rank, self._peer_sig.ptr_array(), 0,
-                                      self.flags.data_ptr(), self._status_dev + 4, self.pose_grad.data_ptr(),
+                                      self.flags.data_ptr(), self.frame.word(ST_OVERFLOW).data_ptr(),
+                                      self.pose_grad.data_ptr(),
                                       self.pose_grad.numel(), st), "gsb_peer_exchange")
         else:
             # one small SUM all-reduce carries both the gate flags (as counts) and the pose-gradient table
             # (self.pose_grad is a view of self._xch[8:]); it is also the pre-barrier of the fused kernel
             self._xch[:8].copy_(self.flags)
-            self._xch[7:8].copy_(self._status_t[1:2])          # slot 7: binning overflow (summed over ranks)
+            self._xch[7:8].copy_(self.frame.word(ST_OVERFLOW))  # slot 7: binning overflow (summed over ranks)
             dist.all_reduce(self._xch, op=dist.ReduceOp.SUM, group=self.pg)
             self.flags.copy_(self._xch[:8])
         # 2. the fused kernel over this rank's shard
@@ -562,7 +526,6 @@ class JointTrainer:
         if self._fused:
             raise _lib.GsbError("changing the number of Gaussians is not supported with peer-memory buffers "
                                 "(exchange='fused_p2p'); use exchange='allreduce'")
-        L = _lib.lib()
         new = {name: rows(name, self.view(self.params, name), self.view(self.exp_avg, name),
                           self.view(self.exp_avg_sq, name)) for name, _ in SEGMENTS}
         offs, total = {}, 0
@@ -579,16 +542,10 @@ class JointTrainer:
             self.view(self.params, name).copy_(p_.reshape(new_P, k))
             self.view(self.exp_avg, name).copy_(m_.reshape(new_P, k))
             self.view(self.exp_avg_sq, name).copy_(v_.reshape(new_P, k))
-        self.geom_bytes = L.gsb_geom_bytes(new_P)
-        self.geom = torch.empty(self.geom_bytes, dtype=torch.uint8, device=self.dev)
-        self.radii = torch.empty(new_P, dtype=torch.int32, device=self.dev)
-        self._status_dev = L.gsb_status_device(self.geom.data_ptr(), new_P)
-        so = self._status_dev - self.geom.data_ptr()
-        self._status_t = self.geom[so:so + 32].view(torch.int32)
-        self.cap = 0                                  # the next forward sizes the binning buffer from the new count
+        self.frame = Frame(self.dev, new_P, self.W, self.H)   # the next forward sizes its binning buffer
         self._keep = None
         self._graphs.clear()
-        self._status_t.zero_()
+        self.frame.status.zero_()
         self._fwd_count = 0
 
     def _set_per_point_lr(self, values: Optional[torch.Tensor]) -> None:
@@ -638,14 +595,11 @@ class JointTrainer:
     def blend_stats(self, view: int, gt: Optional[torch.Tensor] = None) -> Dict[str, int]:
         """Pair statistics of the blend kernels for one forward+backward of `view` (instrumented re-run of the same
         kernels, outside any timed region): evaluated / contributing (pixel, Gaussian) pairs."""
-        L = _lib.lib()
         self.render(view)
         self.loss_and_backward(view, self.gt[view] if gt is None else gt)
         cam, _ = self._keep
         stats = torch.zeros(8, dtype=torch.int64, device=self.dev)
-        check(L.gsb_blend_stats(ctypes.byref(cam), self.P, self.geom.data_ptr(), self.binning.data_ptr(), self.cap,
-                                self.image_buf.data_ptr(), self.color.data_ptr(), self.dL_dimg.data_ptr(),
-                                stats.data_ptr(), _lib.stream_ptr()), "gsb_blend_stats")
+        self.frame.blend_stats(cam, self.dL_dimg, stats)
         s = stats.cpu().tolist()
         return dict(instances=self.last_R, fwd_warp_iters=s[0], fwd_pairs_evaluated=64 * s[0], fwd_pairs_contributing=s[1],
                     bwd_warp_iters=s[2], bwd_pairs_evaluated=64 * s[2], bwd_pairs_contributing=s[3],

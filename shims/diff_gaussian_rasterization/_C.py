@@ -42,7 +42,6 @@ def rasterize_gaussians(bg, means3D, colors_precomp, opacities, scales, rotation
     M = sh_.shape[1] if sh_ is not None else 1
     color, radii, st = _R._forward(rs, means3D, _opt(scales), _opt(rotations), opacities.reshape(-1), sh_, None, 1, M,
                                    _opt(colors_precomp), _opt(cov3D_precomp), None, 0)
-    _R._verify(st, means3D.device)                   # upstream returns num_rendered as a host int: settle it now
     geom, binning, image = st.geom, st.binning, st.image
     st.geom = st.binning = st.image = None          # the registry must not keep the scratch alive
     # upstream's signature has no room for a handle, so the call is keyed on the buffer's address; the entry dies

@@ -16,11 +16,12 @@ The checks are integer checks on the GPU (configs[4] has ~46 M instances), so th
 import numpy as np
 import torch
 
+from instantsplat_b200.frame import ST_HUGE_TILES, ST_MAX_LIST, ST_NHUGE, ST_NLARGE, ST_OVERFLOW, ST_R, u32
+
 BLOCK = 16
 ALIGN = 256
 SMALL_LIST, LARGE_LIST = 2048, 8192      # kSmallList / kLargeList: the per-tile sort's size classes
 SKEW = 24                                # kSkew: a bucket longer than this sends a tile to the bitonic fallback
-ST_R, ST_OVERFLOW, ST_MAX_LIST, ST_HUGE_TILES, ST_NLARGE, ST_NHUGE = range(6)
 
 
 def align_up(v, a=ALIGN):
@@ -41,11 +42,7 @@ def bin_layout(cap, W, H):
 
 def status_words(st):
     """The forward's device status words (uint32, as Python ints)."""
-    from instantsplat_b200 import _lib
-    base = st.geom.data_ptr()
-    off = _lib.lib().gsb_status_device(base, st.P) - base
-    w = st.geom[off:off + 32].view(torch.int32).cpu().tolist()
-    return [x & 0xFFFFFFFF for x in w]
+    return [u32(x) for x in st.status.cpu().tolist()]
 
 
 def decode(st):
@@ -76,7 +73,7 @@ def check_lists(d):
     R = s[ST_R]
     assert R <= d["cap"], f"binning overflow (R {R}, capacity {d['cap']})"
     # a render phase that overflowed its estimated capacity raised the overflow word and was repeated with an exact
-    # buffer (rasterizer._verify): the lists are then those of the second pass, and the huge tiles were sorted twice
+    # buffer (rasterizer._forward): the lists are then those of the second pass, and the huge tiles were sorted twice
     passes = 2 if s[ST_OVERFLOW] else 1
     lens = rng[:, 1] - rng[:, 0]
     assert bool((lens >= 0).all()), "negative tile range"
