@@ -147,11 +147,11 @@ __global__ void __launch_bounds__(kThreads) k_abs_max(size_t n, const float* __r
 
 // Adds the warp's totals to a Gaussian's fixed-point slots.  After warp_reduce9 / warp_reduce8, lane 4i holds total i
 // (i < 8) in v0 and every lane holds total 8 in v8; lane 1 adds slot 8 when `ninth`.
-__device__ __forceinline__ void flush_fixed(unsigned long long* dst, float v0, float v8, float radius, float inv_m, int lane,
+__device__ __forceinline__ void flush_fixed(unsigned long long* dst, float v0, float v8, float extent, float inv_m, int lane,
                                             bool ninth) {
   if ((lane & 3) == 0 || (ninth && lane == 1)) {
     const int slot = (lane & 3) ? 8 : lane >> 2;
-    atomicAdd(dst + slot, fix_encode((lane & 3) ? v8 : v0, fix_scale(slot, radius, inv_m)));
+    atomicAdd(dst + slot, fix_encode((lane & 3) ? v8 : v0, fix_scale(slot, extent, inv_m)));
   }
 }
 

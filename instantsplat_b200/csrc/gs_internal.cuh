@@ -63,23 +63,32 @@ constexpr uint32_t kSmallList = 2048, kLargeList = 8192;
 // The blend backward adds per-Gaussian pixel moments from many tiles.  Floating-point atomics would make each sum
 // depend on the order in which the CTAs arrive, so the gradients -- and, through Adam, a whole training run -- would
 // differ from run to run.  The moments are added as 64-bit integers instead; integer addition is associative, so every
-// run produces the same bits.  Slot k of Gaussian i counts in units of 1 / fix_scale(k, radius_i, M) with
-// M = max |dL/dpixel| of the launch: |slot k| <= c * M * (radius + 1)^fix_exp(k) for a small constant c (pixels covered
-// ~ radius^2, |dx|, |dy| <= radius), so the unit 2^-50 * M * (radius + 1)^fix_exp(k) leaves 13 bits of headroom above
-// that bound and ~50 bits of resolution below it -- finer than the float each contribution starts from.
+// run produces the same bits.  Slot k of Gaussian i counts in units of 1 / fix_scale(k, e_i, M) with
+// M = max |dL/dpixel| of the launch and e_i the Gaussian's extent (fix_extent): the smaller of its radius and the
+// Chebyshev distance from its centre to the farthest pixel centre of the frame.  Every pixel it contributes to lies
+// within both, so |dx|, |dy| <= ~e and the pixels covered are ~e^2: |slot k| <= c * M * (e + 1)^fix_exp(k) for a small
+// constant c, and the unit 2^-50 * M * (e + 1)^fix_exp(k) leaves 13 bits of headroom above that bound and ~50 bits of
+// resolution below it -- finer than the float each contribution starts from.  (With the radius alone, a Gaussian just
+// in front of the near plane -- radius 1e5 px on a 256 px frame -- would lose ~35 of those bits.)
 // Slots: [S w dx, S w dy, S w dx^2, S w dx dy, S w dy^2, S w (tracking: dL/db), dL/dr, dL/dg, dL/db].
 constexpr int kDaccSlots = 9;
 __host__ __device__ constexpr int fix_exp(int k) { return k < 2 ? 3 : (k < 5 ? 4 : 2); }
+// the extent of the fixed-point unit, stored in the splat record (rec[2].w) by k_preprocess for the blend backward
+// (encoder) and k_preprocess_bwd (decoder); 0 for a Gaussian that covers nothing
+__host__ __device__ inline float fix_extent(int radius, float x, float y, int W, int H) {
+  const float reach = fmaxf(fmaxf(fabsf(x), fabsf((float)(W - 1) - x)), fmaxf(fabsf(y), fabsf((float)(H - 1) - y)));
+  return fminf((float)radius, reach);
+}
 #if defined(__CUDACC__)
 // 2^50 / M (M floored at 1e-20 so that the scale stays a finite float)
 __device__ __forceinline__ float fix_inv_m(const uint32_t* dscale) {
   return __fdiv_rn(0x1p50f, fmaxf(__uint_as_float(*dscale), 1e-20f));
 }
-// integer steps per unit of slot k for a Gaussian of the given radius.  Encoder and decoder evaluate the same expression
+// integer steps per unit of slot k for a Gaussian of the given extent.  Encoder and decoder evaluate the same expression
 // (MUFU.RCP is deterministic), so the approximate reciprocal costs nothing in reproducibility.
-__device__ __forceinline__ float fix_scale(int k, float radius, float inv_m) {
+__device__ __forceinline__ float fix_scale(int k, float extent, float inv_m) {
   float ri;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(ri) : "f"(radius + 1.f));
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(ri) : "f"(extent + 1.f));
   const int e = fix_exp(k);
   float s = __fmul_rn(__fmul_rn(inv_m, ri), ri);
   if (e >= 3) s = __fmul_rn(s, ri);
@@ -98,7 +107,7 @@ struct GeomView {
   CamConst* cam;
   float4* rec;         // [3P] one 48-byte splat record per Gaussian, array of structures (the blend kernels gather it by id):
                        //   [0] x, y, A', B'      [1] C', opacity, cull threshold', id (bits)      (conic in the log2 domain:
-                       //   [2] r, g, b, radius                                                     power*log2e = A'dx^2+B'dxdy+C'dy^2)
+                       //   [2] r, g, b, fix_extent                                                 power*log2e = A'dx^2+B'dxdy+C'dy^2)
   float4* brec;        // [P] binning record: depth, rect x (rx0 | rx1<<16), rect y (ry0 | ry1<<16), keep mask (bits)
   uint32_t* tiles;     // tile instances per Gaussian (after culling)
   uint8_t* clamped;

@@ -411,7 +411,7 @@ k_preprocess(InPtrs in, GeomView gv, int* __restrict__ radii) {
     const uint32_t c = visit_tiles_coop(coop, sr_, cam->W, cam->H, cam->gx, cull, sink, 0ull);
     if (coop) ntiles = c;
   }
-  // ---- outputs.  The 48-byte splat record (rows x,y,A',B' | C',o,qthr',id | r,g,b,radius; conic pre-scaled into the log2
+  // ---- outputs.  The 48-byte splat record (rows x,y,A',B' | C',o,qthr',id | r,g,b,extent; conic pre-scaled into the log2
   // domain: power*log2(e) = A' dx^2 + B' dx dy + C' dy^2) is what the blend kernels gather by id, so it is stored as an
   // array of structures -- transposed through shared memory so that the CTA's 128 x 48 B leave as one contiguous block
   // of 128-bit stores.  The binning record (depth, tile rect, keep mask) is a plain coalesced float4 array.
@@ -420,7 +420,7 @@ k_preprocess(InPtrs in, GeomView gv, int* __restrict__ radii) {
   if (active) {
     sm4[3 * t + 0] = make_float4(p.x, p.y, -0.5f * kLog2e * p.A, -kLog2e * p.B);
     sm4[3 * t + 1] = make_float4(-0.5f * kLog2e * p.C, p.opacity, 0.5f * kLog2e * qthr, __uint_as_float((uint32_t)i));
-    sm4[3 * t + 2] = make_float4(p.rgb[0], p.rgb[1], p.rgb[2], (float)p.radius);
+    sm4[3 * t + 2] = make_float4(p.rgb[0], p.rgb[1], p.rgb[2], fix_extent(p.radius, p.x, p.y, cam->W, cam->H));
     gv.brec[i] = make_float4(p.depth, __uint_as_float((uint32_t)p.rx0 | ((uint32_t)p.rx1 << 16)),
                              __uint_as_float((uint32_t)p.ry0 | ((uint32_t)p.ry1 << 16)), __uint_as_float(kmask));
     gv.tiles[i] = ntiles;
@@ -487,15 +487,15 @@ k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out
   float* row_rest = sm + kSmSh + sr.rest_off + sr.rest_stride * t;
   bool has = false;
   if (t < nv) {
-    // the record (and its radius) is only written for Gaussians that cover a tile; the others have no moments
+    // the record (and its extent) is only read for Gaussians that cover a tile; the others have no moments
     float ds[kDaccSlots];
 #pragma unroll
     for (int k = 0; k < kDaccSlots; ++k) ds[k] = 0.f;
     if (gv.tiles[i] > 0) {
       const unsigned long long* acc = gv.dacc + (size_t)i * kDaccSlots;
-      const float radius = gv.rec[3 * (size_t)i + 2].w, inv_m = fix_inv_m(gv.dscale);
-      const double unit[3] = {1.0 / (double)fix_scale(5, radius, inv_m), 1.0 / (double)fix_scale(0, radius, inv_m),
-                              1.0 / (double)fix_scale(2, radius, inv_m)};      // exponents 2, 3, 4
+      const float extent = gv.rec[3 * (size_t)i + 2].w, inv_m = fix_inv_m(gv.dscale);
+      const double unit[3] = {1.0 / (double)fix_scale(5, extent, inv_m), 1.0 / (double)fix_scale(0, extent, inv_m),
+                              1.0 / (double)fix_scale(2, extent, inv_m)};      // exponents 2, 3, 4
 #pragma unroll
       for (int k = 0; k < kDaccSlots; ++k) ds[k] = fix_decode(acc[k], unit[fix_exp(k) - 2]);
     }
