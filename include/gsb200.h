@@ -17,6 +17,11 @@
  *                                     utils/pose_utils.py:57-104 (quad2rotation / quadmultiply) that
  *                                     yields gaussians.P.grad.
  *   gsb_mark_visible              ->  _C.mark_visible (GaussianRasterizer.markVisible).
+ *   gsb_preprocess_ex / _backward_ex, gsb_mip_filter3d
+ *                                 ->  Mip-Splatting (Yu et al., CVPR 2024), listed as a TODO in the reference's
+ *                                     README.md:31-34: the 2D Mip filter (GaussianRasterizationSettings.kernel_size)
+ *                                     and the 3D smoothing filter (GaussianModel.compute_3D_filter,
+ *                                     get_scaling_with_3D_filter / get_opacity_with_3D_filter).  DESIGN.md 4.7.
  *   gsb_ssim_forward/backward     ->  fused_ssim.fused_ssim, train.py:39-43,172-173
  *                                     (fallback utils/loss_utils.py:55-85).
  *   gsb_loss_forward/backward     ->  train.py:171-176: l1_loss (utils/loss_utils.py:39-40) + SSIM +
@@ -128,6 +133,38 @@ GSB_API uint32_t* gsb_status_device(void* geom, int32_t P);
 /* Backward of gsb_preprocess + gsb_render (same R as given to gsb_render).  dL_dout [3,H,W]. */
 GSB_API int gsb_backward(const GsbCamera* cam, const GsbGaussians* g, void* geom, void* binning, int64_t R,
                  void* image, const float* dL_dout, const GsbGrads* grads, gsb_stream_t stream);
+
+/* Mip-Splatting filters (DESIGN.md section 4.7).  A NULL GsbFilter is the reference path.
+ * flags & GSB_FILTER_MIP2D: the 2D Mip filter, kernel_size * I replaces the 0.3 px^2 dilation of the screen-space
+ *   covariance and the opacity is multiplied by sqrt(max(2.5e-5, det(cov2D) / det(cov2D + kernel_size I))).
+ *   (kernel_size 0.3 is the upstream rasterizer's later `antialiasing` mode.)
+ * filter3D ([P], or NULL): the 3D smoothing filter, raw_params only: scale s -> sqrt(s^2 + f^2) before
+ *   scale_modifier, opacity * prod_k s_k / sqrt(s_k^2 + f^2).  f is a constant: it receives no gradient.
+ * The record opacity every later stage reads (cull threshold, tile keep mask, 1/255 cutoff, blend) is the filtered one. */
+#define GSB_FILTER_MIP2D 1
+typedef struct GsbFilter {
+  float kernel_size;
+  int32_t flags;
+  const float* filter3D;
+} GsbFilter;
+
+/* gsb_preprocess / gsb_backward with filters; those two are these with filt = NULL.  Like cam and g, the same filter
+ * must be passed to a forward and its backward.  With GSB_FILTER_MIP2D a pose-only backward takes the full 9-value
+ * blend backward (the filtered opacity depends on the pose). */
+GSB_API int gsb_preprocess_ex(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, void* geom,
+                              size_t geom_bytes, int32_t* radii, uint32_t* status_host, gsb_stream_t stream);
+GSB_API int gsb_backward_ex(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, void* geom,
+                            void* binning, int64_t R, void* image, const float* dL_dout, const GsbGrads* grads,
+                            gsb_stream_t stream);
+
+/* Size of the 3D smoothing filter (Mip-Splatting's GaussianModel.compute_3D_filter) from the training views' pose
+ * table: poses7 [n_views, 7] (the rows gsb_preprocess takes as GsbGaussians.pose, p = R x + t), xyz [P, 3] world
+ * points, one shared intrinsics (width, height, tanfovx, tanfovy).  A view counts for a point when p_z > 0.2 and
+ * its projection lies in the frame widened by 15 % on every side; d = the smallest p_z over the views that count
+ * (points no view counts for take the largest d found); out [P] = d / fx * sqrt(0.2).  Deterministic (min / max
+ * reductions only). */
+GSB_API int gsb_mip_filter3d(int32_t P, const float* xyz, int32_t n_views, const float* poses7, int32_t width,
+                             int32_t height, float tanfovx, float tanfovy, float* out, gsb_stream_t stream);
 
 GSB_API int gsb_mark_visible(int32_t P, const float* means3D, const float* viewmatrix,
                      const float* projmatrix, uint8_t* present, gsb_stream_t stream);

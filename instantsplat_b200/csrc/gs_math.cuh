@@ -90,12 +90,26 @@ GS_HD void pose_grad_finalize(const float* pose, const float* acc, float* dpose)
   dpose[4] = acc[4]; dpose[5] = acc[5]; dpose[6] = acc[6];
 }
 
+// Mip-Splatting filters (DESIGN.md section 4.7).  on2d: the 2D Mip filter, kappa * I replaces the 0.3 px^2 dilation and
+// the opacity is compensated by h2 = sqrt(max(kMipH2Min, det(Sigma2) / det(Sigma2 + kappa I))).  on3d: the 3D
+// smoothing filter of size f (world units, raw parameters only): s~ = sqrt(s^2 + f^2), opacity * prod_k s_k / s~_k.
+// Mip() (on == 0) is the reference path, operation for operation.
+constexpr float kMipH2Min = 2.5e-5f;
+struct Mip {
+  int on = 0, on2d = 0, on3d = 0;
+  float kappa = 0.f, f = 0.f;
+};
+
 // Everything the forward produces for one Gaussian, plus what the backward re-derives from.
 struct Proj {
   int visible;
   float x, y;              // pixel-centre coordinates
   float A, B, C;           // conic
-  float opacity;           // activated
+  float opacity;           // activated; with a Mip filter the record opacity o_eff = o3 * h2
+  float sig;               // activated opacity before the filters (filters on only)
+  float o3, h2, h3;        // o3 = sig * h3; h2, h3 the 2D / 3D compensations (1 when off)
+  float a0, c0, det0;      // undilated cov2D diagonal and determinant (2D filter)
+  int h2clamp;             // 1: h2 sits at its floor, no gradient through it
   float depth;             // view-space z
   float rgb[3];
   unsigned clamped;        // bit c set: channel c was clamped at 0
@@ -195,9 +209,13 @@ GS_HD void sh_to_rgb_bwd(int D, const float* sh_rest, float x, float y, float z,
   ddir[0] = gx; ddir[1] = gy; ddir[2] = gz;
 }
 
-// Geometry part of the forward (Appendix A.2 steps 1-7).  cov3D_pre: 6 floats or nullptr.
-GS_HD void project_geometry(const CamConst& c, const GaussIn& in, const float* cov3D_pre, Proj& o) {
+// Geometry part of the forward (Appendix A.2 steps 1-7).  cov3D_pre: 6 floats or nullptr; mf: the Mip filters, read
+// only by the kMip instantiation (kMip == false compiles the reference arithmetic and nothing else).
+template <bool kMip = false>
+GS_HD void project_geometry(const CamConst& c, const GaussIn& in, const float* cov3D_pre, Proj& o,
+                            const Mip mf = Mip()) {
   o.visible = 0; o.radius = 0; o.rx0 = o.ry0 = o.rx1 = o.ry1 = 0; o.clamped = 0;
+  if constexpr (kMip) { o.h2 = o.h3 = 1.f; o.h2clamp = 0; }
   // ---- fused pose pre-transform + activations
   if (c.pose_on) {
     o.mc[0] = c.Rc[0] * in.m[0] + c.Rc[1] * in.m[1] + c.Rc[2] * in.m[2] + c.tc[0];
@@ -213,7 +231,18 @@ GS_HD void project_geometry(const CamConst& c, const GaussIn& in, const float* c
     o.mc[0] = in.m[0]; o.mc[1] = in.m[1]; o.mc[2] = in.m[2];
     o.q[0] = in.q[0]; o.q[1] = in.q[1]; o.q[2] = in.q[2]; o.q[3] = in.q[3];
   }
-  if (c.raw_params) {
+  if (kMip && c.raw_params && mf.on3d) {                // kMip == false: folded away at compile time
+    const float f2 = mf.f * mf.f;
+    float r = 1.f;                                 // prod_k s_k^2 / (s_k^2 + f^2), one bounded factor at a time
+    for (int k = 0; k < 3; ++k) {
+      const float s = expf(in.sc[k]), v = s * s + f2;
+      o.s[k] = c.scale_mod * sqrtf(v);
+      r *= (s * s) / v;
+    }
+    o.sig = sigmoidf_(in.op);
+    o.h3 = sqrtf(r);
+    o.opacity = o.sig * o.h3;
+  } else if (c.raw_params) {
     o.s[0] = c.scale_mod * expf(in.sc[0]); o.s[1] = c.scale_mod * expf(in.sc[1]);
     o.s[2] = c.scale_mod * expf(in.sc[2]);
     o.opacity = sigmoidf_(in.op);
@@ -221,6 +250,7 @@ GS_HD void project_geometry(const CamConst& c, const GaussIn& in, const float* c
     o.s[0] = c.scale_mod * in.sc[0]; o.s[1] = c.scale_mod * in.sc[1]; o.s[2] = c.scale_mod * in.sc[2];
     o.opacity = in.op;
   }
+  if (kMip && mf.on) { if (!(c.raw_params && mf.on3d)) o.sig = o.opacity; o.o3 = o.opacity; }
   const float* m = o.mc;
   // ---- view / clip transforms
   float tx = m[0] * c.V[0] + m[1] * c.V[4] + m[2] * c.V[8] + c.V[12];
@@ -269,11 +299,27 @@ GS_HD void project_geometry(const CamConst& c, const GaussIn& in, const float* c
                  S[2] * T[0] + S[4] * T[1] + S[5] * T[2]};
   float u1[3] = {S[0] * T[3] + S[1] * T[4] + S[2] * T[5], S[1] * T[3] + S[3] * T[4] + S[4] * T[5],
                  S[2] * T[3] + S[4] * T[4] + S[5] * T[5]};
-  o.a = T[0] * u0[0] + T[1] * u0[1] + T[2] * u0[2] + 0.3f;
-  o.b = T[0] * u1[0] + T[1] * u1[1] + T[2] * u1[2];
-  o.c = T[3] * u1[0] + T[4] * u1[1] + T[5] * u1[2] + 0.3f;
+  const bool mip2d = kMip && mf.on2d;
+  if (mip2d) {
+    o.a0 = T[0] * u0[0] + T[1] * u0[1] + T[2] * u0[2];
+    o.b = T[0] * u1[0] + T[1] * u1[1] + T[2] * u1[2];
+    o.c0 = T[3] * u1[0] + T[4] * u1[1] + T[5] * u1[2];
+    o.a = o.a0 + mf.kappa;
+    o.c = o.c0 + mf.kappa;
+  } else {
+    o.a = T[0] * u0[0] + T[1] * u0[1] + T[2] * u0[2] + 0.3f;
+    o.b = T[0] * u1[0] + T[1] * u1[1] + T[2] * u1[2];
+    o.c = T[3] * u1[0] + T[4] * u1[1] + T[5] * u1[2] + 0.3f;
+  }
   o.det = o.a * o.c - o.b * o.b;
   if (o.det == 0.0f) return;                                      // A.2.4
+  if (mip2d) {
+    o.det0 = o.a0 * o.c0 - o.b * o.b;
+    const float r = o.det0 / o.det;
+    o.h2clamp = !(r > kMipH2Min);
+    o.h2 = sqrtf(fmaxf(kMipH2Min, r));
+    o.opacity = o.o3 * o.h2;
+  }
   float det_inv = 1.f / o.det;
   o.A = o.c * det_inv; o.B = -o.b * det_inv; o.C = o.a * det_inv;
   float mid = 0.5f * (o.a + o.c);
@@ -294,6 +340,23 @@ GS_HD void project_geometry(const CamConst& c, const GaussIn& in, const float* c
   if ((o.rx1 - o.rx0) * (o.ry1 - o.ry0) == 0) return;
   o.radius = (int)rad;
   o.visible = 1;
+}
+
+// Size of the 3D smoothing filter (DESIGN.md section 4.7): f = d / fx_max * sqrt(0.2), d the smallest depth over the
+// training views that count for the Gaussian.  A view (rotation R row-major, translation t: p = R x + t, the transform the
+// fused preprocess applies to a pose row) counts when p_z > 0.2 and the projection lies in the frame widened by 15 %.
+constexpr float kMipMargin = 0.15f;
+constexpr float kMipSqrtVar = 0.44721359549995794f;   // sqrt(0.2)
+// p_z when the view counts for world point x, else -1
+GS_HD float mip_view_depth(const float* R, const float* t, const float* x, float fx, float fy, int W, int H) {
+  const float pz = R[6] * x[0] + R[7] * x[1] + R[8] * x[2] + t[2];
+  if (!(pz > kNear)) return -1.f;
+  const float px = R[0] * x[0] + R[1] * x[1] + R[2] * x[2] + t[0];
+  const float py = R[3] * x[0] + R[4] * x[1] + R[5] * x[2] + t[1];
+  const float u = px / pz * fx + 0.5f * W, v = py / pz * fy + 0.5f * H;
+  const bool in = u >= -kMipMargin * W && u <= (1.f + kMipMargin) * W && v >= -kMipMargin * H &&
+                  v <= (1.f + kMipMargin) * H;
+  return in ? pz : -1.f;
 }
 
 // Colour part (A.2.8).  Uses the mean handed to the rasterizer and campos.
@@ -411,9 +474,10 @@ struct GaussGrad {
   float dcolor[3];      // dL/drgb after the clamp mask (colors_precomp path)
 };
 
+template <bool kMip = false>
 GS_HD void project_bwd(const CamConst& c, const GaussIn& in, const Proj& p, const float* sh_rest,
                        bool use_sh, bool cov_pre, const float* ds, GaussGrad& g, float* d_sh_dc,
-                       float* d_sh_rest, float* pose_acc) {
+                       float* d_sh_rest, float* pose_acc, const Mip mf = Mip()) {
   float dmc[3] = {0.f, 0.f, 0.f};
   // ---- colour
   float dL[3] = {ds[6], ds[7], ds[8]};
@@ -438,6 +502,13 @@ GS_HD void project_bwd(const CamConst& c, const GaussIn& in, const Proj& p, cons
   float dL_da = d2i * (-cc * cc * dA + b * cc * dB - b * b * dC);
   float dL_dc = d2i * (-a * a * dC + a * b * dB - b * b * dA);
   float dL_db = d2i * (2.f * b * cc * dA - (det + 2.f * b * b) * dB + 2.f * a * b * dC);
+  if (kMip && mf.on2d && !p.h2clamp) {
+    // o_eff = o3 h2, h2 = sqrt(r), r = det0 / det: dL/dr = dL/do_eff * o3 / (2 h2), chained to (a0, b, c0)
+    const float dr = ds[5] * p.o3 * 0.5f / p.h2, i2 = dr / (det * det);
+    dL_da += (p.c0 * det - p.det0 * cc) * i2;
+    dL_dc += (p.a0 * det - p.det0 * a) * i2;
+    dL_db += -2.f * b * (det - p.det0) * i2;
+  }
   // ---- cov2D = T Sigma T^T
   const float* T = p.T;
   const float* S = p.Sig;
@@ -502,7 +573,23 @@ GS_HD void project_bwd(const CamConst& c, const GaussIn& in, const Proj& p, cons
   }
   // ---- activations
   float dop = ds[5];
-  if (c.raw_params) {
+  if (kMip && mf.on) {
+    // o_eff = sig * h3 * h2 (h3 = prod_k s_k / s~_k with the 3D filter, else 1); neither filter's f or kappa is trained
+    const float dsig = dop * p.h2 * p.h3;
+    if (c.raw_params && mf.on3d) {
+      // o.s = mod * s~, s~^2 = s^2 + f^2, s = exp(sc):  d(mod s~)/dsc = o.s * s^2 / s~^2,  dh3/dsc = h3 f^2 / s~^2
+      const float f2 = mf.f * mf.f, dh3 = dop * p.h2 * p.sig * p.h3;
+      for (int k = 0; k < 3; ++k) {
+        const float s = expf(in.sc[k]), v = s * s + f2;
+        g.dsc[k] = dsc[k] * p.s[k] * ((s * s) / v) + dh3 * (f2 / v);
+      }
+    } else if (c.raw_params) {
+      g.dsc[0] = dsc[0] * p.s[0]; g.dsc[1] = dsc[1] * p.s[1]; g.dsc[2] = dsc[2] * p.s[2];
+    } else {
+      g.dsc[0] = dsc[0] * c.scale_mod; g.dsc[1] = dsc[1] * c.scale_mod; g.dsc[2] = dsc[2] * c.scale_mod;
+    }
+    g.dop = c.raw_params ? dsig * p.sig * (1.f - p.sig) : dsig;
+  } else if (c.raw_params) {
     // s = mod * exp(sc): ds/dsc = s ; (dsc[] currently holds dL/ds)
     g.dsc[0] = dsc[0] * p.s[0]; g.dsc[1] = dsc[1] * p.s[1]; g.dsc[2] = dsc[2] * p.s[2];
     g.dop = dop * p.opacity * (1.f - p.opacity);

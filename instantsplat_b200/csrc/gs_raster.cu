@@ -128,7 +128,16 @@ struct InPtrs {
   int sh_packed;
   int vec_ok;       // all base pointers 16-byte aligned
   int exact_cull;
+  Mip mip;          // mip.on == 0: reference path; the 3D filter's f comes from filter3D[i]
+  const float* filter3D;
 };
+
+// this Gaussian's filters
+__device__ __forceinline__ Mip gauss_mip(const InPtrs& in, int i) {
+  Mip m = in.mip;
+  if (m.on3d) m.f = __ldg(in.filter3D + i);
+  return m;
+}
 
 // ------------------------------------------------------------------------------------------
 // k_setup_cam
@@ -328,6 +337,7 @@ __device__ __forceinline__ void read_gauss(const float* sm, int t, bool has_sr, 
 // ------------------------------------------------------------------------------------------
 // k_preprocess
 // ------------------------------------------------------------------------------------------
+template <bool kMip>
 __global__ void __launch_bounds__(kPT)
 k_preprocess(InPtrs in, GeomView gv, int* __restrict__ radii) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -351,7 +361,8 @@ k_preprocess(InPtrs in, GeomView gv, int* __restrict__ radii) {
   GaussIn g;
   read_gauss(sm, active ? t : 0, in.scales != nullptr, g);
   Proj p;
-  project_geometry(*cam, g, in.cov3D ? in.cov3D + (size_t)6 * i : nullptr, p);
+  if constexpr (kMip) project_geometry<true>(*cam, g, in.cov3D ? in.cov3D + (size_t)6 * i : nullptr, p, gauss_mip(in, i));
+  else project_geometry(*cam, g, in.cov3D ? in.cov3D + (size_t)6 * i : nullptr, p);
   if (!active) p.visible = 0;
   float qthr = -1.f;
   uint32_t ntiles = 0, kmask = 0u;
@@ -448,6 +459,7 @@ struct OutPtrs {
 #ifndef GSB_PBWD_MINB
 #define GSB_PBWD_MINB 4
 #endif
+template <bool kMip>
 __global__ void __launch_bounds__(kPT, GSB_PBWD_MINB)
 k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -507,7 +519,8 @@ k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out
       GaussIn g;
       read_gauss(sm, t, in.scales != nullptr, g);
       Proj p;
-      project_geometry(*cam, g, in.cov3D ? in.cov3D + (size_t)6 * i : nullptr, p);
+      const Mip mf = kMip ? gauss_mip(in, i) : Mip();
+      project_geometry<kMip>(*cam, g, in.cov3D ? in.cov3D + (size_t)6 * i : nullptr, p, mf);
       if (p.visible) {
         p.clamped = gv.clamped[i];
         // The blend backward accumulates RAW pixel moments of w = dL/dalpha * (opacity * G) per Gaussian
@@ -524,7 +537,7 @@ k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out
           ds[4] *= -0.5f;
           ds[5] = p.opacity > 0.f ? ds[5] / p.opacity : 0.f;     // contributing pairs have opacity >= 1/255
         }
-        project_bwd(*cam, g, p, row_rest, use_sh, in.cov3D != nullptr, ds, gg, row_dc, row_rest, pa);
+        project_bwd<kMip>(*cam, g, p, row_rest, use_sh, in.cov3D != nullptr, ds, gg, row_dc, row_rest, pa, mf);
         has = use_sh;
       }
     }
@@ -669,6 +682,20 @@ static int make_inptrs(const GsbCamera* cam, const GsbGaussians* g, InPtrs& in) 
   uintptr_t a = (uintptr_t)g->means3D | (uintptr_t)g->scales | (uintptr_t)g->rotations |
                 (uintptr_t)g->opacities | (uintptr_t)g->sh_dc | (uintptr_t)g->sh_rest;
   in.vec_ok = (a & 15) == 0;
+  in.mip = Mip(); in.filter3D = nullptr;
+  return GSB_OK;
+}
+
+// the Mip filters of GsbFilter (NULL: reference path)
+static int apply_filter(const GsbFilter* f, const GsbGaussians* g, InPtrs& in) {
+  if (!f) return GSB_OK;
+  GSB_REQUIRE((f->flags & ~GSB_FILTER_MIP2D) == 0, "GsbFilter: unknown flags");
+  const bool on2d = (f->flags & GSB_FILTER_MIP2D) != 0, on3d = f->filter3D != nullptr;
+  if (on2d) GSB_REQUIRE(f->kernel_size >= 0.f && f->kernel_size < 1.0e30f, "GsbFilter: kernel_size must be >= 0");
+  if (on3d) GSB_REQUIRE(g->raw_params && g->scales, "GsbFilter: filter3D needs raw parameters with scales");
+  in.mip.on = on2d || on3d;
+  in.mip.on2d = on2d; in.mip.on3d = on3d; in.mip.kappa = on2d ? f->kernel_size : 0.f;
+  in.filter3D = f->filter3D;
   return GSB_OK;
 }
 
@@ -678,8 +705,10 @@ static int ensure_attrs() {
   int dev = 0;
   GSB_CUDA(cudaGetDevice(&dev));
   if (dev < 0 || dev >= 64 || !done[dev]) {
-    GSB_CUDA(cudaFuncSetAttribute(k_preprocess, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPrepSmem));
-    GSB_CUDA(cudaFuncSetAttribute(k_preprocess_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPrepSmem));
+    for (auto k : {k_preprocess<false>, k_preprocess<true>})
+      GSB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPrepSmem));
+    for (auto k : {k_preprocess_bwd<false>, k_preprocess_bwd<true>})
+      GSB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPrepSmem));
     if (dev >= 0 && dev < 64) done[dev] = true;
   }
   return GSB_OK;
@@ -695,11 +724,14 @@ static CamArgs cam_args(const GsbCamera* cam, const GsbGaussians* g) {
   return a;
 }
 
-extern "C" GSB_API int gsb_preprocess(const GsbCamera* cam, const GsbGaussians* g, void* geom, size_t geom_bytes,
-                              int32_t* radii, uint32_t* status_host, gsb_stream_t stream_) {
+extern "C" GSB_API int gsb_preprocess_ex(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt,
+                                         void* geom, size_t geom_bytes, int32_t* radii, uint32_t* status_host,
+                                         gsb_stream_t stream_) {
   cudaStream_t st = (cudaStream_t)stream_;
   InPtrs in;
   int rc = make_inptrs(cam, g, in);
+  if (rc) return rc;
+  rc = apply_filter(filt, g, in);
   if (rc) return rc;
   GSB_REQUIRE(geom && (radii || g->P == 0), "null buffer");
   const int P = g->P;
@@ -715,7 +747,7 @@ extern "C" GSB_API int gsb_preprocess(const GsbCamera* cam, const GsbGaussians* 
   if (P > 0) {
     const int nb = (P + kPT - 1) / kPT;
     ProfScope ps(GSB_K_PREPROCESS, st, 2);
-    k_preprocess<<<nb, kPT, kPrepSmem, st>>>(in, gv, radii);
+    (in.mip.on ? k_preprocess<true> : k_preprocess<false>)<<<nb, kPT, kPrepSmem, st>>>(in, gv, radii);
     rc = gsb_launch_big_rects(P, gv, nullptr, cam->width, cam->height, cam->exact_cull, 0u, st);   // count mode
     if (rc) return rc;
   }
@@ -724,6 +756,11 @@ extern "C" GSB_API int gsb_preprocess(const GsbCamera* cam, const GsbGaussians* 
   if (status_host) GSB_CUDA(cudaMemcpyAsync(status_host, gv.status, 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   GSB_CUDA(cudaGetLastError());
   return GSB_OK;
+}
+
+extern "C" GSB_API int gsb_preprocess(const GsbCamera* cam, const GsbGaussians* g, void* geom, size_t geom_bytes,
+                                      int32_t* radii, uint32_t* status_host, gsb_stream_t stream) {
+  return gsb_preprocess_ex(cam, g, nullptr, geom, geom_bytes, radii, status_host, stream);
 }
 
 extern "C" GSB_API int gsb_render(const GsbCamera* cam, int32_t P, void* geom, void* binning, size_t binning_bytes,
@@ -745,11 +782,14 @@ extern "C" GSB_API int gsb_render(const GsbCamera* cam, int32_t P, void* geom, v
   return GSB_OK;
 }
 
-extern "C" GSB_API int gsb_backward(const GsbCamera* cam, const GsbGaussians* g, void* geom, void* binning, int64_t R,
-                            void* image, const float* dL_dout, const GsbGrads* grads, gsb_stream_t stream_) {
+extern "C" GSB_API int gsb_backward_ex(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, void* geom,
+                                       void* binning, int64_t R, void* image, const float* dL_dout, const GsbGrads* grads,
+                                       gsb_stream_t stream_) {
   cudaStream_t st = (cudaStream_t)stream_;
   InPtrs in;
   int rc = make_inptrs(cam, g, in);
+  if (rc) return rc;
+  rc = apply_filter(filt, g, in);
   if (rc) return rc;
   GSB_REQUIRE(geom && binning && image && dL_dout && grads, "null buffer");
   if (g->pose) GSB_REQUIRE(grads->dL_dpose != nullptr, "dL_dpose required when pose is fused");
@@ -765,8 +805,9 @@ extern "C" GSB_API int gsb_backward(const GsbCamera* cam, const GsbGaussians* g,
   }
   GSB_CUDA(cudaMemsetAsync(gv.dacc, 0, (size_t)P * kDaccSlots * 8, st));
   GSB_CUDA(cudaMemsetAsync(gv.dscale, 0, 4, st));
-  // tracking mode (render.py:99-170): only dL/dpose is wanted -> the blend backward reduces 8 values instead of 9
-  const bool pose_only = g->pose && grads->dL_dpose && !grads->dL_dmeans3D && !grads->dL_dmeans2D && !grads->dL_dscales &&
+  // tracking mode (render.py:99-170): only dL/dpose is wanted -> the blend backward reduces 8 values instead of 9.
+  // Not with the 2D Mip filter: o_eff depends on Sigma2 and so on the pose, whose gradient then needs S w (slot 5).
+  const bool pose_only = !in.mip.on2d && g->pose && grads->dL_dpose && !grads->dL_dmeans3D && !grads->dL_dmeans2D && !grads->dL_dscales &&
                          !grads->dL_drotations && !grads->dL_dopacities && !grads->dL_dsh_dc && !grads->dL_dsh_rest &&
                          !grads->dL_dcolors && !grads->dL_dcov3D && gsb_option_blend_version() == 2 &&
                          gsb_option_stage_bulk() == 1;
@@ -781,13 +822,19 @@ extern "C" GSB_API int gsb_backward(const GsbCamera* cam, const GsbGaussians* g,
   if (a & 15) in.vec_ok = 0;
   const int nb = (P + kPT - 1) / kPT;
   { ProfScope ps(GSB_K_PREPROCESS_BWD, st, g->pose ? 3 : 1);
-    k_preprocess_bwd<<<nb, kPT, kPrepSmem, st>>>(in, gv, pose_only ? 1 : 0, out);
+    (in.mip.on ? k_preprocess_bwd<true> : k_preprocess_bwd<false>)<<<nb, kPT, kPrepSmem, st>>>(in, gv, pose_only ? 1 : 0,
+                                                                                             out);
     if (g->pose) {
       k_pose_reduce<<<16, 256, 0, st>>>(gv.pose_part, nb, gv.pose_acc);
       k_pose_finalize<<<1, 32, 0, st>>>(gv.pose_acc, g->pose, grads->dL_dpose);
     } }
   GSB_CUDA(cudaGetLastError());
   return GSB_OK;
+}
+
+extern "C" GSB_API int gsb_backward(const GsbCamera* cam, const GsbGaussians* g, void* geom, void* binning, int64_t R,
+                                    void* image, const float* dL_dout, const GsbGrads* grads, gsb_stream_t stream) {
+  return gsb_backward_ex(cam, g, nullptr, geom, binning, R, image, dL_dout, grads, stream);
 }
 
 extern "C" GSB_API int gsb_mark_visible(int32_t P, const float* means3D, const float* viewmatrix,

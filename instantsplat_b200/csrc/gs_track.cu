@@ -9,6 +9,8 @@
 //                         render.py:146-151 -- all by one thread, from device-resident inputs
 #include "gs_internal.cuh"
 
+using namespace gsb;
+
 namespace {
 
 constexpr int kLT = 256;
@@ -87,7 +89,72 @@ __global__ void k_track_step(TrackArgs a) {
   }
 }
 
+// ---- size of the 3D smoothing filter (DESIGN.md section 4.7) -------------------------------------------------------
+// Pass 1: one thread per Gaussian, the views staged in shared memory kMV at a time as (R row-major, t):
+// out[i] = smallest p_z over the views that count, -1 when none does.
+constexpr int kMV = 256;
+__global__ void __launch_bounds__(kLT) k_mip_depth(int P, const float* __restrict__ xyz, int V,
+                                                   const float* __restrict__ poses7, float fx, float fy, int W, int H,
+                                                   float* __restrict__ out) {
+  __shared__ float s_v[kMV][12];
+  const int i = blockIdx.x * kLT + threadIdx.x;
+  float x[3] = {0.f, 0.f, 0.f};
+  if (i < P) { x[0] = xyz[3 * (size_t)i]; x[1] = xyz[3 * (size_t)i + 1]; x[2] = xyz[3 * (size_t)i + 2]; }
+  float d = 3.0e38f;
+  for (int v0 = 0; v0 < V; v0 += kMV) {
+    const int nv = min(kMV, V - v0);
+    __syncthreads();
+    for (int v = threadIdx.x; v < nv; v += kLT) {
+      const float* q = poses7 + 7 * (size_t)(v0 + v);
+      const float n = sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+      quat_to_R(q[0] / n, q[1] / n, q[2] / n, q[3] / n, s_v[v]);
+      s_v[v][9] = q[4]; s_v[v][10] = q[5]; s_v[v][11] = q[6];
+    }
+    __syncthreads();
+    for (int v = 0; v < nv; ++v) {
+      const float z = mip_view_depth(s_v[v], s_v[v] + 9, x, fx, fy, W, H);
+      if (z >= 0.f) d = fminf(d, z);
+    }
+  }
+  if (i < P) out[i] = d < 3.0e38f ? d : -1.f;
+}
+
+// Pass 2 (one CTA; a max is exact in any order, so the result is deterministic): Gaussians no view counts for take the
+// largest depth found, then f = d / fx * sqrt(0.2).  When no Gaussian is seen at all, f = 0 (no filter).
+constexpr int kMF = 1024;
+__global__ void __launch_bounds__(kMF) k_mip_finish(int P, float fx, float* __restrict__ out) {
+  __shared__ float red[kMF / 32];
+  float m = -1.f;
+  for (int i = threadIdx.x; i < P; i += kMF) m = fmaxf(m, out[i]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  m = red[0];
+  for (int w = 1; w < kMF / 32; ++w) m = fmaxf(m, red[w]);
+  for (int i = threadIdx.x; i < P; i += kMF) {
+    const float d = out[i] >= 0.f ? out[i] : m;
+    out[i] = d >= 0.f ? d / fx * kMipSqrtVar : 0.f;
+  }
+}
+
 }  // namespace
+
+extern "C" GSB_API int gsb_mip_filter3d(int32_t P, const float* xyz, int32_t n_views, const float* poses7,
+                                        int32_t width, int32_t height, float tanfovx, float tanfovy, float* out,
+                                        gsb_stream_t stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  GSB_REQUIRE(P >= 0 && n_views >= 0 && width > 0 && height > 0 && tanfovx > 0.f && tanfovy > 0.f,
+              "gsb_mip_filter3d: bad argument");
+  if (P == 0) return GSB_OK;
+  GSB_REQUIRE(xyz && out && (poses7 || n_views == 0), "gsb_mip_filter3d: null buffer");
+  const float fx = width / (2.0f * tanfovx), fy = height / (2.0f * tanfovy);
+  gsb_count_launch(2);
+  k_mip_depth<<<(P + kLT - 1) / kLT, kLT, 0, st>>>(P, xyz, n_views, poses7, fx, fy, width, height, out);
+  k_mip_finish<<<1, kMF, 0, st>>>(P, fx, out);
+  GSB_CUDA(cudaGetLastError());
+  return GSB_OK;
+}
 
 extern "C" GSB_API int gsb_l1_mask_fwd_bwd(int32_t C, int32_t H, int32_t W, const float* img, const float* gt,
                                            float threshold, double* sums, float* dL_dimg, gsb_stream_t stream_) {

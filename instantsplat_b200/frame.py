@@ -13,7 +13,7 @@ import math
 import torch
 
 from . import _lib
-from ._lib import GsbCamera, GsbGaussians, check
+from ._lib import FILTER_MIP2D, GsbCamera, GsbFilter, GsbGaussians, check
 
 # the status words of a forward (kSt* of csrc/gs_internal.cuh); the library writes them as uint32
 ST_R, ST_OVERFLOW, ST_MAX_LIST, ST_HUGE_TILES, ST_NLARGE, ST_NHUGE, ST_SEQ = range(7)
@@ -82,6 +82,35 @@ def gaussians(P, xyz, rotation, scaling, opacity, f_dc, f_rest, pose, raw_params
     return g
 
 
+def mip_filter(kernel_size=None, filter3D=None):
+    """GsbFilter of the Mip-Splatting filters (DESIGN.md section 4.7), or None (the reference path) when both are off.
+    kernel_size: the 2D Mip filter's dilation (Mip-Splatting uses 0.1); filter3D: contiguous fp32 [P] device tensor of
+    3D smoothing filter sizes (raw parameters only).  The tensor must stay alive while the filter is in use."""
+    if kernel_size is None and filter3D is None:
+        return None
+    f = GsbFilter()
+    if kernel_size is not None:
+        f.kernel_size, f.flags = float(kernel_size), FILTER_MIP2D
+    f.filter3D = _p(filter3D)
+    return f
+
+
+def mip_filter3d(xyz, poses7, W, H, tanfovx, tanfovy, out=None) -> torch.Tensor:
+    """Size of the 3D smoothing filter [P] from world points xyz [P, 3] and the training views' pose table
+    poses7 [V, 7] with one shared intrinsics (gsb_mip_filter3d); written into `out` when given."""
+    xyz, poses7 = xyz.detach().float().contiguous(), poses7.detach().float().contiguous()
+    if out is None:
+        out = torch.empty(xyz.shape[0], dtype=torch.float32, device=xyz.device)
+    check(_lib.lib().gsb_mip_filter3d(xyz.shape[0], xyz.data_ptr(), poses7.shape[0], poses7.data_ptr(), int(W), int(H),
+                                      float(tanfovx), float(tanfovy), out.data_ptr(), _lib.stream_ptr()),
+          "gsb_mip_filter3d")
+    return out
+
+
+def _f(filt):
+    return None if filt is None else ctypes.byref(filt)
+
+
 class Frame:
     """Scratch of forwards at one (device, P, W, H): the geometry buffer (which holds the status words), radii, the
     image buffer, the rendered colour [3, H, W], and a binning buffer of `cap` instances (0: none yet).
@@ -114,19 +143,21 @@ class Frame:
         self.binning = torch.empty(nbytes, dtype=torch.uint8, device=self.geom.device)
         self.cap = cap
 
-    def preprocess(self, cam, g, host_status=None) -> None:
-        check(_lib.lib().gsb_preprocess(ctypes.byref(cam), ctypes.byref(g), self.geom.data_ptr(), self.geom.numel(),
-                                        self.radii.data_ptr(), _p(host_status), _lib.stream_ptr()), "gsb_preprocess")
+    def preprocess(self, cam, g, host_status=None, filt=None) -> None:
+        """filt: mip_filter(...) or None; pass the same one to the backward."""
+        check(_lib.lib().gsb_preprocess_ex(ctypes.byref(cam), ctypes.byref(g), _f(filt), self.geom.data_ptr(),
+                                           self.geom.numel(), self.radii.data_ptr(), _p(host_status),
+                                           _lib.stream_ptr()), "gsb_preprocess")
 
     def render(self, cam, host_status=None) -> None:
         check(_lib.lib().gsb_render(ctypes.byref(cam), self.P, self.geom.data_ptr(), self.binning.data_ptr(),
                                     self.binning.numel(), self.cap, self.image.data_ptr(), self.color.data_ptr(),
                                     _p(host_status), _lib.stream_ptr()), "gsb_render")
 
-    def backward(self, cam, g, dL_dimage, grads) -> None:
-        check(_lib.lib().gsb_backward(ctypes.byref(cam), ctypes.byref(g), self.geom.data_ptr(), self.binning.data_ptr(),
-                                      self.cap, self.image.data_ptr(), dL_dimage.data_ptr(), ctypes.byref(grads),
-                                      _lib.stream_ptr()), "gsb_backward")
+    def backward(self, cam, g, dL_dimage, grads, filt=None) -> None:
+        check(_lib.lib().gsb_backward_ex(ctypes.byref(cam), ctypes.byref(g), _f(filt), self.geom.data_ptr(),
+                                         self.binning.data_ptr(), self.cap, self.image.data_ptr(), dL_dimage.data_ptr(),
+                                         ctypes.byref(grads), _lib.stream_ptr()), "gsb_backward")
 
     def blend_stats(self, cam, dL_dimage, stats) -> None:
         check(_lib.lib().gsb_blend_stats(ctypes.byref(cam), self.P, self.geom.data_ptr(), self.binning.data_ptr(),

@@ -57,6 +57,8 @@ class GaussianModel:
         self.spatial_lr_scale = 0
         self.per_point_lr = None
         self.P = None
+        self.filter_3D = None           # Mip-Splatting's 3D smoothing filter [P, 1] (DESIGN.md section 4.7), a constant
+        self._filter_cams = None
 
     # ---- activations (reference :101-121) ----------------------------------------------------
     get_xyz = property(lambda s: s._xyz)
@@ -64,6 +66,33 @@ class GaussianModel:
     get_rotation = property(lambda s: torch.nn.functional.normalize(s._rotation))
     get_opacity = property(lambda s: torch.sigmoid(s._opacity))
     get_features = property(lambda s: torch.cat((s._features_dc, s._features_rest), dim=1))
+
+    # ---- Mip-Splatting's 3D smoothing filter (same names as its gaussian_model.py) ------------
+    @property
+    def get_scaling_with_3D_filter(self):
+        return torch.sqrt(torch.square(self.get_scaling) + torch.square(self.filter_3D))
+
+    @property
+    def get_opacity_with_3D_filter(self):
+        s2 = torch.square(self.get_scaling)
+        coef = torch.sqrt(s2.prod(dim=1) / (s2 + torch.square(self.filter_3D)).prod(dim=1))
+        return self.get_opacity * coef[..., None]
+
+    @torch.no_grad()
+    def compute_3D_filter(self, cameras):
+        """filter_3D from the training views' current poses (self.P, one row per camera) and their shared intrinsics
+        (FoVx, FoVy, image_width, image_height), computed by gsb_mip_filter3d.  The cameras are remembered so that
+        densification_postfix can recompute the filter for the new rows."""
+        from .frame import mip_filter3d
+        c0 = cameras[0]
+        intr = lambda c: (int(c.image_width), int(c.image_height), float(c.FoVx), float(c.FoVy))
+        if any(intr(c) != intr(c0) for c in cameras):
+            raise ValueError("compute_3D_filter: the training views must share one intrinsics")
+        W, H, fovx, fovy = intr(c0)
+        f = mip_filter3d(self._xyz, self.P[:len(cameras)], W, H, math.tan(fovx * 0.5), math.tan(fovy * 0.5))
+        self.filter_3D = f[:, None]
+        self._filter_cams = list(cameras)
+        return self.filter_3D
 
     def get_covariance(self, scaling_modifier=1):
         """Upper triangle of R S S^T R^T with the NORMALISED quaternion (reference :32-36, general_utils.py:64-110)."""
@@ -200,6 +229,8 @@ class GaussianModel:
             return p.detach()[keep], st
 
         self._rebuild_groups(edit)
+        if self.filter_3D is not None:
+            self.filter_3D = self.filter_3D[keep]
         self.xyz_gradient_accum = self.xyz_gradient_accum[keep]
         self.denom = self.denom[keep]
         self.max_radii2D = self.max_radii2D[keep]
@@ -229,6 +260,15 @@ class GaussianModel:
             add = new_per_point_lr if new_per_point_lr is not None else torch.ones(new_xyz.shape[0], 1, device=self.device)
             self.per_point_lr = torch.cat((self.per_point_lr, add.to(self.device)), dim=0)
             self.optimizer.param_groups[0]["per_point_lr"] = self.per_point_lr
+        if self.filter_3D is not None:
+            if self._filter_cams is not None:
+                self.compute_3D_filter(self._filter_cams)
+            else:
+                # filter_3D was set directly (e.g. loaded from a PLY), so there are no cameras to recompute it from: the
+                # new rows take the largest existing size, the rule for Gaussians no training view counts for
+                fill = self.filter_3D.max() if self.filter_3D.numel() else torch.zeros((), device=self.device)
+                add = fill.reshape(1, 1).expand(new_xyz.shape[0], 1).to(self.filter_3D)
+                self.filter_3D = torch.cat((self.filter_3D, add), dim=0)
 
     def reset_opacity(self):
         """opacity <- min(opacity, 0.01) in logit space, Adam moments of the opacity tensor zeroed (reference :280-283)."""

@@ -15,10 +15,10 @@ import torch.nn as nn
 
 from . import _lib
 from ._lib import GsbGrads, check, f32c, ptr
-from .frame import ST_WORDS, Frame, camera, capacity, gaussians, read_R
+from .frame import ST_WORDS, Frame, camera, capacity, gaussians, mip_filter, read_R
 
 
-class GaussianRasterizationSettings(NamedTuple):
+class _Settings(NamedTuple):
     image_height: int
     image_width: int
     tanfovx: float
@@ -31,6 +31,34 @@ class GaussianRasterizationSettings(NamedTuple):
     campos: torch.Tensor
     prefiltered: bool
     debug: bool
+
+
+class GaussianRasterizationSettings(_Settings):
+    """The upstream settings tuple (its 12 fields, positional or keyword) plus Mip-Splatting's keyword `kernel_size`:
+    the 2D Mip filter (0.1 in Mip-Splatting; 0.3 is the upstream rasterizer's later `antialiasing` mode), None for the
+    reference's 0.3 px^2 dilation.  DESIGN.md section 4.7.  It is an attribute, not a tuple field, so the tuple
+    stays the one upstream callers build and unpack."""
+
+    def __new__(cls, *args, kernel_size: Optional[float] = None, **kw):
+        self = super().__new__(cls, *args, **kw)
+        self.kernel_size = None if kernel_size is None else float(kernel_size)
+        return self
+
+    # the namedtuple helpers, copy and pickle rebuild from the fields alone: carry kernel_size through them
+    def _replace(self, **kw):
+        ks = kw.pop("kernel_size", self.kernel_size)
+        return type(self)(*_Settings._replace(self, **kw), kernel_size=ks)
+
+    @classmethod
+    def _make(cls, iterable, kernel_size: Optional[float] = None):
+        return cls(*iterable, kernel_size=kernel_size)
+
+    def __reduce__(self):
+        return (_settings_with_kernel_size, (tuple(self), self.kernel_size))
+
+
+def _settings_with_kernel_size(fields, kernel_size):
+    return GaussianRasterizationSettings(*fields, kernel_size=kernel_size)
 
 
 EXACT_CULL = True   # lossless alpha<1/255 tile culling (set False for the reference's rect-only binning)
@@ -85,15 +113,16 @@ _BIN_ROUND = 1 << 25    # binning allocations rounded up to 32 MiB so the cachin
 
 
 def _forward(settings, means3D, scales, rotations, opacities, sh_dc, sh_rest, sh_packed, M,
-             colors_precomp, cov3D_precomp, pose, raw_params):
+             colors_precomp, cov3D_precomp, pose, raw_params, filter3D=None):
     dev = means3D.device
     if means3D.dim() != 2 or means3D.shape[1] != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")
     P = means3D.shape[0]
     W, H = int(settings.image_width), int(settings.image_height)
     keep = [f32c(t) for t in (settings.bg, settings.viewmatrix, settings.projmatrix, settings.campos, means3D,
-                              scales, rotations, opacities, sh_dc, sh_rest, colors_precomp, cov3D_precomp, pose)]
-    bg, vm, pm, cp, xyz, sca, rot, op, dc, rest, cpre, cov, pos = keep
+                              scales, rotations, opacities, sh_dc, sh_rest, colors_precomp, cov3D_precomp, pose,
+                              filter3D)]
+    bg, vm, pm, cp, xyz, sca, rot, op, dc, rest, cpre, cov, pos, f3d = keep
     cam = camera(W, H, settings.tanfovx, settings.tanfovy, settings.sh_degree, M, bg, vm, pm, cp,
                  settings.scale_modifier, EXACT_CULL)
     g = gaussians(P, xyz, rot, sca, op, dc, rest, pos, raw_params, sh_packed, cpre, cov)
@@ -101,10 +130,11 @@ def _forward(settings, means3D, scales, rotations, opacities, sh_dc, sh_rest, sh
     with torch.cuda.device(dev):
         st = _State(dev, P, W, H)
         st.cam, st.g, st.keep = cam, g, keep
+        st.filt = mip_filter(getattr(settings, "kernel_size", None), f3d)
         st.M, st.packed, st.has_pose = M, bool(sh_packed), pose is not None
         est = None if settings.debug else _last_R.get(key)
         status = _status_slot()
-        st.preprocess(cam, g, status)
+        st.preprocess(cam, g, status, st.filt)
         event = torch.cuda.Event()
         event.record()
         if est is None:
@@ -161,7 +191,7 @@ def _backward(st: _State, dL_dout, want, dev):
         t = torch.empty(7, dtype=torch.float32, device=dev)     # always required by the ABI when pose is fused
         out["pose"] = t
         gr.dL_dpose = t.data_ptr()
-    st.backward(st.cam, st.g, dL, gr)
+    st.backward(st.cam, st.g, dL, gr, st.filt)
     return out
 
 
@@ -227,13 +257,15 @@ def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales,
 
 class _RasterizeFused(torch.autograd.Function):
     """InstantSplat path with everything fused: raw model tensors + camera pose in, image out.
-    Replaces gaussian_renderer/__init__.py:81-135 and its autograd chain."""
+    Replaces gaussian_renderer/__init__.py:81-135 and its autograd chain.  filter_3D: Mip-Splatting's 3D smoothing
+    filter [P] (or [P, 1]), a constant."""
 
     @staticmethod
-    def forward(ctx, xyz, rotation, scaling, opacity, f_dc, f_rest, pose, means2D, raster_settings):
+    def forward(ctx, xyz, rotation, scaling, opacity, f_dc, f_rest, pose, means2D, raster_settings, filter_3D=None):
         M = 1 + (f_rest.shape[1] if f_rest is not None and f_rest.dim() == 3 else 0)
         color, radii, st = _forward(raster_settings, xyz, scaling, rotation, opacity.reshape(-1),
-                                    f_dc.reshape(-1, 3), f_rest if M > 1 else None, 0, M, None, None, pose, 1)
+                                    f_dc.reshape(-1, 3), f_rest if M > 1 else None, 0, M, None, None, pose, 1,
+                                    None if filter_3D is None else filter_3D.detach().reshape(-1))
         ctx.st = st
         ctx.save_for_backward(*[t for t in (xyz, rotation, scaling, opacity, f_dc, f_rest, pose) if torch.is_tensor(t)])
         ctx.shapes = (opacity.shape, f_dc.shape, None if f_rest is None else f_rest.shape)
@@ -256,11 +288,12 @@ class _RasterizeFused(torch.autograd.Function):
         g_dc = g.get("sh_dc")
         return (g.get("means3D"), g.get("rotations"), g.get("scales"),
                 None if g_op is None else g_op.reshape(osh), None if g_dc is None else g_dc.reshape(dsh), g_rest,
-                g.get("pose") if need[6] else None, g.get("means2D"), None)
+                g.get("pose") if need[6] else None, g.get("means2D"), None, None)
 
 
-def rasterize_fused(xyz, rotation, scaling, opacity, f_dc, f_rest, pose, means2D, raster_settings):
-    return _RasterizeFused.apply(xyz, rotation, scaling, opacity, f_dc, f_rest, pose, means2D, raster_settings)
+def rasterize_fused(xyz, rotation, scaling, opacity, f_dc, f_rest, pose, means2D, raster_settings, filter_3D=None):
+    return _RasterizeFused.apply(xyz, rotation, scaling, opacity, f_dc, f_rest, pose, means2D, raster_settings,
+                                 filter_3D)
 
 
 class GaussianRasterizer(nn.Module):

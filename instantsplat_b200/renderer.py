@@ -52,8 +52,12 @@ def quadmultiply(q1, q2):
                         w1 * y2 - x1 * z2 + y1 * w2 + z1 * x2, w1 * z2 + x1 * y2 - y1 * x2 + z1 * w2], dim=-1)
 
 
-def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_color=None, camera_pose=None):
-    """Render the scene.  Background tensor (bg_color) must be on GPU!"""
+def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_color=None, camera_pose=None,
+           kernel_size=None):
+    """Render the scene.  Background tensor (bg_color) must be on GPU!
+
+    kernel_size: Mip-Splatting's 2D Mip filter (None: the reference's 0.3 px^2 dilation); pc.filter_3D, when set,
+    applies its 3D smoothing filter.  DESIGN.md section 4.7."""
     xyz = pc.get_xyz
     screenspace_points = torch.zeros_like(xyz, dtype=xyz.dtype, requires_grad=True, device=xyz.device) + 0
     try:
@@ -69,13 +73,15 @@ def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_
         image_height=int(viewpoint_camera.image_height), image_width=int(viewpoint_camera.image_width),
         tanfovx=tanfovx, tanfovy=tanfovy, bg=bg_color, scale_modifier=scaling_modifier, viewmatrix=w2c,
         projmatrix=viewpoint_camera.projection_matrix, sh_degree=pc.active_sh_degree, campos=campos,
-        prefiltered=False, debug=bool(getattr(pipe, "debug", False)))
+        prefiltered=False, debug=bool(getattr(pipe, "debug", False)),
+        **({} if kernel_size is None else {"kernel_size": kernel_size}))
+    filter_3D = getattr(pc, "filter_3D", None)
     fused = (FUSED and override_color is None and not getattr(pipe, "compute_cov3D_python", False)
              and not getattr(pipe, "convert_SHs_python", False))
     if fused:
         rendered_image, radii = rasterize_fused(pc._xyz, pc._rotation, pc._scaling, pc._opacity,
                                                 pc._features_dc, pc._features_rest, camera_pose,
-                                                screenspace_points, raster_settings)
+                                                screenspace_points, raster_settings, filter_3D)
     else:
         rel_w2c = get_camera_from_tensor(camera_pose)
         gaussians_xyz, gaussians_rot = pc._xyz.clone(), pc._rotation.clone()            # reference :83-84
@@ -86,7 +92,7 @@ def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_
         if getattr(pipe, "compute_cov3D_python", False):
             cov3D_precomp = pc.get_covariance(scaling_modifier)
         else:
-            scales, rotations = pc.get_scaling, rots
+            scales, rotations = (pc.get_scaling if filter_3D is None else pc.get_scaling_with_3D_filter), rots
         if override_color is None:
             if getattr(pipe, "convert_SHs_python", False):
                 from .sh import eval_sh_python
@@ -97,7 +103,8 @@ def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_
             colors_precomp = override_color
         rasterizer = Rasterizer(raster_settings=raster_settings)
         rendered_image, radii = rasterizer(means3D=means3D, means2D=screenspace_points, shs=shs,
-                                           colors_precomp=colors_precomp, opacities=pc.get_opacity,
+                                           colors_precomp=colors_precomp,
+                                           opacities=pc.get_opacity if filter_3D is None else pc.get_opacity_with_3D_filter,
                                            scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp)
     return {"render": rendered_image, "viewspace_points": screenspace_points,
             "visibility_filter": radii > 0, "radii": radii}

@@ -9,7 +9,7 @@ What the reference's training stage reads and writes, so a scene produced here c
 * `points3D.ply`: x,y,z f4 | nx,ny,nz f4 | red,green,blue u1 (scene/dataset_readers.py:315-369);
 * `confidence_dsp.npy` [P,1] (train.py:63-96);
 * the trained model `point_cloud.ply`: x,y,z,nx,ny,nz,f_dc_0..2,f_rest_0..44,opacity,scale_0..2,rot_0..3, all f4,
-  SH stored channel-major (scene/gaussian_model.py:247-278);
+  SH stored channel-major (scene/gaussian_model.py:247-278), optionally followed by Mip-Splatting's `filter_3D` f4;
 * `pose_optimized.npy` [n,4,4] world-to-camera matrices ordered by COLMAP image id
   (train.py:46-60).
 
@@ -163,9 +163,10 @@ def gaussian_ply_fields(n_rest: int = 45) -> List[str]:
             + ["opacity"] + [f"scale_{i}" for i in range(3)] + [f"rot_{i}" for i in range(4)])
 
 
-def save_gaussians_ply(path: str, xyz, f_dc, f_rest, opacity, scaling, rotation) -> None:
+def save_gaussians_ply(path: str, xyz, f_dc, f_rest, opacity, scaling, rotation, filter_3D=None) -> None:
     """Model tensors -> point_cloud.ply; f_dc [P,1,3], f_rest [P,M-1,3] are stored channel-major
-    (transpose(1,2).flatten(1)), raw (un-activated) opacity / scaling / rotation, zero normals."""
+    (transpose(1,2).flatten(1)), raw (un-activated) opacity / scaling / rotation, zero normals.  filter_3D [P] or
+    [P,1] (Mip-Splatting's 3D smoothing filter), when given, is the last property, as Mip-Splatting stores it."""
     xyz = np.asarray(xyz, np.float32)
     P = xyz.shape[0]
     dc = np.asarray(f_dc, np.float32).reshape(P, -1, 3).transpose(0, 2, 1).reshape(P, -1)
@@ -174,20 +175,27 @@ def save_gaussians_ply(path: str, xyz, f_dc, f_rest, opacity, scaling, rotation)
                             np.asarray(scaling, np.float32).reshape(P, 3), np.asarray(rotation, np.float32).reshape(P, 4)],
                            axis=1)
     names = gaussian_ply_fields(rest.shape[1])
+    if filter_3D is not None:
+        attrs = np.concatenate([attrs, np.asarray(filter_3D, np.float32).reshape(P, 1)], axis=1)
+        names = names + ["filter_3D"]
     _write_ply(path, [(n, "f4") for n in names], [attrs[:, i] for i in range(attrs.shape[1])])
 
 
 def load_gaussians_ply(path: str) -> Dict[str, np.ndarray]:
-    """Inverse of save_gaussians_ply (what GaussianModel.load_ply does, gaussian_model.py:280+)."""
+    """Inverse of save_gaussians_ply (what GaussianModel.load_ply does, gaussian_model.py:280+).  The dict has a
+    `filter_3D` [P,1] entry only when the file carries that property."""
     d = _read_ply(path)
     P = d.shape[0]
     col = lambda prefix: np.stack([d[n] for n in sorted((n for n in d.dtype.names if n.startswith(prefix)),
                                                         key=lambda s: int(s.split("_")[-1]))], axis=1)
     rest = col("f_rest_")
-    return dict(xyz=np.stack([d["x"], d["y"], d["z"]], axis=1),
-                f_dc=col("f_dc_").reshape(P, 3, 1).transpose(0, 2, 1).copy(),
-                f_rest=rest.reshape(P, 3, rest.shape[1] // 3).transpose(0, 2, 1).copy(),
-                opacity=d["opacity"].reshape(P, 1).copy(), scaling=col("scale_"), rotation=col("rot_"))
+    out = dict(xyz=np.stack([d["x"], d["y"], d["z"]], axis=1),
+               f_dc=col("f_dc_").reshape(P, 3, 1).transpose(0, 2, 1).copy(),
+               f_rest=rest.reshape(P, 3, rest.shape[1] // 3).transpose(0, 2, 1).copy(),
+               opacity=d["opacity"].reshape(P, 1).copy(), scaling=col("scale_"), rotation=col("rot_"))
+    if "filter_3D" in d.dtype.names:
+        out["filter_3D"] = d["filter_3D"].reshape(P, 1).copy()
+    return out
 
 
 def save_pose_npy(path: str, poses7: np.ndarray, colmap_ids: List[int] = None) -> np.ndarray:

@@ -23,7 +23,7 @@ import torch
 
 from . import _lib
 from ._lib import GsbCamera, GsbGaussians, GsbGrads, check
-from .frame import ST_OVERFLOW, ST_WORDS, Frame, IdentityView, capacity, gaussians, read_R
+from .frame import ST_OVERFLOW, ST_WORDS, Frame, IdentityView, capacity, gaussians, mip_filter, read_R
 
 
 def cosine_lr(base_lr: float, k: int, t_max: int, eta_min: float = 1e-4) -> float:
@@ -32,10 +32,11 @@ def cosine_lr(base_lr: float, k: int, t_max: int, eta_min: float = 1e-4) -> floa
 
 
 class PoseTracker:
-    """Frozen Gaussians (raw parameter tensors, the layout of GaussianModel / JointTrainer) + scratch buffers."""
+    """Frozen Gaussians (raw parameter tensors, the layout of GaussianModel / JointTrainer) + scratch buffers.
+    kernel_size / filter_3D: Mip-Splatting's 2D Mip filter and (frozen) 3D smoothing filter, DESIGN.md section 4.7."""
 
     def __init__(self, xyz, rotation, scaling, opacity, f_dc, f_rest, width, height, fovx, fovy, bg=None,
-                 sh_degree: int = 3, device=None):
+                 sh_degree: int = 3, device=None, kernel_size=None, filter_3D=None):
         self.dev = torch.device(device) if device is not None else xyz.device
         f = lambda t: t.detach().to(self.dev).float().contiguous()
         self.xyz, self.rotation, self.scaling = f(xyz), f(rotation), f(scaling)
@@ -49,13 +50,16 @@ class PoseTracker:
         self.host_status = torch.zeros(ST_WORDS, dtype=torch.int32).pin_memory()
         self.headroom = 1.6            # the pose moves during tracking, and with it the instance count
         self.R_seen = 0
+        self.filter_3D = None if filter_3D is None else f(filter_3D).reshape(-1)
+        self.filt = mip_filter(kernel_size, self.filter_3D)
 
     @classmethod
-    def from_model(cls, pc, camera, bg=None, device=None):
+    def from_model(cls, pc, camera, bg=None, device=None, kernel_size=None):
         """pc: a GaussianModel-like object (reference attribute names), camera: FoVx/FoVy/image_width/image_height."""
         return cls(pc._xyz, pc._rotation, pc._scaling, pc._opacity, pc._features_dc, pc._features_rest,
                    camera.image_width, camera.image_height, camera.FoVx, camera.FoVy, bg=bg,
-                   sh_degree=pc.active_sh_degree, device=device)
+                   sh_degree=pc.active_sh_degree, device=device, kernel_size=kernel_size,
+                   filter_3D=getattr(pc, "filter_3D", None))
 
     # ------------------------------------------------------------------------------------------
     def _cam(self) -> GsbCamera:
@@ -67,7 +71,7 @@ class PoseTracker:
 
     def _forward(self, cam, g, first: bool):
         fr = self.frame
-        fr.preprocess(cam, g, self.host_status if first else None)
+        fr.preprocess(cam, g, self.host_status if first else None, self.filt)
         if first:                      # size the binning buffer once, from the real count at the initial pose
             torch.cuda.current_stream().synchronize()
             self.R_seen = R = read_R(self.host_status)
@@ -109,7 +113,7 @@ class PoseTracker:
                 check(L.gsb_l1_mask_fwd_bwd(3, self.H, self.W, self.frame.color.data_ptr(), gt.data_ptr(),
                                             float(threshold), sums[k].data_ptr(), self.dL.data_ptr(), st),
                       "gsb_l1_mask_fwd_bwd")
-                self.frame.backward(cam, g, self.dL, gr)
+                self.frame.backward(cam, g, self.dL, gr, self.filt)
                 check(L.gsb_track_step(pose.data_ptr(), dpose.data_ptr(), sums[k].data_ptr(), m.data_ptr(), v.data_ptr(),
                                        best.data_ptr(), trace[k:].data_ptr() if return_trace else None, k + 1,
                                        cosine_lr(lr_q, k, num_iter, eta_min), cosine_lr(lr_T, k, num_iter, eta_min),

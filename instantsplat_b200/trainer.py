@@ -25,7 +25,8 @@ import torch
 
 from . import _lib
 from ._lib import GsbGaussians, GsbGrads, check
-from .frame import ST_OVERFLOW, ST_SEQ, ST_WORDS, Frame, IdentityView, capacity, gaussians, read_R
+from .frame import (ST_OVERFLOW, ST_SEQ, ST_WORDS, Frame, IdentityView, capacity, gaussians, mip_filter, mip_filter3d,
+                    read_R)
 from .per_point_adam import launch_adam
 from .scenes import Scene
 
@@ -66,6 +67,11 @@ class OptimConfig:
     spatial_lr_scale = 1.0
     sh_increase_interval = 1000      # train.py:146-147: oneupSHdegree() when iteration % 1000 == 0
     max_sh_degree = 3
+    # Mip-Splatting (DESIGN.md section 4.7): None = off; else the 2D Mip filter's kernel size (0.1 in Mip-Splatting)
+    # together with the 3D smoothing filter, computed at construction and after every change of the Gaussian count, and
+    # recomputed from the current poses and xyz each time the iteration count crosses a multiple of `mip_filter3d_interval`, except in the last 100.
+    mip_kernel_size = None
+    mip_filter3d_interval = 100
 
 
 def L_sig_words():
@@ -142,6 +148,8 @@ class JointTrainer:
         self.ident = IdentityView(self.W, self.H, scene.fovx, scene.fovy, scene.bg, self.dev)
         self.frame = Frame(self.dev, P, self.W, self.H)     # scratch; its binning buffer is sized by the first forward
         self.headroom = 1.5
+        self.filter_3D, self.filt, self.mip_recomputed_at = None, None, []
+        self._mip_setup()
         self.dL_dimg = torch.empty_like(self.color)
         self.maps = torch.empty(3, 3, self.H, self.W, dtype=torch.float32, device=self.dev)
         self.sums = torch.zeros(2, dtype=torch.float64, device=self.dev)
@@ -200,6 +208,20 @@ class JointTrainer:
         """Instance capacity of the binning buffer (0: not sized yet)."""
         return self.frame.cap
 
+    def _mip_setup(self) -> None:
+        """A filter_3D buffer for the current P, filled; the GsbFilter points at it for the buffer's lifetime, so the
+        recompute (outside any captured graph) changes what graph replays read without changing the graphs."""
+        if self.cfg.mip_kernel_size is None:
+            return
+        self.filter_3D = torch.empty(self.P, dtype=torch.float32, device=self.dev)
+        self.filt = mip_filter(self.cfg.mip_kernel_size, self.filter_3D)
+        self.compute_filter_3D()
+
+    def compute_filter_3D(self) -> None:
+        """Recompute the 3D smoothing filter from the current xyz and pose table (gsb_mip_filter3d, deterministic)."""
+        mip_filter3d(self.view(self.params, "xyz"), self.poses, self.W, self.H, self.ident.tanfovx, self.ident.tanfovy,
+                     out=self.filter_3D)
+
     def _gauss(self, view: int) -> GsbGaussians:
         p = self.params
         return gaussians(self.P, *(self.view(p, n) for n in ("xyz", "rotation", "scaling", "opacity", "f_dc", "f_rest")),
@@ -214,7 +236,7 @@ class JointTrainer:
         host only provides a capacity (sized from the counts seen so far, +50 %) and reads R back lazily."""
         cam, g = self.ident.camera(self.active_sh_degree, 16, self.exact_cull), self._gauss(view)
         capturing = torch.cuda.is_current_stream_capturing()
-        self.frame.preprocess(cam, g, self.host_status[0])
+        self.frame.preprocess(cam, g, self.host_status[0], self.filt)
         if not capturing:
             self._fwd_count += 1
             self._polling = False
@@ -278,7 +300,7 @@ class JointTrainer:
         gr.dL_dsh_rest = self.view(gd, "f_rest").data_ptr()
         self.pose_grad.zero_()
         gr.dL_dpose = self.pose_grad[view].data_ptr()
-        self.frame.backward(cam, g, self.dL_dimg, gr)
+        self.frame.backward(cam, g, self.dL_dimg, gr, self.filt)
 
     def loss_value(self) -> torch.Tensor:
         n = 3 * self.H * self.W
@@ -501,7 +523,15 @@ class JointTrainer:
         do_opt = self.iteration < c.iterations
         if self.use_graph and self.cap > 0:
             self._graph_iteration(view, gt, do_opt)
-            return
+        else:
+            self._run_iteration_settled(view, gt, do_opt)
+        # crossing a multiple of the interval (with G ranks `iteration` advances by G per step)
+        if self.filt is not None and self.iteration // c.mip_filter3d_interval > before // c.mip_filter3d_interval and \
+                self.iteration < c.iterations - 100:
+            self.compute_filter_3D()
+            self.mip_recomputed_at.append(self.iteration)
+
+    def _run_iteration_settled(self, view: int, gt: torch.Tensor, do_opt: bool) -> None:
         self._run_iteration(view, gt, do_opt)
         if not self._settle():
             # The binning capacity was exceeded: the device skipped the update by itself (gated on the overflow word,
@@ -543,6 +573,7 @@ class JointTrainer:
             self.view(self.exp_avg, name).copy_(m_.reshape(new_P, k))
             self.view(self.exp_avg_sq, name).copy_(v_.reshape(new_P, k))
         self.frame = Frame(self.dev, new_P, self.W, self.H)   # the next forward sizes its binning buffer
+        self._mip_setup()
         self._keep = None
         self._graphs.clear()
         self.frame.status.zero_()
