@@ -157,6 +157,25 @@ GSB_API int gsb_backward_ex(const GsbCamera* cam, const GsbGaussians* g, const G
                             void* binning, int64_t R, void* image, const float* dL_dout, const GsbGrads* grads,
                             gsb_stream_t stream);
 
+/* Densification statistics of the reference loop (train.py:197-199 with gaussian_model.py:476-478), accumulated by
+ * the per-Gaussian backward from the same dL/dmeans2D it writes to GsbGrads.dL_dmeans2D.  All arrays are [P]:
+ * radii is the forward's output (gsb_preprocess), the other three are read and updated in place.  For every Gaussian
+ * with radii > 0 (the reference's visibility_filter):
+ *   grad_accum += |dL/dmeans2D[:2]|,  denom += 1,  max_radii2D = max(max_radii2D, radii).
+ * Nothing is updated when the forward's binning capacity was exceeded (status word 1), so that a repeated
+ * iteration counts once.  One thread per Gaussian, no atomics: the result is bit-reproducible. */
+typedef struct GsbDensifyStats {
+  const int32_t* radii;
+  float* grad_accum;
+  float* denom;
+  float* max_radii2D;
+} GsbDensifyStats;
+
+/* gsb_backward_ex that also accumulates the densification statistics; gsb_backward_ex is this with stats = NULL. */
+GSB_API int gsb_backward_stats(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt,
+                               const GsbDensifyStats* stats, void* geom, void* binning, int64_t R, void* image,
+                               const float* dL_dout, const GsbGrads* grads, gsb_stream_t stream);
+
 /* Size of the 3D smoothing filter (Mip-Splatting's GaussianModel.compute_3D_filter) from the training views' pose
  * table: poses7 [n_views, 7] (the rows gsb_preprocess takes as GsbGaussians.pose, p = R x + t), xyz [P, 3] world
  * points, one shared intrinsics (width, height, tanfovx, tanfovy).  A view counts for a point when p_z > 0.2 and

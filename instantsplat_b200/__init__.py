@@ -17,3 +17,4 @@ from .per_point_adam import PerPointAdam  # noqa: F401
 from .trainer import JointTrainer, OptimConfig  # noqa: F401
 from .model import GaussianModel, PipelineDefaults, SimpleGaussianModel, optimization_defaults  # noqa: F401
 from .knn import distCUDA2  # noqa: F401
+from .densify import cameras_extent, densify_plan  # noqa: F401

@@ -49,6 +49,11 @@ class GsbFilter(ctypes.Structure):
 FILTER_MIP2D = 1
 
 
+class GsbDensifyStats(ctypes.Structure):
+    _fields_ = [("radii", ctypes.c_void_p), ("grad_accum", ctypes.c_void_p), ("denom", ctypes.c_void_p),
+                ("max_radii2D", ctypes.c_void_p)]
+
+
 class GsbAdamTensor(ctypes.Structure):
     _fields_ = [("param", ctypes.c_void_p), ("grad", ctypes.c_void_p), ("exp_avg", ctypes.c_void_p),
                 ("exp_avg_sq", ctypes.c_void_p), ("per_point_lr", ctypes.c_void_p),
@@ -71,7 +76,7 @@ EXPORTS = ("gsb_geom_bytes", "gsb_binning_bytes", "gsb_image_bytes", "gsb_prepro
            "gsb_abi_version", "gsb_profile_enable", "gsb_profile_collect", "gsb_launch_count", "gsb_set_option", "gsb_adam_gate",
            "gsb_ipc_alloc", "gsb_ipc_open", "gsb_ipc_close", "gsb_ipc_free", "gsb_fused_rs_adam_ag",
            "gsb_knn_scratch_bytes", "gsb_knn_mean_dist2", "gsb_status_device", "gsb_adam_step_gated", "gsb_blend_stats", "gsb_l1_mask_fwd_bwd", "gsb_track_step", "gsb_peer_signal_bytes", "gsb_peer_barrier", "gsb_peer_exchange", "gsb_adam_step_ex",
-           "gsb_preprocess_ex", "gsb_backward_ex", "gsb_mip_filter3d")
+           "gsb_preprocess_ex", "gsb_backward_ex", "gsb_mip_filter3d", "gsb_backward_stats")
 KERNEL_IDS = ("preprocess", "sort_depth", "scan", "duplicate", "sort_tile", "gather", "blend_fwd", "blend_bwd",
               "preprocess_bwd", "loss_fwd", "loss_bwd", "adam")
 
@@ -112,6 +117,8 @@ def lib() -> ctypes.CDLL:
                                     vp, sz, vp, vp, vp]
     L.gsb_backward_ex.argtypes = [ctypes.POINTER(GsbCamera), ctypes.POINTER(GsbGaussians), ctypes.POINTER(GsbFilter),
                                   vp, vp, i64, vp, vp, ctypes.POINTER(GsbGrads), vp]
+    L.gsb_backward_stats.argtypes = [ctypes.POINTER(GsbCamera), ctypes.POINTER(GsbGaussians), ctypes.POINTER(GsbFilter),
+                                     ctypes.POINTER(GsbDensifyStats), vp, vp, i64, vp, vp, ctypes.POINTER(GsbGrads), vp]
     L.gsb_mip_filter3d.argtypes = [i32, vp, i32, vp, i32, i32, ctypes.c_float, ctypes.c_float, vp, vp]
     L.gsb_render.argtypes = [ctypes.POINTER(GsbCamera), i32, vp, vp, sz, i64, vp, vp, vp, vp]
     L.gsb_blend_stats.argtypes = [ctypes.POINTER(GsbCamera), i32, vp, vp, i64, vp, vp, vp, vp, vp]
@@ -163,7 +170,7 @@ def lib() -> ctypes.CDLL:
     for f in ("gsb_adam_gate", "gsb_ipc_alloc", "gsb_ipc_open", "gsb_ipc_close", "gsb_ipc_free",
               "gsb_fused_rs_adam_ag"):
         getattr(L, f).restype = ctypes.c_int
-    for f in ("gsb_preprocess", "gsb_preprocess_ex", "gsb_backward_ex", "gsb_mip_filter3d", "gsb_render", "gsb_backward", "gsb_mark_visible", "gsb_ssim_forward",
+    for f in ("gsb_preprocess", "gsb_preprocess_ex", "gsb_backward_ex", "gsb_backward_stats", "gsb_mip_filter3d", "gsb_render", "gsb_backward", "gsb_mark_visible", "gsb_ssim_forward",
               "gsb_ssim_backward", "gsb_loss_forward", "gsb_loss_backward", "gsb_adam_step"):
         getattr(L, f).restype = ctypes.c_int
     _lib = L

@@ -455,13 +455,17 @@ struct OutPtrs {
   float* dmeans; float* dmeans2D; float* dscales; float* drots; float* dopac;
   float* dsh_dc; float* dsh_rest; float* dcolors; float* dcov3D;
 };
+// densification statistics (GsbDensifyStats), read only by the kStats instances
+struct StatsPtrs {
+  const int32_t* radii; float* accum; float* denom; float* max_r;
+};
 
 #ifndef GSB_PBWD_MINB
 #define GSB_PBWD_MINB 4
 #endif
-template <bool kMip>
+template <bool kMip, bool kStats>
 __global__ void __launch_bounds__(kPT, GSB_PBWD_MINB)
-k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out) {
+k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out, StatsPtrs stats) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   CamConst* cam = reinterpret_cast<CamConst*>(smem_raw);
   float* sm = reinterpret_cast<float*>(smem_raw + ((sizeof(CamConst) + 15) / 16) * 16);
@@ -560,6 +564,15 @@ k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out
     if (out.dcov3D) {
 #pragma unroll
       for (int k = 0; k < 6; ++k) out.dcov3D[6 * (size_t)i + k] = gg.dcov3D[k];
+    }
+    // train.py:197-199: every Gaussian with radii > 0 (visibility_filter; also those that kept no tile, whose
+    // dmeans2D is 0) adds |dL/dmeans2D[:2]| and one view, and raises its largest screen radius.  One writer per
+    // Gaussian, no atomics.  Not after a binning overflow: the caller repeats that iteration.
+    if (kStats && stats.radii[i] > 0 && gv.status[kStOverflow] == 0u) {
+      const float dx = gg.dmeans2D[0], dy = gg.dmeans2D[1];
+      stats.accum[i] += sqrtf(dx * dx + dy * dy);
+      stats.denom[i] += 1.f;
+      stats.max_r[i] = fmaxf(stats.max_r[i], (float)stats.radii[i]);
     }
   }
   // Full CTA, aligned, split SH layout: every gradient array of the CTA leaves as one bulk store (shared -> global)
@@ -707,7 +720,8 @@ static int ensure_attrs() {
   if (dev < 0 || dev >= 64 || !done[dev]) {
     for (auto k : {k_preprocess<false>, k_preprocess<true>})
       GSB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPrepSmem));
-    for (auto k : {k_preprocess_bwd<false>, k_preprocess_bwd<true>})
+    for (auto k : {k_preprocess_bwd<false, false>, k_preprocess_bwd<true, false>, k_preprocess_bwd<false, true>,
+                   k_preprocess_bwd<true, true>})
       GSB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPrepSmem));
     if (dev >= 0 && dev < 64) done[dev] = true;
   }
@@ -782,9 +796,9 @@ extern "C" GSB_API int gsb_render(const GsbCamera* cam, int32_t P, void* geom, v
   return GSB_OK;
 }
 
-extern "C" GSB_API int gsb_backward_ex(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, void* geom,
-                                       void* binning, int64_t R, void* image, const float* dL_dout, const GsbGrads* grads,
-                                       gsb_stream_t stream_) {
+extern "C" GSB_API int gsb_backward_stats(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt,
+                                          const GsbDensifyStats* stats, void* geom, void* binning, int64_t R, void* image,
+                                          const float* dL_dout, const GsbGrads* grads, gsb_stream_t stream_) {
   cudaStream_t st = (cudaStream_t)stream_;
   InPtrs in;
   int rc = make_inptrs(cam, g, in);
@@ -793,6 +807,9 @@ extern "C" GSB_API int gsb_backward_ex(const GsbCamera* cam, const GsbGaussians*
   if (rc) return rc;
   GSB_REQUIRE(geom && binning && image && dL_dout && grads, "null buffer");
   if (g->pose) GSB_REQUIRE(grads->dL_dpose != nullptr, "dL_dpose required when pose is fused");
+  if (stats)
+    GSB_REQUIRE((stats->radii && stats->grad_accum && stats->denom && stats->max_radii2D) || g->P == 0,
+                "GsbDensifyStats: null buffer");
   const int P = g->P, W = cam->width, H = cam->height;
   GeomView gv = geom_view(geom, P);
   BinView bv = bin_view(binning, R, W, H);
@@ -820,16 +837,26 @@ extern "C" GSB_API int gsb_backward_ex(const GsbCamera* cam, const GsbGaussians*
   uintptr_t a = (uintptr_t)out.dmeans | (uintptr_t)out.dscales | (uintptr_t)out.drots | (uintptr_t)out.dopac |
                 (uintptr_t)out.dsh_dc | (uintptr_t)out.dsh_rest;
   if (a & 15) in.vec_ok = 0;
+  StatsPtrs sp;
+  sp.radii = stats ? stats->radii : nullptr; sp.accum = stats ? stats->grad_accum : nullptr;
+  sp.denom = stats ? stats->denom : nullptr; sp.max_r = stats ? stats->max_radii2D : nullptr;
   const int nb = (P + kPT - 1) / kPT;
   { ProfScope ps(GSB_K_PREPROCESS_BWD, st, g->pose ? 3 : 1);
-    (in.mip.on ? k_preprocess_bwd<true> : k_preprocess_bwd<false>)<<<nb, kPT, kPrepSmem, st>>>(in, gv, pose_only ? 1 : 0,
-                                                                                             out);
+    auto kern = in.mip.on ? (stats ? k_preprocess_bwd<true, true> : k_preprocess_bwd<true, false>)
+                          : (stats ? k_preprocess_bwd<false, true> : k_preprocess_bwd<false, false>);
+    kern<<<nb, kPT, kPrepSmem, st>>>(in, gv, pose_only ? 1 : 0, out, sp);
     if (g->pose) {
       k_pose_reduce<<<16, 256, 0, st>>>(gv.pose_part, nb, gv.pose_acc);
       k_pose_finalize<<<1, 32, 0, st>>>(gv.pose_acc, g->pose, grads->dL_dpose);
     } }
   GSB_CUDA(cudaGetLastError());
   return GSB_OK;
+}
+
+extern "C" GSB_API int gsb_backward_ex(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, void* geom,
+                                       void* binning, int64_t R, void* image, const float* dL_dout, const GsbGrads* grads,
+                                       gsb_stream_t stream) {
+  return gsb_backward_stats(cam, g, filt, nullptr, geom, binning, R, image, dL_dout, grads, stream);
 }
 
 extern "C" GSB_API int gsb_backward(const GsbCamera* cam, const GsbGaussians* g, void* geom, void* binning, int64_t R,

@@ -13,7 +13,7 @@ import math
 import torch
 
 from . import _lib
-from ._lib import FILTER_MIP2D, GsbCamera, GsbFilter, GsbGaussians, check
+from ._lib import FILTER_MIP2D, GsbCamera, GsbDensifyStats, GsbFilter, GsbGaussians, check
 
 # the status words of a forward (kSt* of csrc/gs_internal.cuh); the library writes them as uint32
 ST_R, ST_OVERFLOW, ST_MAX_LIST, ST_HUGE_TILES, ST_NLARGE, ST_NHUGE, ST_SEQ = range(7)
@@ -107,6 +107,14 @@ def mip_filter3d(xyz, poses7, W, H, tanfovx, tanfovy, out=None) -> torch.Tensor:
     return out
 
 
+def densify_stats(radii, grad_accum, denom, max_radii2D) -> GsbDensifyStats:
+    """GsbDensifyStats over contiguous device tensors of P elements: radii int32 (the forward's), the other three fp32,
+    updated in place by the backward (train.py:197-199).  The tensors must stay alive while the struct is in use."""
+    s = GsbDensifyStats()
+    s.radii, s.grad_accum, s.denom, s.max_radii2D = _p(radii), _p(grad_accum), _p(denom), _p(max_radii2D)
+    return s
+
+
 def _f(filt):
     return None if filt is None else ctypes.byref(filt)
 
@@ -154,10 +162,17 @@ class Frame:
                                     self.binning.numel(), self.cap, self.image.data_ptr(), self.color.data_ptr(),
                                     _p(host_status), _lib.stream_ptr()), "gsb_render")
 
-    def backward(self, cam, g, dL_dimage, grads, filt=None) -> None:
-        check(_lib.lib().gsb_backward_ex(ctypes.byref(cam), ctypes.byref(g), _f(filt), self.geom.data_ptr(),
-                                         self.binning.data_ptr(), self.cap, self.image.data_ptr(), dL_dimage.data_ptr(),
-                                         ctypes.byref(grads), _lib.stream_ptr()), "gsb_backward")
+    def backward(self, cam, g, dL_dimage, grads, filt=None, stats=None) -> None:
+        """stats: densify_stats(...) over this frame's radii, or None; accumulated by the same launch."""
+        if stats is None:
+            check(_lib.lib().gsb_backward_ex(ctypes.byref(cam), ctypes.byref(g), _f(filt), self.geom.data_ptr(),
+                                             self.binning.data_ptr(), self.cap, self.image.data_ptr(),
+                                             dL_dimage.data_ptr(), ctypes.byref(grads), _lib.stream_ptr()), "gsb_backward")
+        else:
+            check(_lib.lib().gsb_backward_stats(ctypes.byref(cam), ctypes.byref(g), _f(filt), ctypes.byref(stats),
+                                                self.geom.data_ptr(), self.binning.data_ptr(), self.cap,
+                                                self.image.data_ptr(), dL_dimage.data_ptr(), ctypes.byref(grads),
+                                                _lib.stream_ptr()), "gsb_backward_stats")
 
     def blend_stats(self, cam, dL_dimage, stats) -> None:
         check(_lib.lib().gsb_blend_stats(ctypes.byref(cam), self.P, self.geom.data_ptr(), self.binning.data_ptr(),

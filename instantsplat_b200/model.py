@@ -311,23 +311,67 @@ class GaussianModel:
                                    None if self.per_point_lr is None else self.per_point_lr[sel].repeat(N, 1))
         self.prune_points(torch.cat((sel, torch.zeros(N * int(sel.sum()), device=self.device, dtype=torch.bool))))
 
-    def densify_and_prune(self, max_grad, min_opacity, extent, max_screen_size, clone_and_split=False):
+    def densify_and_prune(self, max_grad, min_opacity, extent, max_screen_size, clone_and_split=False, generator=None):
         """Reference :455-474 (InstantSplat keeps clone / split commented out; `clone_and_split=True` enables the
-        vanilla-3DGS behaviour)."""
-        grads = self.xyz_gradient_accum / self.denom
-        grads[grads.isnan()] = 0.0
-        if clone_and_split:
-            self.densify_and_clone(grads, max_grad, extent)
-            self.densify_and_split(grads, max_grad, extent)
-        prune = (self.get_opacity < min_opacity).squeeze()
-        if max_screen_size:
-            prune = prune | (self.max_radii2D > max_screen_size) | (self.get_scaling.max(dim=1).values > 0.1 * extent)
-        self.prune_points(prune)
+        vanilla-3DGS behaviour, split samples drawn from `generator`).  The rows of densify_and_clone,
+        densify_and_split and the prune come from one `densify_plan` (shared with JointTrainer) and are applied in one
+        rebuild; the result is that of running the three in sequence."""
+        from .densify import densify_plan
+        plan = densify_plan(self._xyz.detach(), self._scaling.detach(), self._rotation.detach(), self._opacity.detach(),
+                            self.xyz_gradient_accum, self.denom, self.max_radii2D, max_grad, min_opacity, extent,
+                            max_screen_size, self.percent_dense, clone_and_split, generator)
+        self.apply_densify_plan(plan)
+        return plan
+
+    def apply_densify_plan(self, plan):
+        computed = dict(xyz=plan.split_xyz, scaling=plan.split_scaling)
+
+        def edit(name, p, st):
+            if st is not None:
+                st["exp_avg"], st["exp_avg_sq"] = plan.moments(st["exp_avg"]), plan.moments(st["exp_avg_sq"])
+            return plan.gather(p.detach(), computed.get(name)), st
+
+        xyz_before_prune = plan.gather(self._xyz.detach(), plan.split_xyz, prune=False) if plan.reset_stats else None
+        self._rebuild_groups(edit)
+        if plan.reset_stats:     # densification_postfix ran
+            n = plan.P
+            self.xyz_gradient_accum = torch.zeros(n, 1, device=self.device)
+            self.denom = torch.zeros(n, 1, device=self.device)
+            self.max_radii2D = torch.zeros(n, device=self.device)
+        else:
+            self.xyz_gradient_accum = self.xyz_gradient_accum[plan.src]
+            self.denom = self.denom[plan.src]
+            self.max_radii2D = self.max_radii2D[plan.src]
+        if self.per_point_lr is not None:
+            self.per_point_lr = plan.gather(self.per_point_lr)
+            self.optimizer.param_groups[0]["per_point_lr"] = self.per_point_lr
+        if self.filter_3D is not None:
+            if plan.reset_stats and self._filter_cams is not None:
+                # postfix recomputes from the cameras over the rows before the prune, which then keeps its rows
+                cams = self._filter_cams
+                c0 = cams[0]
+                f = mip_filter3d_of(xyz_before_prune, self.P[:len(cams)], c0)
+                self.filter_3D = f[:, None][plan.keep]
+            elif plan.reset_stats:
+                # no cameras: new rows take the largest existing size (densification_postfix)
+                fill = self.filter_3D.max() if self.filter_3D.numel() else torch.zeros((), device=self.device)
+                f = self.filter_3D[plan.src2].clone()
+                f[plan.new2] = fill.to(f)
+                self.filter_3D = f[plan.keep]
+            else:
+                self.filter_3D = self.filter_3D[plan.src]
 
     def add_densification_stats(self, viewspace_point_tensor, update_filter):
         self.xyz_gradient_accum[update_filter] += torch.norm(viewspace_point_tensor.grad[update_filter, :2], dim=-1,
                                                               keepdim=True)
         self.denom[update_filter] += 1
+
+
+def mip_filter3d_of(xyz, poses, cam):
+    """gsb_mip_filter3d for camera-like intrinsics (FoVx, FoVy, image_width, image_height)."""
+    from .frame import mip_filter3d
+    return mip_filter3d(xyz, poses, int(cam.image_width), int(cam.image_height), math.tan(float(cam.FoVx) * 0.5),
+                        math.tan(float(cam.FoVy) * 0.5))
 
 
 def w2c_to_pose(RT: torch.Tensor) -> torch.Tensor:

@@ -27,6 +27,8 @@ from . import _lib
 from ._lib import GsbGaussians, GsbGrads, check
 from .frame import (ST_OVERFLOW, ST_SEQ, ST_WORDS, Frame, IdentityView, capacity, gaussians, mip_filter, mip_filter3d,
                     read_R)
+from .densify import cameras_extent, densify_plan
+from .frame import densify_stats
 from .per_point_adam import launch_adam
 from .scenes import Scene
 
@@ -72,6 +74,21 @@ class OptimConfig:
     # recomputed from the current poses and xyz each time the iteration count crosses a multiple of `mip_filter3d_interval`, except in the last 100.
     mip_kernel_size = None
     mip_filter3d_interval = 100
+    # Adaptive density control (DESIGN.md section 4.8), train.py:195-206 with the block enabled; one GPU only.
+    # densify_clone_split=False is InstantSplat's prune-only densify_and_prune, True the vanilla-3DGS clone + split.
+    # scene_extent=None: getNerfppNorm's radius of the initial pose table (densify.cameras_extent).
+    densify = False
+    densify_from_iter = 500
+    densify_until_iter = 15_000
+    densification_interval = 100
+    opacity_reset_interval = 3000
+    densify_grad_threshold = 0.0002
+    min_opacity = 0.005
+    percent_dense = 0.01
+    size_threshold = 20
+    densify_clone_split = False
+    scene_extent = None
+    densify_seed = 0                 # seed of the generator the split samples are drawn from
 
 
 def L_sig_words():
@@ -87,6 +104,9 @@ class JointTrainer:
                  cfg: Optional[OptimConfig] = None, world_size: int = 1, rank: int = 0,
                  process_group=None, exchange: str = "allreduce", use_graph: bool = False):
         self.cfg = cfg or OptimConfig()
+        if self.cfg.densify and world_size > 1:
+            raise _lib.GsbError("densify=True needs world_size == 1: every rank would accumulate different "
+                                "densification statistics")
         self.dev = torch.device(device)
         self.world_size, self.rank, self.pg = world_size, rank, process_group
         if exchange not in ("allreduce", "fused_p2p", "fused_p2p_nccl"):
@@ -187,6 +207,16 @@ class JointTrainer:
         self.cam_sched = get_expon_lr_func(c.rotation_lr * 0.1, c.rotation_lr * 0.001,
                                            lr_delay_mult=c.position_lr_delay_mult, max_steps=c.iterations)
         self._keep = None
+        # per-tensor Adam step counts are opt_step minus the optimizer steps that skipped the tensor (the densify and
+        # opacity-reset iterations replace tensors, which then have no gradient in the reference)
+        self._lag = {name: 0 for name, _ in SEGMENTS}
+        self._stats = None
+        if c.densify:
+            self._stats = torch.zeros(3, P, dtype=torch.float32, device=self.dev)
+            self.scene_extent = cameras_extent(scene.poses) if c.scene_extent is None else float(c.scene_extent)
+            self.densify_generator = torch.Generator(device=self.dev).manual_seed(int(c.densify_seed))
+            self.white_background = bool((scene.bg == 1).all())
+        self.densified_at, self.reset_at = [], []
 
     # ------------------------------------------------------------------------------------------
     def view(self, flat: torch.Tensor, name: str) -> torch.Tensor:
@@ -207,6 +237,23 @@ class JointTrainer:
     def cap(self) -> int:
         """Instance capacity of the binning buffer (0: not sized yet)."""
         return self.frame.cap
+
+    # densification statistics with the reference's names and shapes (None unless cfg.densify)
+    @property
+    def xyz_gradient_accum(self) -> Optional[torch.Tensor]:
+        return None if self._stats is None else self._stats[0].view(self.P, 1)
+
+    @property
+    def denom(self) -> Optional[torch.Tensor]:
+        return None if self._stats is None else self._stats[1].view(self.P, 1)
+
+    @property
+    def max_radii2D(self) -> Optional[torch.Tensor]:
+        return None if self._stats is None else self._stats[2]
+
+    def step_count(self, name: str) -> int:
+        """Adam step count of one tensor ("pose" or a SEGMENTS name)."""
+        return self.opt_step - self._lag.get(name, 0)
 
     def _mip_setup(self) -> None:
         """A filter_3D buffer for the current P, filled; the GsbFilter points at it for the buffer's lifetime, so the
@@ -281,7 +328,8 @@ class JointTrainer:
             assert self._settle()
         return self.color
 
-    def loss_and_backward(self, view: int, gt: torch.Tensor) -> None:
+    def loss_and_backward(self, view: int, gt: torch.Tensor, stats: bool = False) -> None:
+        """stats: the backward also accumulates the densification statistics (train.py:197-199)."""
         L = _lib.lib()
         st = _lib.stream_ptr()
         cam, g = self._keep
@@ -300,7 +348,10 @@ class JointTrainer:
         gr.dL_dsh_rest = self.view(gd, "f_rest").data_ptr()
         self.pose_grad.zero_()
         gr.dL_dpose = self.pose_grad[view].data_ptr()
-        self.frame.backward(cam, g, self.dL_dimg, gr, self.filt)
+        st = None
+        if stats:
+            st = densify_stats(self.frame.radii, self._stats[0], self._stats[1], self._stats[2])
+        self.frame.backward(cam, g, self.dL_dimg, gr, self.filt, st)
 
     def loss_value(self) -> torch.Tensor:
         n = 3 * self.H * self.W
@@ -319,7 +370,7 @@ class JointTrainer:
         t = max(1, self.opt_step)
         corr = (1 - 0.999 ** t) ** 0.5 / (1 - 0.9 ** t)
         lrs = self._lrs()
-        out = [lrs[name] * corr for name, _ in SEGMENTS]
+        out = [lrs[name] * self._corr(max(1, self.step_count(name))) for name, _ in SEGMENTS]
         if c.optim_pose:
             out.append(self.cam_sched(self.iteration) * corr)
         return out
@@ -330,12 +381,20 @@ class JointTrainer:
             self._step_host[i] = v
         self._step_dev.copy_(self._step_host, non_blocking=True)
 
-    def optimizer_step(self, grad_scale: Optional[float] = None, _advance: bool = True, _dev_steps: bool = False) -> None:
+    @staticmethod
+    def _corr(t: int) -> float:
+        return (1 - 0.999 ** t) ** 0.5 / (1 - 0.9 ** t)
+
+    def optimizer_step(self, grad_scale: Optional[float] = None, _advance: bool = True, _dev_steps: bool = False,
+                       skip=()) -> None:
         """PerPointAdam.step over the 6 Gaussian tensors + the pose table in one launch
-        (param groups and LRs of scene/gaussian_model.py:203-243)."""
+        (param groups and LRs of scene/gaussian_model.py:203-243).  skip: Gaussian tensors that take no step (they
+        were replaced in this iteration, so the reference's parameter has no gradient); their step counts stay."""
         c = self.cfg
         if _advance:
             self.opt_step += 1
+        for name in skip:
+            self._lag[name] += 1
         t = self.opt_step
         b1, b2, eps = 0.9, 0.999, 1e-15
         corr = (1 - b2 ** t) ** 0.5 / (1 - b1 ** t)
@@ -344,11 +403,13 @@ class JointTrainer:
         gs = 1.0 / self.world_size if grad_scale is None else grad_scale
         entries = []
         for name, k in SEGMENTS:
+            if name in skip:
+                continue
             entries.append(dict(param=self.view(self.params, name), grad=self.view(self.grads, name),
                                 exp_avg=self.view(self.exp_avg, name), exp_avg_sq=self.view(self.exp_avg_sq, name),
                                 per_point_lr=self.per_point_lr if name == "xyz" else None, row_len=k,
-                                step_size=lrs[name] * corr, beta1=b1, beta2=b2, eps=eps, weight_decay=0.0,
-                                grad_scale=gs))
+                                step_size=lrs[name] * self._corr(self.step_count(name)), beta1=b1, beta2=b2, eps=eps,
+                                weight_decay=0.0, grad_scale=gs))
         if c.optim_pose:
             entries.append(dict(param=self.poses, grad=self.pose_grad, exp_avg=self.pose_m, exp_avg_sq=self.pose_v,
                                 per_point_lr=None, row_len=7, step_size=self.cam_sched(self.iteration) * corr,
@@ -441,13 +502,13 @@ class JointTrainer:
         else:
             dist.all_reduce(self._sync, group=self.pg)
 
-    def _graph_iteration(self, view: int, gt: torch.Tensor, do_opt: bool) -> None:
+    def _graph_iteration(self, view: int, gt: torch.Tensor, do_opt: bool, stats: bool = False) -> None:
         """Replay (capturing on first use) the CUDA graph of one iteration on `view`."""
         if do_opt:
             self.opt_step += 1
             self._upload_step_sizes()                    # stream-ordered before the replay
         for _attempt in range(2):
-            key = (view, gt.data_ptr(), do_opt, self.active_sh_degree, self.cap, self.exact_cull)
+            key = (view, gt.data_ptr(), do_opt, self.active_sh_degree, self.cap, self.exact_cull, stats)
             g = self._graphs.get(key)
             if g is None:
                 if len(self._graphs) > 64:
@@ -456,7 +517,7 @@ class JointTrainer:
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g):
                     self._launch_forward(view)
-                    self.loss_and_backward(view, gt)
+                    self.loss_and_backward(view, gt, stats)
                     if self._after_backward is not None:
                         self._after_backward()
                     if do_opt and self._fused:
@@ -476,9 +537,9 @@ class JointTrainer:
             # capacity exceeded: the device skipped the update, the buffer has been enlarged -> new graph, once more
         raise _lib.GsbError("graph replay: binning capacity exceeded twice in a row")
 
-    def _run_iteration(self, view: int, gt: torch.Tensor, do_opt: bool) -> None:
+    def _run_iteration(self, view: int, gt: torch.Tensor, do_opt: bool, stats: bool = False) -> None:
         self._launch_forward(view)
-        self.loss_and_backward(view, gt)
+        self.loss_and_backward(view, gt, stats)
         if self._after_backward is not None:
             self._after_backward()
         if not do_opt:
@@ -521,18 +582,40 @@ class JointTrainer:
         if gt is None:
             gt = self.gt[view]
         do_opt = self.iteration < c.iterations
-        if self.use_graph and self.cap > 0:
-            self._graph_iteration(view, gt, do_opt)
+        it = self.iteration
+        stats = self._stats is not None and it < c.densify_until_iter
+        densify_now = stats and it > c.densify_from_iter and it % c.densification_interval == 0
+        reset_now = stats and (it % c.opacity_reset_interval == 0 or
+                               (self.white_background and it == c.densify_from_iter))
+        if densify_now or reset_now:
+            # train.py:201-211: densify / reset between the backward and the optimizer step, eagerly (the optimizer's
+            # tensor set differs); the replaced tensors take no step in this iteration
+            self._run_iteration_settled(view, gt, False, stats)
+            skip = set()
+            if densify_now:
+                size = c.size_threshold if it > c.opacity_reset_interval else None
+                self.densify_and_prune(c.densify_grad_threshold, c.min_opacity, self.scene_extent, size,
+                                       c.densify_clone_split, self.densify_generator)
+                self.densified_at.append(it)
+                skip.update(name for name, _ in SEGMENTS)
+            if reset_now:
+                self.reset_opacity()
+                self.reset_at.append(it)
+                skip.add("opacity")
+            if do_opt:
+                self.optimizer_step(skip=[name for name, _ in SEGMENTS if name in skip])
+        elif self.use_graph and self.cap > 0:
+            self._graph_iteration(view, gt, do_opt, stats)
         else:
-            self._run_iteration_settled(view, gt, do_opt)
+            self._run_iteration_settled(view, gt, do_opt, stats)
         # crossing a multiple of the interval (with G ranks `iteration` advances by G per step)
         if self.filt is not None and self.iteration // c.mip_filter3d_interval > before // c.mip_filter3d_interval and \
                 self.iteration < c.iterations - 100:
             self.compute_filter_3D()
             self.mip_recomputed_at.append(self.iteration)
 
-    def _run_iteration_settled(self, view: int, gt: torch.Tensor, do_opt: bool) -> None:
-        self._run_iteration(view, gt, do_opt)
+    def _run_iteration_settled(self, view: int, gt: torch.Tensor, do_opt: bool, stats: bool = False) -> None:
+        self._run_iteration(view, gt, do_opt, stats)
         if not self._settle():
             # The binning capacity was exceeded: the device skipped the update by itself (gated on the overflow word,
             # summed over ranks in multi-GPU mode), so parameters and moments are untouched.  Single GPU: repeat the
@@ -543,7 +626,7 @@ class JointTrainer:
                                     "consistent).  Raise JointTrainer.headroom.")
             if do_opt:
                 self.opt_step -= 1
-            self._run_iteration(view, gt, do_opt)
+            self._run_iteration(view, gt, do_opt, stats)
             assert self._settle()
 
     # ---- densify / prune / opacity reset on the flat buffers (SURVEY.md section 8 row f4) -----------------------
@@ -551,8 +634,9 @@ class JointTrainer:
     # parameter AND of both Adam moments; densification_postfix (:399-418) appends rows with zero moments;
     # reset_opacity (:280-283) clamps the opacity to 0.01 (in logit space) and zeroes that tensor's moments.  The
     # optimizer's step counter is untouched by all three, as in the reference (state["step"] survives the surgery).
-    def _resize(self, new_P: int, rows) -> None:
-        """rows(name, old_param_view, old_m_view, old_v_view) -> (param, m, v) tensors of shape [new_P, k]."""
+    def _resize(self, new_P: int, rows, stats: Optional[torch.Tensor] = None) -> None:
+        """rows(name, old_param_view, old_m_view, old_v_view) -> (param, m, v) tensors of shape [new_P, k].
+        stats: the densification statistics [3, new_P] of the new rows (None: zeros, as densification_postfix)."""
         if self._fused:
             raise _lib.GsbError("changing the number of Gaussians is not supported with peer-memory buffers "
                                 "(exchange='fused_p2p'); use exchange='allreduce'")
@@ -572,6 +656,9 @@ class JointTrainer:
             self.view(self.params, name).copy_(p_.reshape(new_P, k))
             self.view(self.exp_avg, name).copy_(m_.reshape(new_P, k))
             self.view(self.exp_avg_sq, name).copy_(v_.reshape(new_P, k))
+        if self._stats is not None:
+            self._stats = torch.zeros(3, new_P, dtype=torch.float32, device=self.dev) if stats is None else \
+                stats.contiguous()
         self.frame = Frame(self.dev, new_P, self.W, self.H)   # the next forward sizes its binning buffer
         self._mip_setup()
         self._keep = None
@@ -591,7 +678,8 @@ class JointTrainer:
         """Remove the Gaussians where `mask` [P] is True."""
         keep = ~mask.to(self.dev).bool()
         ppl = None if self.per_point_lr is None else self.per_point_lr[:self.P][keep]
-        self._resize(int(keep.sum()), lambda name, p, m, v: (p[keep], m[keep], v[keep]))
+        stats = None if self._stats is None else self._stats[:, keep]
+        self._resize(int(keep.sum()), lambda name, p, m, v: (p[keep], m[keep], v[keep]), stats)
         self._set_per_point_lr(ppl)
 
     def densification_postfix(self, new_xyz, new_features_dc, new_features_rest, new_opacities, new_scaling,
@@ -614,6 +702,23 @@ class JointTrainer:
 
         self._resize(self.P + n_new, rows)
         self._set_per_point_lr(ppl)
+
+    def densify_and_prune(self, max_grad, min_opacity, extent, max_screen_size, clone_and_split=False, generator=None):
+        """GaussianModel.densify_and_prune on the flat buffers from the accumulated statistics: the rows of
+        densify.densify_plan (the mirror's), one rebuild; returns the plan."""
+        if self._stats is None:
+            raise _lib.GsbError("densify_and_prune needs the densification statistics (OptimConfig.densify=True)")
+        v = lambda name: self.view(self.params, name)
+        plan = densify_plan(v("xyz"), v("scaling"), v("rotation"), v("opacity"), self.xyz_gradient_accum, self.denom,
+                            self.max_radii2D, max_grad, min_opacity, extent, max_screen_size, self.cfg.percent_dense,
+                            clone_and_split, generator)
+        computed = dict(xyz=plan.split_xyz, scaling=plan.split_scaling)
+        ppl = None if self.per_point_lr is None else plan.gather(self.per_point_lr[:self.P])
+        stats = None if plan.reset_stats else self._stats[:, plan.src]
+        self._resize(plan.P, lambda name, p, m, v_: (plan.gather(p, computed.get(name)), plan.moments(m),
+                                                      plan.moments(v_)), stats)
+        self._set_per_point_lr(ppl)
+        return plan
 
     def reset_opacity(self) -> None:
         op = self.view(self.params, "opacity")
