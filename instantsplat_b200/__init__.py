@@ -14,7 +14,7 @@ from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, rast
 from .renderer import render  # noqa: F401
 from .ssim import fused_ssim, fused_training_loss  # noqa: F401
 from .per_point_adam import PerPointAdam  # noqa: F401
-from .trainer import JointTrainer, OptimConfig  # noqa: F401
+from .trainer import CHECKPOINT_KEY, JointTrainer, OptimConfig, read_checkpoint  # noqa: F401
 from .model import GaussianModel, PipelineDefaults, SimpleGaussianModel, optimization_defaults  # noqa: F401
 from .knn import distCUDA2  # noqa: F401
 from .densify import cameras_extent, densify_plan  # noqa: F401

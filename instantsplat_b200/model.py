@@ -1,7 +1,8 @@
 """Host-side mirror of the part of the reference's `GaussianModel` that the training hot path touches
 (scene/gaussian_model.py): parameter tensors and their activations (:101-121), the pose table
 (:126-136), `oneupSHdegree` (:142-144), `create_from_pcd` (:146-172, with `distCUDA2` served by libgsb200.so),
-`training_setup_pp` (:203-232), `update_learning_rate` (:234-243) and the optimizer-state surgery behind
+`capture` / `restore` (:65-99), `training_setup` (:174-200), `training_setup_pp` (:203-232),
+`update_learning_rate` (:234-243) and the optimizer-state surgery behind
 densify / prune / opacity reset (:280-283, :328-478; SURVEY.md section 8 row f4).
 
 Same attribute and method names, argument meaning and param-group layout as the reference, so that the body of
@@ -185,6 +186,49 @@ class GaussianModel:
         self.cam_scheduler_args = get_expon_lr_func(lr_init=a.rotation_lr * 0.1, lr_final=a.rotation_lr * 0.001,
                                                     lr_delay_mult=a.position_lr_delay_mult, max_steps=a.iterations)
         return self.optimizer
+
+    def training_setup(self, training_args=None):
+        """Reference :174-200: the groups and learning rates of training_setup_pp, without the per-point multiplier, on
+        torch.optim.Adam."""
+        a = training_args or optimization_defaults()
+        self.percent_dense = a.percent_dense
+        n = self.get_xyz.shape[0]
+        self.xyz_gradient_accum = torch.zeros(n, 1, device=self.device)
+        self.denom = torch.zeros(n, 1, device=self.device)
+        lrs = dict(xyz=a.position_lr_init * self.spatial_lr_scale, f_dc=a.feature_lr * 10,
+                   f_rest=a.feature_lr / 20.0 * 10, opacity=a.opacity_lr, scaling=a.scaling_lr * 10,
+                   rotation=a.rotation_lr * 10)
+        groups = [{"params": [getattr(self, self._ATTR[g])], "lr": lrs[g], "name": g} for g in self._GROUPS]
+        groups.append({"params": [self.P], "lr": a.rotation_lr * 0.1, "name": "pose"})
+        self.optimizer = torch.optim.Adam(groups, lr=0.0, eps=1e-15)
+        self.xyz_scheduler_args = get_expon_lr_func(lr_init=a.position_lr_init * self.spatial_lr_scale,
+                                                    lr_final=a.position_lr_final * self.spatial_lr_scale,
+                                                    lr_delay_mult=a.position_lr_delay_mult,
+                                                    max_steps=a.position_lr_max_steps)
+        self.cam_scheduler_args = get_expon_lr_func(lr_init=a.rotation_lr * 0.1, lr_final=a.rotation_lr * 0.001,
+                                                    lr_delay_mult=a.position_lr_delay_mult, max_steps=a.iterations)
+        return self.optimizer
+
+    # ---- checkpoints (reference :65-99; train.py:103-105, :225-227) ---------------------------
+    def capture(self):
+        """The reference's 13-tuple, in its order: what train.py saves as chkpnt<N>.pth."""
+        return (self.active_sh_degree, self._xyz, self._features_dc, self._features_rest, self._scaling, self._rotation,
+                self._opacity, self.max_radii2D, self.xyz_gradient_accum, self.denom, self.optimizer.state_dict(),
+                self.spatial_lr_scale, self.P)
+
+    def restore(self, model_args, training_args=None):
+        """Reference :82-99.  Like the reference, this calls training_setup, not training_setup_pp: a restored model
+        continues on torch.optim.Adam without the per-point learning rate, even when the checkpoint was written by a
+        PerPointAdam run (the saved groups, `per_point_lr` key included, replace the new ones; Adam ignores the key).
+        A state dict with extra top-level keys (JointTrainer's checkpoints) loads the same way: load_state_dict reads
+        only `state` and `param_groups`."""
+        (self.active_sh_degree, self._xyz, self._features_dc, self._features_rest, self._scaling, self._rotation,
+         self._opacity, self.max_radii2D, xyz_gradient_accum, denom, opt_dict, self.spatial_lr_scale,
+         self.P) = model_args
+        self.training_setup(training_args)
+        self.xyz_gradient_accum = xyz_gradient_accum
+        self.denom = denom
+        self.optimizer.load_state_dict(opt_dict)
 
     def update_learning_rate(self, iteration):
         for group in self.optimizer.param_groups:

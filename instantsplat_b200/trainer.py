@@ -22,6 +22,7 @@ from typing import Dict, List, Optional
 
 import numpy as np
 import torch
+from torch import nn
 
 from . import _lib
 from ._lib import GsbGaussians, GsbGrads, check
@@ -117,6 +118,7 @@ class JointTrainer:
         self._fused = self.exchange in ("fused_p2p", "fused_p2p_nccl")
         self.P = P = scene.P
         self.W, self.H = scene.width, scene.height
+        self.fovx, self.fovy = float(scene.fovx), float(scene.fovy)
         self.sh_degree = scene.sh_degree
         self.n_views = scene.n_views
         # ---- flat buffers
@@ -728,6 +730,186 @@ class JointTrainer:
         self.view(self.exp_avg, "opacity").zero_()
         self.view(self.exp_avg_sq, "opacity").zero_()
 
+    # ---- save points (train.py:103-105, :220-227; DESIGN.md section 4.9) ---------------------------------------
+    def _shapes(self):
+        m1 = dict(SEGMENTS)["f_rest"] // 3
+        return dict(xyz=(self.P, 3), f_dc=(self.P, 1, 3), f_rest=(self.P, m1, 3), opacity=(self.P, 1),
+                    scaling=(self.P, 3), rotation=(self.P, 4))
+
+    def _group_lrs(self):
+        """The `lr` of every param group as the reference's optimizer holds it after update_learning_rate(iteration)
+        (before the first iteration: training_setup_pp's initial values)."""
+        c = self.cfg
+        lrs = self._lrs()
+        if self.iteration == 0:
+            lrs["xyz"], pose = c.position_lr_init * c.spatial_lr_scale, c.rotation_lr * 0.1
+        else:
+            pose = self.cam_sched(self.iteration)
+        return [float(lrs[name]) for name, _ in SEGMENTS] + [float(pose)]
+
+    def capture(self):
+        """The reference's 13-tuple (GaussianModel.capture) built from the flat buffers: copies, as nn.Parameters on
+        this device; a PerPointAdam state dict (seven groups, current LRs, `step` = step_count(name)) that also carries
+        what the tuple has no slot for under CHECKPOINT_KEY."""
+        if self.world_size > 1:
+            raise _lib.GsbError("checkpoints need world_size == 1: the fused exchange shards the Adam moments")
+        shapes = self._shapes()
+        prm = {name: nn.Parameter(self.view(self.params, name).reshape(shapes[name]).clone()) for name, _ in SEGMENTS}
+        pose = nn.Parameter(self.poses.clone())
+        groups, state = [], {}
+        for i, ((name, _), lr) in enumerate(zip(SEGMENTS + (("pose", 7),), self._group_lrs())):
+            ppl = None
+            if name == "xyz" and self.per_point_lr is not None:
+                ppl = self.per_point_lr[:self.P].reshape(self.P, 1).clone()
+            groups.append(dict(lr=lr, betas=(0.9, 0.999), eps=1e-15, weight_decay=0.0, per_point_lr=ppl, name=name,
+                               params=[i]))
+            if name == "pose":
+                if self.cfg.optim_pose and self.opt_step > 0:
+                    state[i] = dict(step=self.opt_step, exp_avg=self.pose_m.clone(), exp_avg_sq=self.pose_v.clone())
+            elif self.step_count(name) > 0:
+                state[i] = dict(step=self.step_count(name),
+                                exp_avg=self.view(self.exp_avg, name).reshape(shapes[name]).clone(),
+                                exp_avg_sq=self.view(self.exp_avg_sq, name).reshape(shapes[name]).clone())
+        c = self.cfg
+        gen = getattr(self, "densify_generator", None)
+        extra = dict(
+            version=1, iteration=self.iteration, opt_step=self.opt_step, lag=dict(self._lag),
+            densify_generator=None if gen is None else gen.get_state(),
+            scene_extent=getattr(self, "scene_extent", None),
+            filter_3D=None if self.filter_3D is None else self.filter_3D.clone(),
+            mip_recomputed_at=list(self.mip_recomputed_at), densified_at=list(self.densified_at),
+            reset_at=list(self.reset_at),
+            cfg={k: getattr(c, k) for k in dir(OptimConfig) if not k.startswith("_")},
+            frame=dict(W=self.W, H=self.H, fovx=self.fovx, fovy=self.fovy,
+                       bg=[float(b) for b in self.ident.bg.tolist()], n_views=self.n_views, sh_degree=self.sh_degree))
+        sd = {"state": state, "param_groups": groups, CHECKPOINT_KEY: extra}
+        if self._stats is not None:
+            accum, denom, radii = self.xyz_gradient_accum.clone(), self.denom.clone(), self.max_radii2D.clone()
+        else:
+            accum = torch.zeros(self.P, 1, device=self.dev)
+            denom, radii = torch.zeros_like(accum), torch.zeros(self.P, device=self.dev)
+        return (self.active_sh_degree, prm["xyz"], prm["f_dc"], prm["f_rest"], prm["scaling"], prm["rotation"],
+                prm["opacity"], radii, accum, denom, sd, float(c.spatial_lr_scale), pose)
+
+    def save_checkpoint(self, path: str) -> None:
+        """train.py:225-227: torch.save((capture(), iteration), path).  train.py:104 reads it back unchanged, and so does
+        torch.load's default weights_only=True (tensors, nn.Parameter, dicts, lists, tuples and primitives only)."""
+        torch.save((self.capture(), self.iteration), path)
+
+    def load_checkpoint(self, path: str) -> None:
+        """Continue from a checkpoint: this trainer's frame, views and SH layout, the checkpoint's Gaussians."""
+        self.restore(*read_checkpoint(path, self.dev))
+
+    @classmethod
+    def from_checkpoint(cls, path: str, scene: Scene, gt_images: Optional[torch.Tensor] = None,
+                        cfg: Optional[OptimConfig] = None, device="cuda", use_graph: bool = False) -> "JointTrainer":
+        """A trainer that continues the run saved in `path` on `scene`'s views (frame size, intrinsics, background,
+        number of views, SH layout; its Gaussians are replaced by the checkpoint's).  cfg=None: the OptimConfig the
+        checkpoint was written with (the defaults for a checkpoint without JointTrainer's state)."""
+        model_args, first_iter = read_checkpoint(path, torch.device(device))
+        if cfg is None:
+            cfg = OptimConfig()
+            extra = model_args[10].get(CHECKPOINT_KEY) if isinstance(model_args[10], dict) else None
+            for k, v in (extra or {}).get("cfg", {}).items():
+                if hasattr(OptimConfig, k):
+                    setattr(cfg, k, v)
+        tr = cls(scene, device, gt_images=gt_images, cfg=cfg, use_graph=use_graph)
+        tr.restore(model_args, first_iter)
+        return tr
+
+    def restore(self, model_args, first_iter: int) -> None:
+        """Load a capture()d tuple (this trainer's or the reference's / mirror's) and continue after iteration
+        `first_iter`.  With CHECKPOINT_KEY present the continuation is bit-identical to the run that was not stopped.
+        Without it (DESIGN.md section 4.9): opt_step and the lags come from the per-group step counts, the densify
+        generator restarts from densify_seed, filter_3D is recomputed from the restored xyz and poses, and the update
+        stays PerPointAdam's (the reference's restore switches to torch.optim.Adam)."""
+        if self.world_size > 1:
+            raise _lib.GsbError("checkpoints need world_size == 1: the fused exchange shards the Adam moments, and "
+                                "multi-GPU resume is not implemented")
+        t = _parse_capture(model_args, first_iter)
+        extra = t["extra"]
+        P, n_views = t["P"], t["pose"].shape[0]
+        if n_views != self.n_views:
+            raise _lib.GsbError(f"checkpoint: the pose table has {n_views} views, the scene {self.n_views}")
+        shapes = self._shapes()
+        m1 = shapes["f_rest"][1]
+        if tuple(t["f_rest"].shape[1:]) != (m1, 3):
+            raise _lib.GsbError(f"checkpoint: f_rest is {tuple(t['f_rest'].shape)}, the trainer's SH layout needs "
+                                f"[P,{m1},3]")
+        if not 0 <= t["active_sh_degree"] <= self.cfg.max_sh_degree:
+            raise _lib.GsbError(f"checkpoint: active_sh_degree {t['active_sh_degree']} is out of range")
+        if extra is not None:
+            fr = extra["frame"]
+            mine = dict(W=self.W, H=self.H, fovx=self.fovx, fovy=self.fovy,
+                        bg=[float(b) for b in self.ident.bg.tolist()], n_views=self.n_views, sh_degree=self.sh_degree)
+            bad = [k for k in mine if fr.get(k) != mine[k]]
+            if bad:
+                raise _lib.GsbError("checkpoint: written for another frame: " +
+                                    ", ".join(f"{k} {fr.get(k)} != {mine[k]}" for k in bad))
+        steps = t["steps"]
+        if extra is not None:
+            opt_step, lag = int(extra["opt_step"]), {name: int(extra["lag"][name]) for name, _ in SEGMENTS}
+            want = {name: opt_step - lag[name] for name, _ in SEGMENTS if opt_step - lag[name] > 0}
+            if "pose" in steps:
+                want["pose"] = opt_step
+            if steps != want:
+                raise _lib.GsbError(f"checkpoint: step counts {steps} disagree with opt_step {opt_step} and the lags")
+        else:
+            opt_step = steps.get("pose", 0) or max(steps.get(name, 0) for name, _ in SEGMENTS)
+            lag = {name: opt_step - steps.get(name, 0) for name, _ in SEGMENTS}
+        dev = self.dev
+        self.poses.copy_(t["pose"].to(dev))
+        for buf, key in ((self.pose_m, "m"), (self.pose_v, "v")):
+            mv = t["moments"].get("pose")
+            buf.copy_(mv[key].to(dev)) if mv is not None else buf.zero_()
+        stats = None
+        if self._stats is not None:
+            stats = torch.stack((t["xyz_gradient_accum"].reshape(P), t["denom"].reshape(P),
+                                 t["max_radii2D"].reshape(P))).to(dev).float()
+
+        def rows(name, p, m, v):
+            k = dict(SEGMENTS)[name]
+            new = t[name].detach().to(dev).float().reshape(P, k)
+            mv = t["moments"].get(name)
+            if mv is None:
+                return new, torch.zeros_like(new), torch.zeros_like(new)
+            return new, mv["m"].to(dev).float().reshape(P, k), mv["v"].to(dev).float().reshape(P, k)
+
+        self._resize(P, rows, stats)         # also rebuilds the Frame, clears the graphs, recomputes filter_3D
+        ppl = t["per_point_lr"]
+        self._set_per_point_lr(ppl if self.cfg.pp_optimizer else None)
+        self.iteration, self.opt_step, self._lag = int(first_iter), opt_step, lag
+        self.active_sh_degree = t["active_sh_degree"]
+        self.densified_at, self.reset_at = [], []
+        if self.filt is not None:
+            self.mip_recomputed_at = []
+        if extra is not None:
+            self.densified_at, self.reset_at = list(extra["densified_at"]), list(extra["reset_at"])
+            if self.filt is not None:
+                self.mip_recomputed_at = list(extra["mip_recomputed_at"])
+                if extra["filter_3D"] is not None:
+                    self.filter_3D.copy_(extra["filter_3D"].to(dev).reshape(P))
+        if self._stats is not None:
+            if extra is not None and extra["scene_extent"] is not None:
+                self.scene_extent = float(extra["scene_extent"])
+            gen = None if extra is None else extra["densify_generator"]
+            if gen is not None:
+                self.densify_generator.set_state(gen.cpu())
+            else:
+                self.densify_generator.manual_seed(int(self.cfg.densify_seed))
+
+    def save_ply(self, path: str) -> None:
+        """scene.save: point_cloud.ply of the current Gaussians (with the filter_3D property when Mip is on)."""
+        from .scene_io import save_gaussians_ply
+        v = lambda name: self.view(self.params, name).cpu().numpy()
+        save_gaussians_ply(path, v("xyz"), v("f_dc"), v("f_rest"), v("opacity"), v("scaling"), v("rotation"),
+                           None if self.filter_3D is None else self.filter_3D.cpu().numpy())
+
+    def save_poses(self, path: str, colmap_ids: Optional[List[int]] = None):
+        """train.py save_pose: the pose table as [n_views,4,4] world-to-camera matrices in COLMAP id order."""
+        from .scene_io import save_pose_npy
+        return save_pose_npy(path, self.poses.detach().cpu().numpy(), colmap_ids)
+
     def blend_stats(self, view: int, gt: Optional[torch.Tensor] = None) -> Dict[str, int]:
         """Pair statistics of the blend kernels for one forward+backward of `view` (instrumented re-run of the same
         kernels, outside any timed region): evaluated / contributing (pixel, Gaussian) pairs."""
@@ -756,3 +938,89 @@ class JointTrainer:
             loss=HW * 36,
             adam=59 * P * 28 + P * 4,
         )
+
+
+# ---- checkpoint files (DESIGN.md section 4.9) ----------------------------------------------------------------------
+# The top-level key of the optimizer state dict under which JointTrainer stores what the reference tuple has no slot for;
+# torch.optim.Optimizer.load_state_dict reads only "state" and "param_groups", so the reference's restore() ignores it.
+CHECKPOINT_KEY = "joint_trainer"
+_GROUP_NAMES = tuple(name for name, _ in SEGMENTS) + ("pose",)
+_EXTRA_KEYS = ("iteration", "opt_step", "lag", "densify_generator", "scene_extent", "filter_3D", "mip_recomputed_at",
+               "densified_at", "reset_at", "cfg", "frame")
+
+
+def read_checkpoint(path: str, device=None):
+    """(model_args, first_iter) of a train.py checkpoint, with torch.load's default weights_only=True.  The reference's
+    (and the mirror's) state dicts hold the scheduled learning rates as numpy float64 scalars, so those two numpy globals
+    are allowed as well; JointTrainer writes Python floats."""
+    mod = getattr(np, "_core", None) or np.core
+    with torch.serialization.safe_globals([mod.multiarray.scalar, np.dtype, type(np.dtype(np.float64))]):
+        obj = torch.load(path, map_location=device)
+    if not (isinstance(obj, (tuple, list)) and len(obj) == 2):
+        raise _lib.GsbError(f"checkpoint {path}: expected (model_params, first_iter), got {type(obj).__name__}")
+    return obj[0], obj[1]
+
+
+def _parse_capture(model_args, first_iter) -> dict:
+    """Check a GaussianModel.capture() tuple entry by entry; returns its parts by name, the moments and step count of
+    every param group by group name, and the extra state (None when absent)."""
+    def bad(msg):
+        raise _lib.GsbError("checkpoint: " + msg)
+
+    if not (isinstance(model_args, (tuple, list)) and len(model_args) == 13):
+        bad("model_params must be GaussianModel.capture()'s 13-tuple")
+    if isinstance(first_iter, bool) or not isinstance(first_iter, int) or first_iter < 0:
+        bad(f"first_iter must be a non-negative int, got {first_iter!r}")
+    names = ("active_sh_degree", "xyz", "f_dc", "f_rest", "scaling", "rotation", "opacity", "max_radii2D",
+             "xyz_gradient_accum", "denom", "optimizer", "spatial_lr_scale", "pose")
+    t = dict(zip(names, model_args))
+    if isinstance(t["active_sh_degree"], bool) or not isinstance(t["active_sh_degree"], int):
+        bad("active_sh_degree must be an int")
+    for k in names[1:10] + ("pose",):
+        if not torch.is_tensor(t[k]):
+            bad(f"{k} must be a tensor, got {type(t[k]).__name__}")
+    P = int(t["xyz"].shape[0]) if t["xyz"].dim() == 2 else -1
+    want = dict(xyz=(P, 3), f_dc=(P, 1, 3), scaling=(P, 3), rotation=(P, 4), opacity=(P, 1), max_radii2D=(P,),
+                xyz_gradient_accum=(P, 1), denom=(P, 1))
+    for k, s in want.items():
+        if tuple(t[k].shape) != s:
+            bad(f"{k} has shape {tuple(t[k].shape)}, expected {s}")
+    if t["f_rest"].dim() != 3 or t["f_rest"].shape[0] != P or t["f_rest"].shape[2] != 3:
+        bad(f"f_rest has shape {tuple(t['f_rest'].shape)}, expected [P,M-1,3]")
+    if t["pose"].dim() != 2 or t["pose"].shape[1] != 7:
+        bad(f"the pose table has shape {tuple(t['pose'].shape)}, expected [n_views,7]")
+    sd = t["optimizer"]
+    if not (isinstance(sd, dict) and isinstance(sd.get("state"), dict) and isinstance(sd.get("param_groups"), list)):
+        bad("the optimizer state dict needs 'state' and 'param_groups'")
+    groups = {}
+    for g in sd["param_groups"]:
+        if not (isinstance(g, dict) and g.get("name") in _GROUP_NAMES and len(g.get("params", ())) == 1):
+            bad(f"unexpected param group {g.get('name') if isinstance(g, dict) else g!r}")
+        groups[g["name"]] = g
+    if sorted(groups) != sorted(_GROUP_NAMES) or len(sd["param_groups"]) != len(_GROUP_NAMES):
+        bad(f"param groups {[g.get('name') for g in sd['param_groups']]}, expected {list(_GROUP_NAMES)}")
+    steps, moments = {}, {}
+    for name, g in groups.items():
+        st = sd["state"].get(g["params"][0])
+        if not st:
+            continue
+        shape = tuple(t[name].shape)
+        if not all(k in st for k in ("step", "exp_avg", "exp_avg_sq")) or \
+                any(not torch.is_tensor(st[k]) or tuple(st[k].shape) != shape for k in ("exp_avg", "exp_avg_sq")):
+            bad(f"the optimizer state of '{name}' needs step, exp_avg and exp_avg_sq of shape {shape}")
+        steps[name] = int(float(st["step"]))
+        moments[name] = dict(m=st["exp_avg"], v=st["exp_avg_sq"])
+    ppl = groups["xyz"].get("per_point_lr")
+    if ppl is not None and not (torch.is_tensor(ppl) and ppl.numel() == P):
+        bad("the xyz group's per_point_lr must be a tensor with one value per Gaussian")
+    extra = sd.get(CHECKPOINT_KEY)
+    if extra is not None:
+        missing = [k for k in _EXTRA_KEYS if k not in extra] if isinstance(extra, dict) else list(_EXTRA_KEYS)
+        if missing:
+            bad(f"'{CHECKPOINT_KEY}' lacks {missing}")
+        if int(extra["iteration"]) != first_iter:
+            bad(f"first_iter {first_iter} differs from the saved iteration {extra['iteration']}")
+        if extra["filter_3D"] is not None and extra["filter_3D"].numel() != P:
+            bad("filter_3D must have one value per Gaussian")
+    t.update(P=P, steps=steps, moments=moments, extra=extra, per_point_lr=None if ppl is None else ppl.reshape(P))
+    return t
