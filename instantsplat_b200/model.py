@@ -20,7 +20,7 @@ import torch
 from torch import nn
 
 from .per_point_adam import PerPointAdam
-from .trainer import get_expon_lr_func
+from .trainer import ADAM_BETAS, ADAM_EPS, OptimConfig, group_lrs, lr_schedules
 
 SH_C0 = 0.28209479177387814
 
@@ -30,19 +30,19 @@ def inverse_sigmoid(x):
 
 
 def optimization_defaults(**over):
-    """arguments/__init__.py:73-94 (OptimizationParams defaults; InstantSplat's scripts pass
+    """arguments/__init__.py:73-94 (OptimizationParams defaults, as in OptimConfig; InstantSplat's scripts pass
     --iterations 1000 --pp_optimizer --optim_pose)."""
-    d = dict(iterations=30_000, position_lr_init=0.00016, position_lr_final=0.0000016, position_lr_delay_mult=0.01,
-             position_lr_max_steps=30_000, feature_lr=0.0025, opacity_lr=0.05, scaling_lr=0.005, rotation_lr=0.001,
-             percent_dense=0.01, lambda_dssim=0.2, densification_interval=100, opacity_reset_interval=3000,
-             densify_from_iter=500, densify_until_iter=15_000, densify_grad_threshold=0.0002,
-             random_background=False, pp_optimizer=True, optim_pose=True)
+    keys = ("iterations", "position_lr_init", "position_lr_final", "position_lr_delay_mult", "position_lr_max_steps",
+            "feature_lr", "opacity_lr", "scaling_lr", "rotation_lr", "percent_dense", "lambda_dssim",
+            "densification_interval", "opacity_reset_interval", "densify_from_iter", "densify_until_iter",
+            "densify_grad_threshold", "pp_optimizer", "optim_pose")
+    d = {k: getattr(OptimConfig, k) for k in keys}
+    d["random_background"] = False
     d.update(over)
     return SimpleNamespace(**d)
 
 
 class GaussianModel:
-    _GROUPS = ("xyz", "f_dc", "f_rest", "opacity", "scaling", "rotation")
     _ATTR = dict(xyz="_xyz", f_dc="_features_dc", f_rest="_features_rest", opacity="_opacity", scaling="_scaling",
                  rotation="_rotation")
 
@@ -151,63 +151,42 @@ class GaussianModel:
     def from_scene(cls, scene, device="cuda", active_sh_degree: Optional[int] = None):
         """Bench / test helper: parameters and poses of a synthetic `Scene` (instantsplat_b200/scenes.py)."""
         m = cls(3, device)
-        m._set_params(scene.params)
-        m.active_sh_degree = scene.sh_degree if active_sh_degree is None else active_sh_degree
-        m.init_RT_seq(scene.poses)
-        m.per_point_lr = None if scene.per_point_lr is None else scene.per_point_lr.to(m.device).float().reshape(-1, 1)
-        m.max_radii2D = torch.zeros(scene.P, device=m.device)
-        m.spatial_lr_scale = 1.0
+        m._fill_from_scene(scene, active_sh_degree)
         return m
 
-    # ---- optimizer (reference :203-243) ------------------------------------------------------
+    def _fill_from_scene(self, scene, active_sh_degree: Optional[int]):
+        self._set_params(scene.params)
+        self.active_sh_degree = scene.sh_degree if active_sh_degree is None else active_sh_degree
+        self.init_RT_seq(scene.poses)
+        self.per_point_lr = None if scene.per_point_lr is None else scene.per_point_lr.to(self.device).float().reshape(-1, 1)
+        self.max_radii2D = torch.zeros(scene.P, device=self.device)
+        self.spatial_lr_scale = 1.0
+
+    # ---- optimizer (reference :174-243) ------------------------------------------------------
     def training_setup_pp(self, training_args=None, confidence_lr=None):
-        a = training_args or optimization_defaults()
         if confidence_lr is not None:
             self.per_point_lr = confidence_lr
-        n = self.get_xyz.shape[0]
-        self.percent_dense = a.percent_dense
-        self.xyz_gradient_accum = torch.zeros(n, 1, device=self.device)
-        self.denom = torch.zeros(n, 1, device=self.device)
-        lrs = dict(xyz=a.position_lr_init * self.spatial_lr_scale, f_dc=a.feature_lr * 10,
-                   f_rest=a.feature_lr / 20.0 * 10, opacity=a.opacity_lr, scaling=a.scaling_lr * 10,
-                   rotation=a.rotation_lr * 10)
-        groups = []
-        for g in self._GROUPS:
-            grp = {"params": [getattr(self, self._ATTR[g])], "lr": lrs[g], "name": g}
-            if g == "xyz":
-                grp["per_point_lr"] = self.per_point_lr
-            groups.append(grp)
-        groups.append({"params": [self.P], "lr": a.rotation_lr * 0.1, "name": "pose"})
-        self.optimizer = PerPointAdam(groups, lr=0, betas=(0.9, 0.999), eps=1e-15, weight_decay=0.0)
-        self.xyz_scheduler_args = get_expon_lr_func(lr_init=a.position_lr_init * self.spatial_lr_scale,
-                                                    lr_final=a.position_lr_final * self.spatial_lr_scale,
-                                                    lr_delay_mult=a.position_lr_delay_mult,
-                                                    max_steps=a.position_lr_max_steps)
-        self.cam_scheduler_args = get_expon_lr_func(lr_init=a.rotation_lr * 0.1, lr_final=a.rotation_lr * 0.001,
-                                                    lr_delay_mult=a.position_lr_delay_mult, max_steps=a.iterations)
+        groups = self._setup_groups(training_args or optimization_defaults())
+        groups[0]["per_point_lr"] = self.per_point_lr
+        self.optimizer = PerPointAdam(groups, lr=0, betas=ADAM_BETAS, eps=ADAM_EPS, weight_decay=0.0)
         return self.optimizer
 
     def training_setup(self, training_args=None):
         """Reference :174-200: the groups and learning rates of training_setup_pp, without the per-point multiplier, on
         torch.optim.Adam."""
-        a = training_args or optimization_defaults()
-        self.percent_dense = a.percent_dense
+        self.optimizer = torch.optim.Adam(self._setup_groups(training_args or optimization_defaults()), lr=0.0,
+                                          eps=ADAM_EPS)
+        return self.optimizer
+
+    def _setup_groups(self, a):
+        """What both setups share: the densification statistics, the two schedules and the seven param groups."""
         n = self.get_xyz.shape[0]
+        self.percent_dense = a.percent_dense
         self.xyz_gradient_accum = torch.zeros(n, 1, device=self.device)
         self.denom = torch.zeros(n, 1, device=self.device)
-        lrs = dict(xyz=a.position_lr_init * self.spatial_lr_scale, f_dc=a.feature_lr * 10,
-                   f_rest=a.feature_lr / 20.0 * 10, opacity=a.opacity_lr, scaling=a.scaling_lr * 10,
-                   rotation=a.rotation_lr * 10)
-        groups = [{"params": [getattr(self, self._ATTR[g])], "lr": lrs[g], "name": g} for g in self._GROUPS]
-        groups.append({"params": [self.P], "lr": a.rotation_lr * 0.1, "name": "pose"})
-        self.optimizer = torch.optim.Adam(groups, lr=0.0, eps=1e-15)
-        self.xyz_scheduler_args = get_expon_lr_func(lr_init=a.position_lr_init * self.spatial_lr_scale,
-                                                    lr_final=a.position_lr_final * self.spatial_lr_scale,
-                                                    lr_delay_mult=a.position_lr_delay_mult,
-                                                    max_steps=a.position_lr_max_steps)
-        self.cam_scheduler_args = get_expon_lr_func(lr_init=a.rotation_lr * 0.1, lr_final=a.rotation_lr * 0.001,
-                                                    lr_delay_mult=a.position_lr_delay_mult, max_steps=a.iterations)
-        return self.optimizer
+        self.xyz_scheduler_args, self.cam_scheduler_args = lr_schedules(a, self.spatial_lr_scale)
+        return [{"params": [self.P if g == "pose" else getattr(self, self._ATTR[g])], "lr": lr, "name": g}
+                for g, lr in group_lrs(a, self.spatial_lr_scale).items()]
 
     # ---- checkpoints (reference :65-99; train.py:103-105, :225-227) ---------------------------
     def capture(self):
@@ -443,12 +422,7 @@ class SimpleGaussianModel(GaussianModel):
 
     def __init__(self, scene, device="cuda", sh_degree=None):
         super().__init__(3, device)
-        self._set_params(scene.params)
-        self.active_sh_degree = scene.sh_degree if sh_degree is None else sh_degree
-        self.init_RT_seq(scene.poses)
-        self.per_point_lr = None if scene.per_point_lr is None else scene.per_point_lr.to(self.device).float().reshape(-1, 1)
-        self.max_radii2D = torch.zeros(scene.P, device=self.device)
-        self.spatial_lr_scale = 1.0
+        self._fill_from_scene(scene, sh_degree)
 
 
 class PipelineDefaults:

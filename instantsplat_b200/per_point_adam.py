@@ -18,7 +18,7 @@ def launch_adam(entries, flags, skip_ptr=None, step_sizes_dev=None):
     """entries: list of dicts(param, grad, exp_avg, exp_avg_sq, per_point_lr, step_size, beta1, beta2,
     eps, weight_decay, grad_scale, row_len).  skip_ptr: optional device address of a word that, when non-zero,
     makes the device skip the whole update (gsb_adam_step_gated).  step_sizes_dev: optional fp32 device tensor with one
-    step size per entry, read by the kernel instead of the launch arguments (CUDA-graph replay)."""
+    step size per entry, read by the kernel instead of the entries' `step_size` (then not needed)."""
     if step_sizes_dev is not None and len(entries) > ADAM_MAX_TENSORS:
         raise _lib.GsbError("device-side step sizes support at most one launch (8 tensors)")
     L = _lib.lib()
@@ -39,7 +39,8 @@ def _launch_adam_on_device(L, entries, flags, skip_ptr, step_sizes_dev):
             t.per_point_lr = None if ppl is None else ppl.data_ptr()
             t.numel, t.row_len = e["param"].numel(), int(e.get("row_len", 1))
             t.grad_scale = float(e.get("grad_scale", 1.0))
-            t.step_size, t.beta1, t.beta2 = float(e["step_size"]), float(e["beta1"]), float(e["beta2"])
+            t.step_size = 0.0 if step_sizes_dev is not None else float(e["step_size"])
+            t.beta1, t.beta2 = float(e["beta1"]), float(e["beta2"])
             t.eps, t.weight_decay = float(e["eps"]), float(e["weight_decay"])
         check(L.gsb_adam_step_ex(len(chunk), arr, flags.data_ptr(), skip_ptr,
                                  None if step_sizes_dev is None else step_sizes_dev.data_ptr(), _lib.stream_ptr()),

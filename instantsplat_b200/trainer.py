@@ -34,6 +34,7 @@ from .per_point_adam import launch_adam
 from .scenes import Scene
 
 SEGMENTS = (("xyz", 3), ("f_dc", 3), ("f_rest", 45), ("opacity", 1), ("scaling", 3), ("rotation", 4))
+ADAM_BETAS, ADAM_EPS = (0.9, 0.999), 1e-15       # training_setup_pp's PerPointAdam (scene/gaussian_model.py:221)
 
 
 def get_expon_lr_func(lr_init, lr_final, lr_delay_steps=0, lr_delay_mult=1.0, max_steps=1000000):
@@ -92,12 +93,52 @@ class OptimConfig:
     densify_seed = 0                 # seed of the generator the split samples are drawn from
 
 
+def lr_schedules(args, spatial_lr_scale):
+    """training_setup_pp's xyz and pose learning-rate schedules (scene/gaussian_model.py:223-232).  args: anything with
+    the OptimizationParams field names (OptimConfig, optimization_defaults())."""
+    xyz = get_expon_lr_func(args.position_lr_init * spatial_lr_scale, args.position_lr_final * spatial_lr_scale,
+                            lr_delay_mult=args.position_lr_delay_mult, max_steps=args.position_lr_max_steps)
+    pose = get_expon_lr_func(args.rotation_lr * 0.1, args.rotation_lr * 0.001, lr_delay_mult=args.position_lr_delay_mult,
+                             max_steps=args.iterations)
+    return xyz, pose
+
+
+def group_lrs(args, spatial_lr_scale, iteration: Optional[int] = None) -> Dict[str, float]:
+    """The `lr` of the seven param groups (SEGMENTS order, then "pose"): training_setup_pp's initial values, or, given
+    an iteration, those after update_learning_rate(iteration)."""
+    lrs = dict(xyz=args.position_lr_init * spatial_lr_scale, f_dc=args.feature_lr * 10,
+               f_rest=args.feature_lr / 20.0 * 10, opacity=args.opacity_lr, scaling=args.scaling_lr * 10,
+               rotation=args.rotation_lr * 10, pose=args.rotation_lr * 0.1)
+    if iteration is not None:
+        xyz, pose = lr_schedules(args, spatial_lr_scale)
+        lrs.update(xyz=xyz(iteration), pose=pose(iteration))
+    return lrs
+
+
+def adam_step_sizes(cfg, iteration: int, opt_step: int, lag: Dict[str, int]) -> Dict[str, float]:
+    """PerPointAdam's step size lr * sqrt(1-b2^t)/(1-b1^t) of the seven groups after update_learning_rate(iteration),
+    where t = opt_step - lag[name] is the group's step count (the pose table has no lag).  A group that has taken no
+    step yet gets the size of t = 1; it is not stepped with it."""
+    b1, b2 = ADAM_BETAS
+    out = {}
+    for name, lr in group_lrs(cfg, cfg.spatial_lr_scale, iteration).items():
+        t = max(1, opt_step - lag.get(name, 0))
+        out[name] = lr * ((1 - b2 ** t) ** 0.5 / (1 - b1 ** t))
+    return out
+
+
 def L_sig_words():
     return (_lib.lib().gsb_peer_signal_bytes() + 3) // 4
 
 
-def _align(n, a=64):
-    return (n + a - 1) // a * a
+def _layout(P: int):
+    """Where the SEGMENTS tensors of P Gaussians lie in the flat buffers: {name: (begin, end)}, each segment padded to a
+    multiple of 64 floats (256 bytes), and the buffers' length."""
+    segments, total = {}, 0
+    for name, k in SEGMENTS:
+        segments[name] = (total, total + (P * k + 63) // 64 * 64)
+        total = segments[name][1]
+    return segments, total
 
 
 class JointTrainer:
@@ -122,11 +163,8 @@ class JointTrainer:
         self.sh_degree = scene.sh_degree
         self.n_views = scene.n_views
         # ---- flat buffers
-        offs, total = {}, 0
-        for name, k in SEGMENTS:
-            offs[name] = total
-            total += _align(P * k)
-        self.offs, self.total = offs, total
+        self.segments, self.total = _layout(P)
+        total = self.total
         if self._fused:
             # peer-visible parameter / gradient buffers (CUDA IPC) and shard-sized Adam moments
             from .parallel import PeerBuffer, shard_bounds
@@ -161,11 +199,7 @@ class JointTrainer:
             self.pose_grad = self._pg_buf[:-1].view(scene.n_views, 7)
         self.pose_m = torch.zeros_like(self.poses)
         self.pose_v = torch.zeros_like(self.poses)
-        self.per_point_lr = None
-        if self.cfg.pp_optimizer and scene.per_point_lr is not None:
-            ppl = torch.ones(_align(P * 3) // 3 + 1, dtype=torch.float32, device=self.dev)   # covers the padded tail
-            ppl[:P] = scene.per_point_lr.to(self.dev).float().reshape(P)
-            self.per_point_lr = ppl
+        self._set_per_point_lr(scene.per_point_lr if self.cfg.pp_optimizer else None)
         self.gt = None if gt_images is None else gt_images.to(self.dev).float().contiguous()
         self.ident = IdentityView(self.W, self.H, scene.fovx, scene.fovy, scene.bg, self.dev)
         self.frame = Frame(self.dev, P, self.W, self.H)     # scratch; its binning buffer is sized by the first forward
@@ -190,8 +224,7 @@ class JointTrainer:
         self.use_graph = bool(use_graph) and (world_size == 1 or self.exchange == "fused_p2p")
         self._graphs = {}
         self._after_backward = None   # test hook: called (and captured) between the backward and the optimizer step
-        self._step_host = torch.zeros(8, dtype=torch.float32).pin_memory()
-        self._step_dev = torch.zeros(8, dtype=torch.float32, device=self.dev)
+        self._step_dev = torch.zeros(8, dtype=torch.float32, device=self.dev)   # every update's step sizes (_advance)
         self.frame.status.zero_()     # the forward serial number lives in these words
         self._fwd_count = 0
         self._polling = False
@@ -202,12 +235,6 @@ class JointTrainer:
         self.exact_cull = True
         self.active_sh_degree = min(scene.sh_degree, self.cfg.max_sh_degree)
         c = self.cfg
-        self.xyz_sched = get_expon_lr_func(c.position_lr_init * c.spatial_lr_scale,
-                                           c.position_lr_final * c.spatial_lr_scale,
-                                           lr_delay_mult=c.position_lr_delay_mult,
-                                           max_steps=c.position_lr_max_steps)
-        self.cam_sched = get_expon_lr_func(c.rotation_lr * 0.1, c.rotation_lr * 0.001,
-                                           lr_delay_mult=c.position_lr_delay_mult, max_steps=c.iterations)
         self._keep = None
         # per-tensor Adam step counts are opt_step minus the optimizer steps that skipped the tensor (the densify and
         # opacity-reset iterations replace tensors, which then have no gradient in the reference)
@@ -223,7 +250,7 @@ class JointTrainer:
     # ------------------------------------------------------------------------------------------
     def view(self, flat: torch.Tensor, name: str) -> torch.Tensor:
         k = dict(SEGMENTS)[name]
-        o = self.offs[name]
+        o = self.segments[name][0]
         return flat[o:o + self.P * k].view(self.P, k)
 
     def my_views(self) -> List[int]:
@@ -322,12 +349,25 @@ class JointTrainer:
             self._size_binning(R)
         return True
 
+    def _settled(self, enqueue, local: bool = False) -> None:
+        """enqueue() launches a forward, possibly with the rest of an iteration; then wait for its instance count.  When
+        the binning buffer was too small, the device has skipped the optimizer update by itself (gated on the overflow
+        word, summed over the ranks in multi-GPU mode), so parameters and moments are untouched, and _settle has grown
+        the buffer: enqueue once more.  Several ranks cannot do that within a training iteration, because the other
+        ranks cannot know yet; they stop loudly.  local: only this rank's forward, which any rank may repeat."""
+        for _ in range(2):
+            enqueue()
+            if self._settle():
+                return
+            if self.world_size > 1 and not local:
+                raise _lib.GsbError(f"rank {self.rank}: {self.last_R} instances exceeded the binning capacity; the "
+                                    "optimizer update of this step was skipped on every rank (parameters are "
+                                    "consistent).  Raise JointTrainer.headroom.")
+        raise _lib.GsbError(f"{self.last_R} instances exceeded the binning capacity twice in a row")
+
     def render(self, view: int) -> torch.Tensor:
         """Forward only (exact: repeated with a larger buffer in the unlikely case the capacity was exceeded)."""
-        self._launch_forward(view)
-        if not self._settle():
-            self._launch_forward(view)
-            assert self._settle()
+        self._settled(lambda: self._launch_forward(view), local=True)
         return self.color
 
     def loss_and_backward(self, view: int, gt: torch.Tensor, stats: bool = False) -> None:
@@ -366,57 +406,45 @@ class JointTrainer:
             self._pg_buf[-1:].copy_(self.frame.word(ST_OVERFLOW))
             allreduce_sum_((self.grads, self._pg_buf), self.pg)
 
-    def _step_sizes(self):
-        """lr * sqrt(1-b2^t)/(1-b1^t) per tensor for the current counters (host, double)."""
-        c = self.cfg
-        t = max(1, self.opt_step)
-        corr = (1 - 0.999 ** t) ** 0.5 / (1 - 0.9 ** t)
-        lrs = self._lrs()
-        out = [lrs[name] * self._corr(max(1, self.step_count(name))) for name, _ in SEGMENTS]
-        if c.optim_pose:
-            out.append(self.cam_sched(self.iteration) * corr)
-        return out
+    def _stepped(self, skip=()) -> List[str]:
+        """The tensors an optimizer update steps, in launch order: entry i of the update reads _step_dev[i]."""
+        names = [name for name, _ in SEGMENTS if name not in skip]
+        return names + ["pose"] if self.cfg.optim_pose else names
 
-    def _upload_step_sizes(self) -> None:
-        ss = self._step_sizes()
-        for i, v in enumerate(ss):
-            self._step_host[i] = v
-        self._step_dev.copy_(self._step_host, non_blocking=True)
-
-    @staticmethod
-    def _corr(t: int) -> float:
-        return (1 - 0.999 ** t) ** 0.5 / (1 - 0.9 ** t)
-
-    def optimizer_step(self, grad_scale: Optional[float] = None, _advance: bool = True, _dev_steps: bool = False,
-                       skip=()) -> None:
-        """PerPointAdam.step over the 6 Gaussian tensors + the pose table in one launch
-        (param groups and LRs of scene/gaussian_model.py:203-243).  skip: Gaussian tensors that take no step (they
-        were replaced in this iteration, so the reference's parameter has no gradient); their step counts stay."""
-        c = self.cfg
-        if _advance:
-            self.opt_step += 1
+    def _advance(self, skip=()) -> None:
+        """Count one optimizer step, which the tensors in `skip` do not take (they were replaced in this iteration, so
+        the reference's parameter has no gradient; their step counts stay), and upload the update's step sizes to
+        _step_dev, stream-ordered before whatever is enqueued next.  The pinned staging buffer comes from PyTorch's
+        caching host allocator, which hands it out again only after the copy has run."""
+        self.opt_step += 1
         for name in skip:
             self._lag[name] += 1
-        t = self.opt_step
-        b1, b2, eps = 0.9, 0.999, 1e-15
-        corr = (1 - b2 ** t) ** 0.5 / (1 - b1 ** t)
-        lrs = dict(xyz=self.xyz_sched(self.iteration), f_dc=c.feature_lr * 10, f_rest=c.feature_lr / 20.0 * 10,
-                   opacity=c.opacity_lr, scaling=c.scaling_lr * 10, rotation=c.rotation_lr * 10)
+        sizes = adam_step_sizes(self.cfg, self.iteration, self.opt_step, self._lag)
+        names = self._stepped(skip)
+        host = torch.tensor([float(sizes[name]) for name in names], dtype=torch.float32, pin_memory=True)
+        self._step_dev[:len(names)].copy_(host, non_blocking=True)
+
+    def _adam_entry(self, name: str, grad_scale: float) -> dict:
+        """launch_adam's entry of one tensor ("pose" or a SEGMENTS name); its step size is in _step_dev."""
+        if name == "pose":
+            t = dict(param=self.poses, grad=self.pose_grad, exp_avg=self.pose_m, exp_avg_sq=self.pose_v, row_len=7,
+                     per_point_lr=None)
+        else:
+            t = dict(param=self.view(self.params, name), grad=self.view(self.grads, name),
+                     exp_avg=self.view(self.exp_avg, name), exp_avg_sq=self.view(self.exp_avg_sq, name),
+                     row_len=dict(SEGMENTS)[name], per_point_lr=self.per_point_lr if name == "xyz" else None)
+        return dict(t, beta1=ADAM_BETAS[0], beta2=ADAM_BETAS[1], eps=ADAM_EPS, weight_decay=0.0, grad_scale=grad_scale)
+
+    def optimizer_step(self, grad_scale: Optional[float] = None, skip=()) -> None:
+        """PerPointAdam.step over the 6 Gaussian tensors + the pose table in one launch
+        (param groups and LRs of scene/gaussian_model.py:203-243).  skip: Gaussian tensors that take no step."""
+        self._advance(skip)
+        self._launch_adam(grad_scale, skip)
+
+    def _launch_adam(self, grad_scale: Optional[float] = None, skip=()) -> None:
         gs = 1.0 / self.world_size if grad_scale is None else grad_scale
-        entries = []
-        for name, k in SEGMENTS:
-            if name in skip:
-                continue
-            entries.append(dict(param=self.view(self.params, name), grad=self.view(self.grads, name),
-                                exp_avg=self.view(self.exp_avg, name), exp_avg_sq=self.view(self.exp_avg_sq, name),
-                                per_point_lr=self.per_point_lr if name == "xyz" else None, row_len=k,
-                                step_size=lrs[name] * self._corr(self.step_count(name)), beta1=b1, beta2=b2, eps=eps,
-                                weight_decay=0.0, grad_scale=gs))
-        if c.optim_pose:
-            entries.append(dict(param=self.poses, grad=self.pose_grad, exp_avg=self.pose_m, exp_avg_sq=self.pose_v,
-                                per_point_lr=None, row_len=7, step_size=self.cam_sched(self.iteration) * corr,
-                                beta1=b1, beta2=b2, eps=eps, weight_decay=0.0, grad_scale=gs))
-        launch_adam(entries, self.flags, skip_ptr=self._skip_ptr(), step_sizes_dev=self._step_dev if _dev_steps else None)
+        launch_adam([self._adam_entry(name, gs) for name in self._stepped(skip)], self.flags, skip_ptr=self._skip_ptr(),
+                    step_sizes_dev=self._step_dev)
 
     def _skip_ptr(self):
         """Device word that makes the optimizer kernels skip the update: the forward's overflow status
@@ -425,35 +453,25 @@ class JointTrainer:
             return self._ovf.data_ptr()
         return self.frame.word(ST_OVERFLOW).data_ptr()
 
-    def _lrs(self):
-        c = self.cfg
-        return dict(xyz=self.xyz_sched(self.iteration), f_dc=c.feature_lr * 10, f_rest=c.feature_lr / 20.0 * 10,
-                    opacity=c.opacity_lr, scaling=c.scaling_lr * 10, rotation=c.rotation_lr * 10)
-
-    def fused_exchange_step(self, _advance: bool = True, _dev_steps: bool = False) -> None:
+    def fused_exchange_step(self) -> None:
         """Multi-GPU: gate flags + pose gradients summed over the ranks (one tiny kernel over peer memory, or a tiny
         NCCL all-reduce; either doubles as the pre-barrier), then ONE kernel per rank doing reduce-scatter ->
         per-point Adam -> all-gather over NVLink peer memory (csrc/gs_comm.cu), then a barrier before anyone reads
-        the new parameters.  _dev_steps: the kernels read their Adam step sizes from self._step_dev (graph replay)."""
+        the new parameters."""
+        self._advance()
+        self._launch_fused()
+
+    def _launch_fused(self) -> None:
         import torch.distributed as dist
         from ._lib import GsbAdamTensor, GsbShardPiece
         L = _lib.lib()
         st = _lib.stream_ptr()
-        c = self.cfg
-        if _advance:
-            self.opt_step += 1
-        t = self.opt_step
-        step_dev = self._step_dev if _dev_steps else None
-        b1, b2, eps = 0.9, 0.999, 1e-15
-        corr = (1 - b2 ** t) ** 0.5 / (1 - b1 ** t)
-        lrs = self._lrs()
         # 1. whole-tensor gates on the local gradients, OR-ed across ranks
         arr = (GsbAdamTensor * len(SEGMENTS))()
         for a, (name, k) in zip(arr, SEGMENTS):
             g = self.view(self.grads, name)
             a.param = a.exp_avg = a.exp_avg_sq = a.grad = g.data_ptr()
             a.numel, a.row_len, a.grad_scale = g.numel(), k, 1.0
-            a.step_size, a.beta1, a.beta2, a.eps, a.weight_decay = 0.0, b1, b2, eps, 0.0
         check(L.gsb_adam_gate(len(SEGMENTS), arr, self.flags.data_ptr(), st), "gsb_adam_gate")
         if self.exchange == "fused_p2p":
             # gate flags, the binning-overflow word and the pose-gradient table are summed over the ranks by ONE tiny
@@ -470,33 +488,30 @@ class JointTrainer:
             self._xch[7:8].copy_(self.frame.word(ST_OVERFLOW))  # slot 7: binning overflow (summed over ranks)
             dist.all_reduce(self._xch, op=dist.ReduceOp.SUM, group=self.pg)
             self.flags.copy_(self._xch[:8])
-        # 2. the fused kernel over this rank's shard
+        # 2. the fused kernel over this rank's shard; a piece of segment i reads step size i of _step_dev (nothing is
+        # skipped: the number of Gaussians is fixed with peer-memory buffers)
         lo, hi = self.shard
         pieces = []
         for fi, (name, k) in enumerate(SEGMENTS):
-            s0 = self.offs[name]
-            s1 = s0 + _align(self.P * k)
+            s0, s1 = self.segments[name]
             b, e = max(lo, s0), min(hi, s1)
             if e > b:
                 pc = GsbShardPiece()
                 pc.begin, pc.end, pc.seg_begin = b, e, s0
                 pc.per_point_lr = self.per_point_lr.data_ptr() if (name == "xyz" and self.per_point_lr is not None) else None
                 pc.row_len, pc.flag_index = k, fi
-                pc.step_size, pc.beta1, pc.beta2, pc.eps = lrs[name] * corr, b1, b2, eps
+                pc.beta1, pc.beta2, pc.eps = ADAM_BETAS[0], ADAM_BETAS[1], ADAM_EPS
                 pieces.append(pc)
         parr = (GsbShardPiece * max(1, len(pieces)))(*pieces)
         check(L.gsb_fused_rs_adam_ag(self.world_size, self.rank, self._peer_grads.ptr_array(),
                                      self._peer_params.ptr_array(), self.exp_avg.data_ptr(),
                                      self.exp_avg_sq.data_ptr(), lo, len(pieces), parr, self.flags.data_ptr(),
-                                     self._ovf.data_ptr(), 1.0 / self.world_size,
-                                     None if step_dev is None else step_dev.data_ptr(), st), "gsb_fused_rs_adam_ag")
+                                     self._ovf.data_ptr(), 1.0 / self.world_size, self._step_dev.data_ptr(), st),
+              "gsb_fused_rs_adam_ag")
         # 3. pose table: replicated Adam on the all-reduced pose gradients
-        if c.optim_pose:
-            launch_adam([dict(param=self.poses, grad=self.pose_grad, exp_avg=self.pose_m, exp_avg_sq=self.pose_v,
-                              per_point_lr=None, row_len=7, step_size=self.cam_sched(self.iteration) * corr,
-                              beta1=b1, beta2=b2, eps=eps, weight_decay=0.0, grad_scale=1.0 / self.world_size)],
-                        self._pose_flags, skip_ptr=self._ovf.data_ptr(),
-                        step_sizes_dev=None if step_dev is None else step_dev[len(SEGMENTS):])
+        if self.cfg.optim_pose:
+            launch_adam([self._adam_entry("pose", 1.0 / self.world_size)], self._pose_flags, skip_ptr=self._ovf.data_ptr(),
+                        step_sizes_dev=self._step_dev[len(SEGMENTS):])
         # 4. nobody may start the next forward before every rank's parameter stores have landed
         if self.exchange == "fused_p2p":
             check(L.gsb_peer_barrier(self.world_size, self.rank, self._peer_sig.ptr_array(), 0, 1, st),
@@ -504,42 +519,9 @@ class JointTrainer:
         else:
             dist.all_reduce(self._sync, group=self.pg)
 
-    def _graph_iteration(self, view: int, gt: torch.Tensor, do_opt: bool, stats: bool = False) -> None:
-        """Replay (capturing on first use) the CUDA graph of one iteration on `view`."""
-        if do_opt:
-            self.opt_step += 1
-            self._upload_step_sizes()                    # stream-ordered before the replay
-        for _attempt in range(2):
-            key = (view, gt.data_ptr(), do_opt, self.active_sh_degree, self.cap, self.exact_cull, stats)
-            g = self._graphs.get(key)
-            if g is None:
-                if len(self._graphs) > 64:
-                    self._graphs.clear()
-                torch.cuda.synchronize()
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
-                    self._launch_forward(view)
-                    self.loss_and_backward(view, gt, stats)
-                    if self._after_backward is not None:
-                        self._after_backward()
-                    if do_opt and self._fused:
-                        self.fused_exchange_step(_advance=False, _dev_steps=True)
-                    elif do_opt:
-                        self.optimizer_step(_advance=False, _dev_steps=True)
-                self._graphs[key] = g
-            self._fwd_count += 1
-            self._polling = True
-            g.replay()
-            if self._settle():
-                return
-            if self.world_size > 1:
-                raise _lib.GsbError(f"rank {self.rank}: {self.last_R} instances exceeded the binning capacity; the "
-                                    "optimizer update of this step was skipped on every rank (parameters are "
-                                    "consistent).  Raise JointTrainer.headroom.")
-            # capacity exceeded: the device skipped the update, the buffer has been enlarged -> new graph, once more
-        raise _lib.GsbError("graph replay: binning capacity exceeded twice in a row")
-
-    def _run_iteration(self, view: int, gt: torch.Tensor, do_opt: bool, stats: bool = False) -> None:
+    def _enqueue_iteration(self, view: int, gt: torch.Tensor, do_opt: bool, stats: bool = False) -> None:
+        """One iteration on `view` with no wait, launched eagerly or captured into a graph: forward, loss + backward,
+        the test hook, and (do_opt) the exchange and update with the step sizes _advance uploaded."""
         self._launch_forward(view)
         self.loss_and_backward(view, gt, stats)
         if self._after_backward is not None:
@@ -547,10 +529,26 @@ class JointTrainer:
         if not do_opt:
             return
         if self._fused:
-            self.fused_exchange_step()
+            self._launch_fused()
         else:
             self.reduce_grads()
-            self.optimizer_step()
+            self._launch_adam()
+
+    def _replay(self, view: int, gt: torch.Tensor, do_opt: bool, stats: bool = False) -> None:
+        """Replay (capturing on first use) the CUDA graph of _enqueue_iteration on `view`."""
+        key = (view, gt.data_ptr(), do_opt, self.active_sh_degree, self.cap, self.exact_cull, stats)
+        g = self._graphs.get(key)
+        if g is None:
+            if len(self._graphs) > 64:
+                self._graphs.clear()
+            torch.cuda.synchronize()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self._enqueue_iteration(view, gt, do_opt, stats)
+            self._graphs[key] = g
+        self._fwd_count += 1
+        self._polling = True
+        g.replay()
 
     def close(self) -> None:
         """Release the peer-visible buffers of the fused exchange (collective over the process group)."""
@@ -592,7 +590,7 @@ class JointTrainer:
         if densify_now or reset_now:
             # train.py:201-211: densify / reset between the backward and the optimizer step, eagerly (the optimizer's
             # tensor set differs); the replaced tensors take no step in this iteration
-            self._run_iteration_settled(view, gt, False, stats)
+            self._settled(lambda: self._enqueue_iteration(view, gt, False, stats))
             skip = set()
             if densify_now:
                 size = c.size_threshold if it > c.opacity_reset_interval else None
@@ -606,30 +604,16 @@ class JointTrainer:
                 skip.add("opacity")
             if do_opt:
                 self.optimizer_step(skip=[name for name, _ in SEGMENTS if name in skip])
-        elif self.use_graph and self.cap > 0:
-            self._graph_iteration(view, gt, do_opt, stats)
         else:
-            self._run_iteration_settled(view, gt, do_opt, stats)
+            if do_opt:
+                self._advance()        # once per iteration: a repeat after an overflow takes the same step
+            enqueue = self._replay if self.use_graph and self.cap > 0 else self._enqueue_iteration
+            self._settled(lambda: enqueue(view, gt, do_opt, stats))
         # crossing a multiple of the interval (with G ranks `iteration` advances by G per step)
         if self.filt is not None and self.iteration // c.mip_filter3d_interval > before // c.mip_filter3d_interval and \
                 self.iteration < c.iterations - 100:
             self.compute_filter_3D()
             self.mip_recomputed_at.append(self.iteration)
-
-    def _run_iteration_settled(self, view: int, gt: torch.Tensor, do_opt: bool, stats: bool = False) -> None:
-        self._run_iteration(view, gt, do_opt, stats)
-        if not self._settle():
-            # The binning capacity was exceeded: the device skipped the update by itself (gated on the overflow word,
-            # summed over ranks in multi-GPU mode), so parameters and moments are untouched.  Single GPU: repeat the
-            # iteration with the larger buffer.  Multi GPU: the other ranks cannot know yet -- stop loudly.
-            if self.world_size > 1:
-                raise _lib.GsbError(f"rank {self.rank}: {self.last_R} instances exceeded the binning capacity; the "
-                                    "optimizer update of this step was skipped on every rank (parameters are "
-                                    "consistent).  Raise JointTrainer.headroom.")
-            if do_opt:
-                self.opt_step -= 1
-            self._run_iteration(view, gt, do_opt, stats)
-            assert self._settle()
 
     # ---- densify / prune / opacity reset on the flat buffers (SURVEY.md section 8 row f4) -----------------------
     # Semantics of scene/gaussian_model.py: prune_points (:359-374) keeps the surviving rows of every
@@ -644,11 +628,9 @@ class JointTrainer:
                                 "(exchange='fused_p2p'); use exchange='allreduce'")
         new = {name: rows(name, self.view(self.params, name), self.view(self.exp_avg, name),
                           self.view(self.exp_avg_sq, name)) for name, _ in SEGMENTS}
-        offs, total = {}, 0
-        for name, k in SEGMENTS:
-            offs[name] = total
-            total += _align(new_P * k)
-        self.P, self.offs, self.total = new_P, offs, total
+        self.P = new_P
+        self.segments, total = _layout(new_P)
+        self.total = total
         self.params = torch.zeros(total, dtype=torch.float32, device=self.dev)
         self.grads = torch.zeros(total, dtype=torch.float32, device=self.dev)
         self.exp_avg = torch.zeros(total, dtype=torch.float32, device=self.dev)
@@ -669,10 +651,13 @@ class JointTrainer:
         self._fwd_count = 0
 
     def _set_per_point_lr(self, values: Optional[torch.Tensor]) -> None:
+        """The xyz tensor's per-point learning-rate multiplier [P] (None: off), padded with ones over the xyz
+        segment's padded tail."""
         if values is None:
             self.per_point_lr = None
             return
-        ppl = torch.ones(_align(self.P * 3) // 3 + 1, dtype=torch.float32, device=self.dev)
+        begin, end = self.segments["xyz"]
+        ppl = torch.ones((end - begin) // 3 + 1, dtype=torch.float32, device=self.dev)
         ppl[:self.P] = values.to(self.dev).float().reshape(self.P)
         self.per_point_lr = ppl
 
@@ -740,12 +725,7 @@ class JointTrainer:
         """The `lr` of every param group as the reference's optimizer holds it after update_learning_rate(iteration)
         (before the first iteration: training_setup_pp's initial values)."""
         c = self.cfg
-        lrs = self._lrs()
-        if self.iteration == 0:
-            lrs["xyz"], pose = c.position_lr_init * c.spatial_lr_scale, c.rotation_lr * 0.1
-        else:
-            pose = self.cam_sched(self.iteration)
-        return [float(lrs[name]) for name, _ in SEGMENTS] + [float(pose)]
+        return [float(lr) for lr in group_lrs(c, c.spatial_lr_scale, self.iteration or None).values()]
 
     def capture(self):
         """The reference's 13-tuple (GaussianModel.capture) built from the flat buffers: copies, as nn.Parameters on
@@ -761,7 +741,7 @@ class JointTrainer:
             ppl = None
             if name == "xyz" and self.per_point_lr is not None:
                 ppl = self.per_point_lr[:self.P].reshape(self.P, 1).clone()
-            groups.append(dict(lr=lr, betas=(0.9, 0.999), eps=1e-15, weight_decay=0.0, per_point_lr=ppl, name=name,
+            groups.append(dict(lr=lr, betas=ADAM_BETAS, eps=ADAM_EPS, weight_decay=0.0, per_point_lr=ppl, name=name,
                                params=[i]))
             if name == "pose":
                 if self.cfg.optim_pose and self.opt_step > 0:
