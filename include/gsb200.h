@@ -222,6 +222,46 @@ GSB_API int gsb_track_step(float* pose7, const float* dpose7_raw, const double* 
                            float* exp_avg_sq7, float* best8, float* loss_out, int32_t step, float lr_q, float lr_T,
                            float beta1, float beta2, float eps, float weight_decay, gsb_stream_t stream);
 
+/* ---- batched tracking: render.py:99-170 for V test views at once (the loop over test cameras at :99, each view's
+ * 500-iteration pose optimisation at :113-161).  The views share one cloud (frozen), one GsbCamera (intrinsics,
+ * background) and one GsbFilter; each has its own pose, row v of a [V, 7] table.  Every kernel of the single-view
+ * path runs once for the whole batch with a view index: record id v*P + i, global tile v*T + t (T = tiles of one
+ * frame), one fixed-point unit M per view.  Each view's result is bit-identical to the single-view call on it, and
+ * V = 1 is the single-view path (the single-view entry points are that case of the same kernels).
+ * Status words are one set per batch: [0] is the total R of all views, [1] (overflow) is set if any tile list was
+ * truncated (memory-safe, as in gsb_render).
+ *
+ * Sizes: geom grows by ~145 bytes per (view, Gaussian), the image buffer and out_color by V frames, binning by
+ * 8 bytes per tile and view; at V = 1 each is at least the single-view size. */
+GSB_API size_t gsb_geom_bytes_batch(int32_t P, int32_t V, int32_t width, int32_t height);
+GSB_API size_t gsb_binning_bytes_batch(int64_t R, int32_t width, int32_t height, int32_t V);
+GSB_API size_t gsb_image_bytes_batch(int32_t width, int32_t height, int32_t V);
+/* Device address of the status words inside a batch's geom buffer (gsb_status_device for V views). */
+GSB_API uint32_t* gsb_status_device_batch(void* geom, int32_t P, int32_t V);
+/* gsb_preprocess_ex for V poses: g must hold raw parameters; g->pose is ignored and poses7 [V, 7] used instead.
+ * radii [V, P] (int32). */
+GSB_API int gsb_preprocess_batch(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, int32_t V,
+                                 const float* poses7, void* geom, size_t geom_bytes, int32_t* radii,
+                                 uint32_t* status_host, gsb_stream_t stream);
+/* gsb_render for the batch; R is the instance capacity of the binning buffer for all views.  out_color [V, 3, H, W]. */
+GSB_API int gsb_render_batch(const GsbCamera* cam, int32_t P, int32_t V, void* geom, void* binning,
+                             size_t binning_bytes, int64_t R, void* image, float* out_color, uint32_t* status_host,
+                             gsb_stream_t stream);
+/* Pose-only backward of the batch (gsb_backward_ex with only dL_dpose set, per view): dL_dout [V, 3, H, W] ->
+ * dpose7 [V, 7].  No per-Gaussian gradient is written. */
+GSB_API int gsb_backward_pose_batch(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, int32_t V,
+                                    const float* poses7, void* geom, void* binning, int64_t R, void* image,
+                                    const float* dL_dout, float* dpose7, gsb_stream_t stream);
+/* gsb_l1_mask_fwd_bwd on V images [V, C, H, W] at once; sums [V, 2] (double, caller zeroes). */
+GSB_API int gsb_l1_mask_fwd_bwd_batch(int32_t V, int32_t C, int32_t H, int32_t W, const float* img, const float* gt,
+                                      float threshold, double* sums, float* dL_dimg, gsb_stream_t stream);
+/* gsb_track_step for V views: pose7, dpose7_raw, exp_avg7, exp_avg_sq7 [V, 7], sums2 [V, 2], best8 [V, 8]; view v's
+ * loss goes to loss_out[v * loss_stride] when loss_out is not NULL. */
+GSB_API int gsb_track_step_batch(int32_t V, float* pose7, const float* dpose7_raw, const double* sums2, float* exp_avg7,
+                                 float* exp_avg_sq7, float* best8, float* loss_out, int64_t loss_stride, int32_t step,
+                                 float lr_q, float lr_T, float beta1, float beta2, float eps, float weight_decay,
+                                 gsb_stream_t stream);
+
 /* Per-point Adam (scene/per_point_adam.py:34-98), n tensors in one launch. */
 typedef struct GsbAdamTensor {
   float* param;

@@ -76,7 +76,10 @@ EXPORTS = ("gsb_geom_bytes", "gsb_binning_bytes", "gsb_image_bytes", "gsb_prepro
            "gsb_abi_version", "gsb_profile_enable", "gsb_profile_collect", "gsb_launch_count", "gsb_set_option", "gsb_adam_gate",
            "gsb_ipc_alloc", "gsb_ipc_open", "gsb_ipc_close", "gsb_ipc_free", "gsb_fused_rs_adam_ag",
            "gsb_knn_scratch_bytes", "gsb_knn_mean_dist2", "gsb_status_device", "gsb_adam_step_gated", "gsb_blend_stats", "gsb_l1_mask_fwd_bwd", "gsb_track_step", "gsb_peer_signal_bytes", "gsb_peer_barrier", "gsb_peer_exchange", "gsb_adam_step_ex",
-           "gsb_preprocess_ex", "gsb_backward_ex", "gsb_mip_filter3d", "gsb_backward_stats")
+           "gsb_preprocess_ex", "gsb_backward_ex", "gsb_mip_filter3d", "gsb_backward_stats",
+           "gsb_geom_bytes_batch", "gsb_binning_bytes_batch", "gsb_image_bytes_batch", "gsb_status_device_batch",
+           "gsb_preprocess_batch", "gsb_render_batch", "gsb_backward_pose_batch", "gsb_l1_mask_fwd_bwd_batch",
+           "gsb_track_step_batch")
 KERNEL_IDS = ("preprocess", "sort_depth", "scan", "duplicate", "sort_tile", "gather", "blend_fwd", "blend_bwd",
               "preprocess_bwd", "loss_fwd", "loss_bwd", "adam")
 
@@ -137,6 +140,24 @@ def lib() -> ctypes.CDLL:
     L.gsb_adam_step_ex.restype = ctypes.c_int
     L.gsb_status_device.argtypes = [vp, i32]
     L.gsb_status_device.restype = vp
+    L.gsb_geom_bytes_batch.restype = sz
+    L.gsb_geom_bytes_batch.argtypes = [i32, i32, i32, i32]
+    L.gsb_binning_bytes_batch.restype = sz
+    L.gsb_binning_bytes_batch.argtypes = [i64, i32, i32, i32]
+    L.gsb_image_bytes_batch.restype = sz
+    L.gsb_image_bytes_batch.argtypes = [i32, i32, i32]
+    L.gsb_status_device_batch.argtypes = [vp, i32, i32]
+    L.gsb_status_device_batch.restype = vp
+    L.gsb_preprocess_batch.argtypes = [ctypes.POINTER(GsbCamera), ctypes.POINTER(GsbGaussians),
+                                       ctypes.POINTER(GsbFilter), i32, vp, vp, sz, vp, vp, vp]
+    L.gsb_render_batch.argtypes = [ctypes.POINTER(GsbCamera), i32, i32, vp, vp, sz, i64, vp, vp, vp, vp]
+    L.gsb_backward_pose_batch.argtypes = [ctypes.POINTER(GsbCamera), ctypes.POINTER(GsbGaussians),
+                                          ctypes.POINTER(GsbFilter), i32, vp, vp, vp, i64, vp, vp, vp, vp]
+    L.gsb_l1_mask_fwd_bwd_batch.argtypes = [i32, i32, i32, i32, vp, vp, ctypes.c_float, vp, vp, vp]
+    L.gsb_track_step_batch.argtypes = [i32, vp, vp, vp, vp, vp, vp, vp, i64, i32] + [ctypes.c_float] * 6 + [vp]
+    for f in ("gsb_preprocess_batch", "gsb_render_batch", "gsb_backward_pose_batch", "gsb_l1_mask_fwd_bwd_batch",
+              "gsb_track_step_batch"):
+        getattr(L, f).restype = ctypes.c_int
     L.gsb_adam_step_gated.argtypes = [i32, ctypes.POINTER(GsbAdamTensor), vp, vp, vp]
     L.gsb_adam_step_gated.restype = ctypes.c_int
     L.gsb_backward.argtypes = [ctypes.POINTER(GsbCamera), ctypes.POINTER(GsbGaussians), vp, vp, i64, vp, vp,

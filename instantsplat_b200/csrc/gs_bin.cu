@@ -7,7 +7,7 @@
 // tile-locally instead:
 //
 //   k_preprocess   (gs_raster.cu) counts instances per tile with RED.ADD while it projects     -> tcount[T]
-//   k_tile_scan    one CTA: exclusive scan of the T (<= 65535) tile counts                      -> tstart[T], R
+//   k_tile_scan    one CTA: exclusive scan of the T (<= 65535 per view, V * T in a batch) tile counts -> tstart, R
 //   k_scatter      one thread per Gaussian (any order): (depth bits << 32 | id) appended to its tiles' segments
 //                  through per-tile atomic cursors
 //   k_tile_sort    one CTA per tile: the segment is sorted by the unique 64-bit key in SHARED MEMORY
@@ -108,30 +108,32 @@ __global__ void __launch_bounds__(kScanT) k_tile_scan(GeomView gv, int ntiles) {
 }
 
 // ------------------------------------------------------------------------------------------
-// k_scatter: one thread per Gaussian
+// k_scatter: one thread per Gaussian; grid y = view (record id v * P + i, the view's tiles at v * ntiles)
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kThreads)
-k_scatter(int P, GeomView gv, BinView bv, int W, int H, int gx, int exact_cull, uint32_t cap) {
+k_scatter(int P, GeomView gv, BinView bv, int W, int H, int gx, int ntiles, int exact_cull, uint32_t cap) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const uint32_t n = i < P ? gv.tiles[i] : 0u;
+  const size_t tb = (size_t)blockIdx.y * ntiles;
+  const uint32_t r = (uint32_t)((size_t)blockIdx.y * P + i);
+  const uint32_t n = i < P ? gv.tiles[r] : 0u;
   SplatRect p;
   p.x = p.y = p.A = p.B = p.C = 0.f; p.qthr = -1.f;
   p.rx0 = p.rx1 = p.ry0 = p.ry1 = 0;
   unsigned long long key = 0ull;
   bool coop = false;
-  TileSink sink{gv.tcount, gv.tstart, gv.tcursor, bv.pairs, cap};
+  TileSink sink{gv.tcount + tb, gv.tstart + tb, gv.tcursor + tb, bv.pairs, cap};
   uint32_t mask = 0u;
   if (n) {
-    const float4 r3 = gv.brec[i];                            // depth, rect x, rect y, keep mask
+    const float4 r3 = gv.brec[r];                            // depth, rect x, rect y, keep mask
     const uint32_t rcx = __float_as_uint(r3.y), rcy = __float_as_uint(r3.z);
     p.rx0 = rcx & 0xFFFF; p.rx1 = rcx >> 16; p.ry0 = rcy & 0xFFFF; p.ry1 = rcy >> 16;
-    key = ((unsigned long long)__float_as_uint(r3.x) << 32) | (unsigned long long)(uint32_t)i;
+    key = ((unsigned long long)__float_as_uint(r3.x) << 32) | (unsigned long long)r;
     const int area = (p.rx1 - p.rx0) * (p.ry1 - p.ry0);
     coop = area > kCoopTiles && area <= kBigRect;            // larger rects are emitted by k_big_rects
     if (area > kBigRect) {
       // nothing to do here
     } else if (coop) {                                              // re-walk the rect from the stored record (log2 domain)
-      const float4 e0 = gv.rec[3 * (size_t)i], e1 = gv.rec[3 * (size_t)i + 1];
+      const float4 e0 = gv.rec[3 * (size_t)r], e1 = gv.rec[3 * (size_t)r + 1];
       p.x = e0.x; p.y = e0.y; p.A = -e0.z; p.B = -0.5f * e0.w; p.C = -e1.x; p.qthr = e1.z;
     } else {
       mask = __float_as_uint(r3.w);                          // exactly the tiles k_preprocess counted
@@ -151,16 +153,18 @@ k_scatter(int P, GeomView gv, BinView bv, int W, int H, int gx, int exact_cull, 
 // every CTA computes the exclusive prefix of the trip counts of the queue (redundantly, in shared memory; the queue is
 // short) and the grid's warps take work items w = gw, gw + GW, ...: item -> (entry, trip) by binary search in the
 // prefix.  EMIT = false: count per tile (RED) and per Gaussian (gv.tiles);  EMIT = true: reserve + write the keys.
-// Both passes evaluate the tile test on the STORED record, so they see bit-identical inputs.
+// Both passes evaluate the tile test on the STORED record, so they see bit-identical inputs.  In a batch of V views the
+// queue holds record ids v * P + i; each work item counts / emits into its view's tiles (v * ntiles + t).
 constexpr int kBigT = 256;
 constexpr int kBigBatch = 4096;                 // queue entries per prefix batch
 constexpr int kBigPer = kBigBatch / kBigT;      // entries per thread
 template <bool EMIT>
 __global__ void __launch_bounds__(kBigT)
-k_big_rects(int P, GeomView gv, unsigned long long* pairs, int W, int H, int gx, int exact_cull, uint32_t cap) {
+k_big_rects(int P, int V, GeomView gv, unsigned long long* pairs, int W, int H, int gx, int ntiles, int exact_cull,
+            uint32_t cap) {
   __shared__ uint32_t s_pref[kBigBatch + 1];
   __shared__ uint32_t s_warp[kBigT / 32];
-  const uint32_t n_all = min(gv.aux[0], (uint32_t)P);
+  const uint32_t n_all = min(gv.aux[0], (uint32_t)P * (uint32_t)V);
   if (n_all == 0u) return;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t gw = blockIdx.x * (kBigT / 32) + warp, GW = gridDim.x * (kBigT / 32);
@@ -211,13 +215,15 @@ k_big_rects(int P, GeomView gv, unsigned long long* pairs, int W, int H, int gx,
       const uint32_t trip = w - s_pref[lo];
       const uint32_t id = gv.q_big[b0 + lo];
       const float4 r3 = gv.brec[id], e0 = gv.rec[3 * (size_t)id], e1 = gv.rec[3 * (size_t)id + 1];
+      const size_t tb = (size_t)(id / (uint32_t)P) * ntiles;
+      const TileSink vs{sink.tcount + tb, sink.tstart + tb, sink.tcursor + tb, sink.pairs, cap};
       const uint32_t rcx = __float_as_uint(r3.y), rcy = __float_as_uint(r3.z);
       SplatRect b;
       b.rx0 = rcx & 0xFFFF; b.rx1 = rcx >> 16; b.ry0 = rcy & 0xFFFF; b.ry1 = rcy >> 16;
       b.x = e0.x; b.y = e0.y; b.A = -e0.z; b.B = -0.5f * e0.w; b.C = -e1.x; b.qthr = e1.z;
       const unsigned long long key = ((unsigned long long)__float_as_uint(r3.x) << 32) | (unsigned long long)id;
       const int wd = b.rx1 - b.rx0, n = wd * (b.ry1 - b.ry0);
-      const uint32_t kept = visit_trip(b, (int)(trip * kTripTiles), n, wd, W, H, gx, cull, sink, key);
+      const uint32_t kept = visit_trip(b, (int)(trip * kTripTiles), n, wd, W, H, gx, cull, vs, key);
       if (!EMIT && lane == 0 && kept) atomicAdd(gv.tiles + id, kept);
     }
     __syncthreads();                                     // s_pref is rebuilt for the next batch
@@ -418,17 +424,17 @@ int gsb_launch_tile_scan(const GeomView& gv, int ntiles, cudaStream_t st) {
 }
 
 // pairs == nullptr: count mode (after k_preprocess, before the tile scan); else emit mode (beside k_scatter)
-int gsb_launch_big_rects(int P, const GeomView& gv, unsigned long long* pairs, int W, int H, int exact_cull, uint32_t cap,
-                         cudaStream_t st) {
-  const int gx = (W + kBlock - 1) / kBlock;
+int gsb_launch_big_rects(int P, int V, const GeomView& gv, unsigned long long* pairs, int W, int H, int exact_cull,
+                         uint32_t cap, cudaStream_t st) {
+  const int gx = (W + kBlock - 1) / kBlock, ntiles = gx * ((H + kBlock - 1) / kBlock);
   const int grid = 2 * gsb_sm_count();
-  if (pairs) k_big_rects<true><<<grid, kBigT, 0, st>>>(P, gv, pairs, W, H, gx, exact_cull, cap);
-  else k_big_rects<false><<<grid, kBigT, 0, st>>>(P, gv, nullptr, W, H, gx, exact_cull, cap);
+  if (pairs) k_big_rects<true><<<grid, kBigT, 0, st>>>(P, V, gv, pairs, W, H, gx, ntiles, exact_cull, cap);
+  else k_big_rects<false><<<grid, kBigT, 0, st>>>(P, V, gv, nullptr, W, H, gx, ntiles, exact_cull, cap);
   GSB_CUDA(cudaGetLastError());
   return GSB_OK;
 }
 
-int gsb_launch_binning(int P, const GeomView& gv, const BinView& bv, int W, int H, int exact_cull, uint32_t cap,
+int gsb_launch_binning(int P, int V, const GeomView& gv, const BinView& bv, int W, int H, int exact_cull, uint32_t cap,
                        cudaStream_t st) {
   static bool attr_set[64] = {};
   int dev = 0;
@@ -440,16 +446,17 @@ int gsb_launch_binning(int P, const GeomView& gv, const BinView& bv, int W, int 
   const int gx = (W + kBlock - 1) / kBlock, gy = (H + kBlock - 1) / kBlock;
   // the emission cursors are reset HERE (not by the scan) so that the render phase can be repeated on the same
   // preprocess result, e.g. with a larger buffer after an overflow
-  GSB_CUDA(cudaMemsetAsync(gv.tcursor, 0, (size_t)gx * gy * 4, st));
+  const int ntiles = gx * gy;
+  GSB_CUDA(cudaMemsetAsync(gv.tcursor, 0, (size_t)V * ntiles * 4, st));
   if (P > 0) {
     ProfScope ps(GSB_K_DUPLICATE, st, 2);
-    k_scatter<<<(P + kThreads - 1) / kThreads, kThreads, 0, st>>>(P, gv, bv, W, H, gx, exact_cull, cap);
-    const int rc = gsb_launch_big_rects(P, gv, bv.pairs, W, H, exact_cull, cap, st);                // emit mode
+    k_scatter<<<dim3((P + kThreads - 1) / kThreads, V), kThreads, 0, st>>>(P, gv, bv, W, H, gx, ntiles, exact_cull, cap);
+    const int rc = gsb_launch_big_rects(P, V, gv, bv.pairs, W, H, exact_cull, cap, st);             // emit mode
     if (rc) return rc;
   }
   {
     ProfScope ps(GSB_K_SORT_TILE, st, 2);
-    k_tile_sort<<<gx * gy, kSmallNT, kSmallSmem, st>>>(gv, bv, cap);
+    k_tile_sort<<<V * ntiles, kSmallNT, kSmallSmem, st>>>(gv, bv, cap);
     // persistent CTAs draining the long-list queues, one per SM
     k_tile_sort_long<<<gsb_sm_count(), kLargeNT, kLargeSmem, st>>>(gv, bv, cap);
   }

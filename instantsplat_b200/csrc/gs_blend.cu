@@ -65,13 +65,34 @@ __device__ __forceinline__ bool slab_may_contribute(const float4& e0, const floa
   return rect_may_contribute(e0.x, e0.y, -e0.z, -0.5f * e0.w, -e1.x, e1.z, rx0, ry0, rx1, ry1);
 }
 
+// Batches of V views: the grid is (tiles of one frame, V), so CTA (t, v) blends local tile t of view v.  Returns the
+// global tile index v * ntiles + t (the view's binning lists) and moves the per-pixel buffers to the view's frame; once
+// per CTA, so the per-pair work is the single-view one.
+__device__ __forceinline__ int view_tile(int W, int H, float* __restrict__& color, float* __restrict__& final_T,
+                                         uint32_t* __restrict__& n_contrib) {
+  const size_t hw = (size_t)W * H, v = blockIdx.y;
+  color += 3 * hw * v;
+  final_T += hw * v;
+  n_contrib += hw * v;
+  return (int)(v * gridDim.x) + (int)blockIdx.x;
+}
+__device__ __forceinline__ int view_tile_bwd(int W, int H, const float* __restrict__& dL, const float* __restrict__& final_T,
+                                             const uint32_t* __restrict__& n_contrib, const uint32_t* __restrict__& dscale) {
+  const size_t hw = (size_t)W * H, v = blockIdx.y;
+  dL += 3 * hw * v;
+  final_T += hw * v;
+  n_contrib += hw * v;
+  dscale += v;
+  return (int)(v * gridDim.x) + (int)blockIdx.x;
+}
+
 __global__ void __launch_bounds__(kThreads)
 k_blend_fwd(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids, const float4* __restrict__ rec,
             const float* __restrict__ bg, int W, int H, int gx,
             float* __restrict__ out_color, float* __restrict__ final_T, uint32_t* __restrict__ n_contrib) {
   __shared__ float4 sm0[kChunk1], sm1[kChunk1], sm2[kChunk1];
-  const int tile = blockIdx.x;
-  const int tx = tile % gx, ty = tile / gx;
+  const int tile = view_tile(W, H, out_color, final_T, n_contrib);
+  const int tx = blockIdx.x % gx, ty = blockIdx.x / gx;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int sx0 = tx * kBlock + (warp & 1) * 8, sy0 = ty * kBlock + (warp >> 1) * 4;
   const int px = sx0 + (lane & 7), py = sy0 + (lane >> 3);
@@ -135,8 +156,10 @@ k_blend_fwd(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids, 
 }
 
 // *dscale = max |dL[i]| (float bits of non-negative floats order like the floats, so the integer max is exact and
-// independent of the order of the atomics)
+// independent of the order of the atomics); grid y = view: dscale[v] over the view's n values
 __global__ void __launch_bounds__(kThreads) k_abs_max(size_t n, const float* __restrict__ dL, uint32_t* __restrict__ dscale) {
+  dL += n * blockIdx.y;
+  dscale += blockIdx.y;
   float m = 0.f;
   for (size_t e = (size_t)blockIdx.x * kThreads + threadIdx.x; e < n; e += (size_t)gridDim.x * kThreads)
     m = fmaxf(m, fabsf(__ldg(dL + e)));
@@ -236,9 +259,9 @@ k_blend_bwd(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids, 
             const float* __restrict__ dL_dpix, unsigned long long* __restrict__ dacc, const uint32_t* __restrict__ dscale) {
   __shared__ float4 sm0[kChunk1], sm1[kChunk1], sm2[kChunk1];
   __shared__ int s_bmax;
+  const int tile = view_tile_bwd(W, H, dL_dpix, final_T, n_contrib, dscale);
   const float inv_m = fix_inv_m(dscale);
-  const int tile = blockIdx.x;
-  const int tx = tile % gx, ty = tile / gx;
+  const int tx = blockIdx.x % gx, ty = blockIdx.x / gx;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int sx0 = tx * kBlock + (warp & 1) * 8, sy0 = ty * kBlock + (warp >> 1) * 4;
   const int px = sx0 + (lane & 7), py = sy0 + (lane >> 3);
@@ -434,8 +457,8 @@ k_blend_fwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids,
   __shared__ __align__(8) uint64_t bars[3];
   Stager<BULK, kThreads2> sg{stg, sid, bars, ids, rec, 0, 0};
   sg.init();
-  const int tile = blockIdx.x;
-  const int tx = tile % gx, ty = tile / gx;
+  const int tile = view_tile(W, H, out_color, final_T, n_contrib);
+  const int tx = blockIdx.x % gx, ty = blockIdx.x / gx;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int sx0 = tx * kBlock + (warp & 1) * 8, sy0 = ty * kBlock + (warp >> 1) * 8;
   const int px = sx0 + (lane & 7), pyA = sy0 + (lane >> 3), pyB = pyA + 4;
@@ -548,6 +571,7 @@ k_blend_bwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids,
              const float* __restrict__ dL_dpix, unsigned long long* __restrict__ dacc,
              const uint32_t* __restrict__ dscale, unsigned long long* __restrict__ stats = nullptr) {
   unsigned int st_iter = 0, st_red = 0, st_valid = 0;
+  const int tile = view_tile_bwd(W, H, dL_dpix, final_T, n_contrib, dscale);
   const float inv_m = fix_inv_m(dscale);
   __shared__ __align__(128) SlabStage stg[2];
   __shared__ __align__(16) uint32_t sid[BULK ? 3 : 1][kIdRow];
@@ -555,8 +579,7 @@ k_blend_bwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids,
   __shared__ int s_bmax;
   Stager<BULK, kThreads2> sg{stg, sid, bars, ids, rec, 0, 0};
   sg.init();
-  const int tile = blockIdx.x;
-  const int tx = tile % gx, ty = tile / gx;
+  const int tx = blockIdx.x % gx, ty = blockIdx.x / gx;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int sx0 = tx * kBlock + (warp & 1) * 8, sy0 = ty * kBlock + (warp >> 1) * 8;
   const int px = sx0 + (lane & 7), pyA = sy0 + (lane >> 3), pyB = pyA + 4;
@@ -696,45 +719,47 @@ k_blend_bwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids,
 
 }  // namespace
 
-int gsb_launch_blend_fwd(const GeomView& gv, const BinView& bv, const ImgView& iv, const float* bg, int W, int H, float* out_color,
-                         cudaStream_t st) {
-  const int gx = (W + kBlock - 1) / kBlock, gy = (H + kBlock - 1) / kBlock;
+int gsb_launch_blend_fwd(const GeomView& gv, const BinView& bv, const ImgView& iv, const float* bg, int W, int H, int V,
+                         float* out_color, cudaStream_t st) {
+  const int gx = (W + kBlock - 1) / kBlock;
+  const dim3 grid(gx * ((H + kBlock - 1) / kBlock), V);
   ProfScope ps(GSB_K_BLEND_FWD, st);
   const int ver = gsb_option_blend_version(), bulk = gsb_option_stage_bulk();
   if (ver == 2 && bulk)
-    k_blend_fwd2<true><<<gx * gy, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, out_color,
-                                                      iv.final_T, iv.n_contrib);
+    k_blend_fwd2<true><<<grid, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, out_color,
+                                                   iv.final_T, iv.n_contrib);
   else if (ver == 2)
-    k_blend_fwd2<false><<<gx * gy, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, out_color,
-                                                       iv.final_T, iv.n_contrib);
+    k_blend_fwd2<false><<<grid, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, out_color,
+                                                    iv.final_T, iv.n_contrib);
   else
-    k_blend_fwd<<<gx * gy, kThreads, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, out_color, iv.final_T,
-                                              iv.n_contrib);
+    k_blend_fwd<<<grid, kThreads, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, out_color, iv.final_T,
+                                           iv.n_contrib);
   GSB_CUDA(cudaGetLastError());
   return GSB_OK;
 }
 
-int gsb_launch_blend_bwd(const GeomView& gv, const BinView& bv, const ImgView& iv, const float* bg, int W, int H, const float* dL_dout,
-                         bool pose_only, cudaStream_t st) {
-  const int gx = (W + kBlock - 1) / kBlock, gy = (H + kBlock - 1) / kBlock;
+int gsb_launch_blend_bwd(const GeomView& gv, const BinView& bv, const ImgView& iv, const float* bg, int W, int H, int V,
+                         const float* dL_dout, bool pose_only, cudaStream_t st) {
+  const int gx = (W + kBlock - 1) / kBlock;
+  const dim3 grid(gx * ((H + kBlock - 1) / kBlock), V);
   ProfScope ps(GSB_K_BLEND_BWD, st, 2);
   const size_t n = (size_t)3 * W * H;
   const size_t nb = (n + kThreads - 1) / kThreads, max_blocks = 4 * (size_t)gsb_sm_count();
-  k_abs_max<<<(int)(nb < max_blocks ? nb : max_blocks), kThreads, 0, st>>>(n, dL_dout, gv.dscale);
+  k_abs_max<<<dim3((int)(nb < max_blocks ? nb : max_blocks), V), kThreads, 0, st>>>(n, dL_dout, gv.dscale);
   const int ver = gsb_option_blend_version(), bulk = gsb_option_stage_bulk();
   unsigned long long* dacc = gv.dacc;
   if (pose_only)
-    k_blend_bwd2<true, false, true><<<gx * gy, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, iv.final_T,
-                                                                   iv.n_contrib, dL_dout, dacc, gv.dscale);
+    k_blend_bwd2<true, false, true><<<grid, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, iv.final_T,
+                                                                iv.n_contrib, dL_dout, dacc, gv.dscale);
   else if (ver == 2 && bulk)
-    k_blend_bwd2<true><<<gx * gy, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, iv.final_T,
-                                                      iv.n_contrib, dL_dout, dacc, gv.dscale);
+    k_blend_bwd2<true><<<grid, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, iv.final_T,
+                                                   iv.n_contrib, dL_dout, dacc, gv.dscale);
   else if (ver == 2)
-    k_blend_bwd2<false><<<gx * gy, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, iv.final_T,
-                                                       iv.n_contrib, dL_dout, dacc, gv.dscale);
+    k_blend_bwd2<false><<<grid, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, iv.final_T,
+                                                    iv.n_contrib, dL_dout, dacc, gv.dscale);
   else
-    k_blend_bwd<<<gx * gy, kThreads, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, iv.final_T, iv.n_contrib,
-                                              dL_dout, dacc, gv.dscale);
+    k_blend_bwd<<<grid, kThreads, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, iv.final_T, iv.n_contrib,
+                                           dL_dout, dacc, gv.dscale);
   GSB_CUDA(cudaGetLastError());
   return GSB_OK;
 }

@@ -112,44 +112,52 @@ struct GeomView {
   uint32_t* tiles;     // tile instances per Gaussian (after culling)
   uint8_t* clamped;
   unsigned long long* dacc;   // [kDaccSlots * P] backward accumulators, fixed point (see fix_scale)
-  uint32_t* dscale;    // [1] max |dL/dpixel| of the current backward (float bits), the unit of the fixed point
+  uint32_t* dscale;    // [V] max |dL/dpixel| of each view's current backward (float bits), the unit of the fixed point
   float* pose_part;    // [nblocks*16]
   float* pose_acc;     // [16]
   uint32_t* status;    // [kStWords]
   uint32_t* aux;       // [64] per-forward counters, zeroed together with tcount (they are adjacent): [0] = length of q_big
-  uint32_t* tcount;    // [kMaxTiles] instances per tile (counted by k_preprocess / k_big_rects)
-  uint32_t* tstart;    // [kMaxTiles] exclusive scan of tcount
-  uint32_t* tcursor;   // [kMaxTiles] emission cursors (k_scatter)
-  uint32_t* q_large;   // [kMaxTiles] tiles whose list has kSmallList < n <= kLargeList entries
-  uint32_t* q_huge;    // [kMaxTiles] tiles with longer lists
-  uint32_t* q_big;     // [P] Gaussians whose tile rect exceeds kBigRect tiles (walked by k_big_rects, flattened)
+  uint32_t* tcount;    // [tile_slots] instances per tile (counted by k_preprocess / k_big_rects)
+  uint32_t* tstart;    // [tile_slots] exclusive scan of tcount
+  uint32_t* tcursor;   // [tile_slots] emission cursors (k_scatter)
+  uint32_t* q_large;   // [tile_slots] tiles whose list has kSmallList < n <= kLargeList entries
+  uint32_t* q_huge;    // [tile_slots] tiles with longer lists
+  uint32_t* q_big;     // [V * P] records whose tile rect exceeds kBigRect tiles (walked by k_big_rects, flattened)
   size_t total;
 };
 
-static inline GeomView geom_view(void* base, int P) {
+// V > 1: a batch of V views of the same P Gaussians (gsb_preprocess_batch).  Record id r = v * P + i, so every
+// per-record array has V * P entries; global tile index = v * ntiles + t, so the per-tile arrays hold V * ntiles
+// entries (at least kMaxTiles, which makes V = 1 the single-view layout).
+static inline size_t tile_slots(int V, int ntiles) {
+  const size_t n = (size_t)(V > 0 ? V : 1) * (size_t)(ntiles > 0 ? ntiles : 0);
+  return n > (size_t)kMaxTiles ? n : (size_t)kMaxTiles;
+}
+static inline GeomView geom_view(void* base, int P, int V = 1, int ntiles = 0) {
   GeomView v;
   size_t off = 0;
   char* p = (char*)base;
   size_t Pp = (size_t)(P > 0 ? P : 1);
+  const size_t nv = (size_t)(V > 0 ? V : 1), VP = nv * Pp, TS = tile_slots(V, ntiles);
   auto take = [&](size_t bytes) { void* r = p ? p + off : nullptr; off += align_up(bytes); return r; };
-  v.cam = (CamConst*)take(sizeof(CamConst));
-  v.rec = (float4*)take(Pp * 48);
-  v.brec = (float4*)take(Pp * 16);
-  v.tiles = (uint32_t*)take(Pp * 4);
-  v.clamped = (uint8_t*)take(Pp);
-  v.dacc = (unsigned long long*)take(Pp * kDaccSlots * 8);
-  v.dscale = (uint32_t*)take(4);
+  v.cam = (CamConst*)take(nv * sizeof(CamConst));
+  v.rec = (float4*)take(VP * 48);
+  v.brec = (float4*)take(VP * 16);
+  v.tiles = (uint32_t*)take(VP * 4);
+  v.clamped = (uint8_t*)take(VP);
+  v.dacc = (unsigned long long*)take(VP * kDaccSlots * 8);
+  v.dscale = (uint32_t*)take(nv * 4);
   size_t nb = (Pp + kPT - 1) / kPT;
-  v.pose_part = (float*)take(nb * 16 * 4);
-  v.pose_acc = (float*)take(16 * 4);
+  v.pose_part = (float*)take(nv * nb * 16 * 4);
+  v.pose_acc = (float*)take(nv * 16 * 4);
   v.status = (uint32_t*)take(kStWords * 4);
   v.aux = (uint32_t*)take(64 * 4);                        // exactly 256 bytes: tcount follows immediately
-  v.tcount = (uint32_t*)take((size_t)kMaxTiles * 4);
-  v.tstart = (uint32_t*)take((size_t)kMaxTiles * 4);
-  v.tcursor = (uint32_t*)take((size_t)kMaxTiles * 4);
-  v.q_large = (uint32_t*)take((size_t)kMaxTiles * 4);
-  v.q_huge = (uint32_t*)take((size_t)kMaxTiles * 4);
-  v.q_big = (uint32_t*)take(Pp * 4);
+  v.tcount = (uint32_t*)take(TS * 4);
+  v.tstart = (uint32_t*)take(TS * 4);
+  v.tcursor = (uint32_t*)take(TS * 4);
+  v.q_large = (uint32_t*)take(TS * 4);
+  v.q_huge = (uint32_t*)take(TS * 4);
+  v.q_big = (uint32_t*)take(VP * 4);
   v.total = off;
   return v;
 }
@@ -162,7 +170,7 @@ struct BinView {
   size_t total;
 };
 
-static inline BinView bin_view(void* base, int64_t cap, int W, int H) {
+static inline BinView bin_view(void* base, int64_t cap, int W, int H, int V = 1) {
   BinView v;
   size_t off = 0;
   char* p = (char*)base;
@@ -171,7 +179,7 @@ static inline BinView bin_view(void* base, int64_t cap, int W, int H) {
   auto take = [&](size_t bytes) { void* r = p ? p + off : nullptr; off += align_up(bytes); return r; };
   v.pairs = (unsigned long long*)take(Rp * 8);
   v.ids = (uint32_t*)take((Rp + 8) * 4);       // + 8: bulk copies of id chunks are rounded to 16 bytes
-  v.ranges = (uint2*)take((size_t)ntiles * 8);
+  v.ranges = (uint2*)take((size_t)(V > 0 ? V : 1) * ntiles * 8);
   v.total = off;
   return v;
 }
@@ -181,9 +189,9 @@ struct ImgView {
   uint32_t* n_contrib;
   size_t total;
 };
-static inline ImgView img_view(void* base, int W, int H) {
+static inline ImgView img_view(void* base, int W, int H, int V = 1) {
   ImgView v;
-  size_t hw = (size_t)W * H;
+  size_t hw = (size_t)(V > 0 ? V : 1) * W * H;
   char* p = (char*)base;
   v.final_T = (float*)p;
   v.n_contrib = (uint32_t*)(p ? p + align_up(hw * 4) : nullptr);
@@ -196,14 +204,17 @@ static inline ImgView img_view(void* base, int W, int H) {
 // ---- launchers implemented in gs_bin.cu / gs_blend.cu -----------------------------------------
 // tile scan: tstart = exclusive scan(tcount), status = {R, 0, max list, 0, long-list queue lengths, serial}
 int gsb_launch_tile_scan(const gsb::GeomView& gv, int ntiles, cudaStream_t st);
-int gsb_launch_big_rects(int P, const gsb::GeomView& gv, unsigned long long* pairs, int W, int H, int exact_cull,
+// P: Gaussians per view; V views (record id v * P + i, tile v * ntiles + t)
+int gsb_launch_big_rects(int P, int V, const gsb::GeomView& gv, unsigned long long* pairs, int W, int H, int exact_cull,
                          uint32_t cap, cudaStream_t st);
 // scatter + per-tile (depth, id) sort + slab gather + ranges; cap = instance capacity of the binning buffer
-int gsb_launch_binning(int P, const gsb::GeomView& gv, const gsb::BinView& bv, int W, int H, int exact_cull,
+int gsb_launch_binning(int P, int V, const gsb::GeomView& gv, const gsb::BinView& bv, int W, int H, int exact_cull,
                        uint32_t cap, cudaStream_t st);
+// out_color [V, 3, H, W]
 int gsb_launch_blend_fwd(const gsb::GeomView& gv, const gsb::BinView& bv, const gsb::ImgView& iv, const float* bg, int W, int H,
-                         float* out_color, cudaStream_t st);
+                         int V, float* out_color, cudaStream_t st);
 // pose_only: 8-value accumulator layout (dacc[5] = dL/db, no dL/dopacity), see k_blend_bwd2
 // computes max |dL_dout| into gv.dscale (zeroed by the caller, as is gv.dacc), then the blend backward into gv.dacc
+// dL_dout [V, 3, H, W]; one M per view (gv.dscale[v])
 int gsb_launch_blend_bwd(const gsb::GeomView& gv, const gsb::BinView& bv, const gsb::ImgView& iv, const float* bg, int W, int H,
-                         const float* dL_dout, bool pose_only, cudaStream_t st);
+                         int V, const float* dL_dout, bool pose_only, cudaStream_t st);

@@ -111,6 +111,14 @@ constexpr int kRowPad = 49;      // shared-memory SH row stride (48 + 1, conflic
 extern "C" GSB_API size_t gsb_geom_bytes(int32_t P) { return geom_view(nullptr, P).total; }
 extern "C" GSB_API size_t gsb_binning_bytes(int64_t R, int32_t W, int32_t H) { return bin_view(nullptr, R, W, H).total; }
 extern "C" GSB_API size_t gsb_image_bytes(int32_t W, int32_t H) { return img_view(nullptr, W, H).total; }
+static int frame_tiles(int W, int H) { return ((W + kBlock - 1) / kBlock) * ((H + kBlock - 1) / kBlock); }
+extern "C" GSB_API size_t gsb_geom_bytes_batch(int32_t P, int32_t V, int32_t W, int32_t H) {
+  return geom_view(nullptr, P, V, frame_tiles(W, H)).total;
+}
+extern "C" GSB_API size_t gsb_binning_bytes_batch(int64_t R, int32_t W, int32_t H, int32_t V) {
+  return bin_view(nullptr, R, W, H, V).total;
+}
+extern "C" GSB_API size_t gsb_image_bytes_batch(int32_t W, int32_t H, int32_t V) { return img_view(nullptr, W, H, V).total; }
 
 // ------------------------------------------------------------------------------------------
 // kernel parameter blocks
@@ -162,11 +170,13 @@ __device__ __forceinline__ void fill_cam(CamConst& c, const CamArgs& a) {
   c.qc[0] = 1.f; c.qc[1] = c.qc[2] = c.qc[3] = 0.f;
   if (pose) pose_to_const(pose, c);
 }
+// one CTA per view: CamConst v from pose row v of the [V, 7] pose table
 __global__ void k_setup_cam(CamConst* out, CamArgs a) {
-  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  if (threadIdx.x != 0) return;
+  if (a.pose) a.pose += 7 * blockIdx.x;
   CamConst c;
   fill_cam(c, a);
-  *out = c;
+  out[blockIdx.x] = c;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -337,6 +347,8 @@ __device__ __forceinline__ void read_gauss(const float* sm, int t, bool has_sr, 
 // ------------------------------------------------------------------------------------------
 // k_preprocess
 // ------------------------------------------------------------------------------------------
+// Grid (Gaussian CTAs, V): CTA (b, v) projects Gaussians [b * kPT, ...) in view v.  Inputs are read at the Gaussian's
+// index i, outputs are written at its record id r = v * P + i, and tiles are counted in the view's slice of tcount.
 template <bool kMip>
 __global__ void __launch_bounds__(kPT)
 k_preprocess(InPtrs in, GeomView gv, int* __restrict__ radii) {
@@ -344,7 +356,7 @@ k_preprocess(InPtrs in, GeomView gv, int* __restrict__ radii) {
   CamConst* cam = reinterpret_cast<CamConst*>(smem_raw);
   float* sm = reinterpret_cast<float*>(smem_raw + ((sizeof(CamConst) + 15) / 16) * 16);
   {
-    const uint32_t* s = reinterpret_cast<const uint32_t*>(gv.cam);
+    const uint32_t* s = reinterpret_cast<const uint32_t*>(gv.cam + blockIdx.y);
     uint32_t* d = reinterpret_cast<uint32_t*>(cam);
     for (int k = threadIdx.x; k < (int)(sizeof(CamConst) / 4); k += blockDim.x) d[k] = s[k];
   }
@@ -358,6 +370,9 @@ k_preprocess(InPtrs in, GeomView gv, int* __restrict__ radii) {
   const int t = threadIdx.x;
   const bool active = t < nv;
   const int i = first + (active ? t : 0);
+  const size_t rb = (size_t)blockIdx.y * in.P;             // record ids of this view start here
+  const uint32_t r = (uint32_t)(rb + i);
+  uint32_t* const tcount = gv.tcount + (size_t)blockIdx.y * cam->gx * cam->gy;
   GaussIn g;
   read_gauss(sm, active ? t : 0, in.scales != nullptr, g);
   Proj p;
@@ -370,7 +385,7 @@ k_preprocess(InPtrs in, GeomView gv, int* __restrict__ radii) {
   SplatRect sr_;
   sr_.x = sr_.y = sr_.A = sr_.B = sr_.C = 0.f; sr_.qthr = -1.f;
   sr_.rx0 = sr_.rx1 = sr_.ry0 = sr_.ry1 = 0;
-  const TileSink sink{gv.tcount, nullptr, nullptr, nullptr, 0u};       // count mode
+  const TileSink sink{tcount, nullptr, nullptr, nullptr, 0u};          // count mode
   const bool cull = in.exact_cull != 0;
   if (p.visible) {
     if (use_sh) {
@@ -412,7 +427,7 @@ k_preprocess(InPtrs in, GeomView gv, int* __restrict__ radii) {
     else {
       // per-tile counts: plain fire-and-forget RED.ADD per kept tile (measured faster here than warp-aggregating
       // them: nothing waits for the result, unlike the emit pass in k_scatter)
-      kmask = rect_keep_mask_count(sr_, cam->W, cam->H, cam->gx, cull, gv.tcount);
+      kmask = rect_keep_mask_count(sr_, cam->W, cam->H, cam->gx, cull, tcount);
       ntiles = (uint32_t)__popc(kmask);
     }
   } else {
@@ -430,19 +445,19 @@ k_preprocess(InPtrs in, GeomView gv, int* __restrict__ radii) {
   float4* sm4 = reinterpret_cast<float4*>(sm);
   if (active) {
     sm4[3 * t + 0] = make_float4(p.x, p.y, -0.5f * kLog2e * p.A, -kLog2e * p.B);
-    sm4[3 * t + 1] = make_float4(-0.5f * kLog2e * p.C, p.opacity, 0.5f * kLog2e * qthr, __uint_as_float((uint32_t)i));
+    sm4[3 * t + 1] = make_float4(-0.5f * kLog2e * p.C, p.opacity, 0.5f * kLog2e * qthr, __uint_as_float(r));
     sm4[3 * t + 2] = make_float4(p.rgb[0], p.rgb[1], p.rgb[2], fix_extent(p.radius, p.x, p.y, cam->W, cam->H));
-    gv.brec[i] = make_float4(p.depth, __uint_as_float((uint32_t)p.rx0 | ((uint32_t)p.rx1 << 16)),
+    gv.brec[r] = make_float4(p.depth, __uint_as_float((uint32_t)p.rx0 | ((uint32_t)p.rx1 << 16)),
                              __uint_as_float((uint32_t)p.ry0 | ((uint32_t)p.ry1 << 16)), __uint_as_float(kmask));
-    gv.tiles[i] = ntiles;
-    if (big) gv.q_big[atomicAdd(gv.aux, 1u)] = (uint32_t)i;     // at most once per Gaussian: the queue holds P entries
-    gv.clamped[i] = (uint8_t)p.clamped;
-    radii[i] = p.radius;
+    gv.tiles[r] = ntiles;
+    if (big) gv.q_big[atomicAdd(gv.aux, 1u)] = r;      // at most once per record: the queue holds V * P entries
+    gv.clamped[r] = (uint8_t)p.clamped;
+    radii[r] = p.radius;
   }
   tma_store_fence();                                 // the records leave as ONE bulk store (shared -> global, 48 nv bytes)
   __syncthreads();
   if (threadIdx.x == 0) {
-    bulk_s2g(gv.rec + 3 * (size_t)first, sm4, (uint32_t)(48 * nv));
+    bulk_s2g(gv.rec + 3 * (rb + first), sm4, (uint32_t)(48 * nv));
     bulk_commit();
     bulk_wait_read();
   }
@@ -471,7 +486,7 @@ k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out
   float* sm = reinterpret_cast<float*>(smem_raw + ((sizeof(CamConst) + 15) / 16) * 16);
   __shared__ float s_pose[kPT / 32][16];
   {
-    const uint32_t* s = reinterpret_cast<const uint32_t*>(gv.cam);
+    const uint32_t* s = reinterpret_cast<const uint32_t*>(gv.cam + blockIdx.y);
     uint32_t* d = reinterpret_cast<uint32_t*>(cam);
     for (int k = threadIdx.x; k < (int)(sizeof(CamConst) / 4); k += blockDim.x) d[k] = s[k];
   }
@@ -486,6 +501,7 @@ k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out
   stage_block_inputs(in, first, nv, use_sh, D, M, sm, &s_bar);
   const int t = threadIdx.x;
   const int i = first + t;
+  const size_t r = (size_t)blockIdx.y * in.P + i;          // record id (grid y = view, as in k_preprocess)
   float pa[16];
 #pragma unroll
   for (int k = 0; k < 16; ++k) pa[k] = 0.f;
@@ -507,9 +523,9 @@ k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out
     float ds[kDaccSlots];
 #pragma unroll
     for (int k = 0; k < kDaccSlots; ++k) ds[k] = 0.f;
-    if (gv.tiles[i] > 0) {
-      const unsigned long long* acc = gv.dacc + (size_t)i * kDaccSlots;
-      const float extent = gv.rec[3 * (size_t)i + 2].w, inv_m = fix_inv_m(gv.dscale);
+    if (gv.tiles[r] > 0) {
+      const unsigned long long* acc = gv.dacc + r * kDaccSlots;
+      const float extent = gv.rec[3 * r + 2].w, inv_m = fix_inv_m(gv.dscale + blockIdx.y);
       const double unit[3] = {1.0 / (double)fix_scale(5, extent, inv_m), 1.0 / (double)fix_scale(0, extent, inv_m),
                               1.0 / (double)fix_scale(2, extent, inv_m)};      // exponents 2, 3, 4
 #pragma unroll
@@ -519,14 +535,14 @@ k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out
     bool any = false;
 #pragma unroll
     for (int k = 0; k < 9; ++k) any |= (ds[k] != 0.f);
-    if (any && gv.tiles[i] > 0) {
+    if (any && gv.tiles[r] > 0) {
       GaussIn g;
       read_gauss(sm, t, in.scales != nullptr, g);
       Proj p;
       const Mip mf = kMip ? gauss_mip(in, i) : Mip();
       project_geometry<kMip>(*cam, g, in.cov3D ? in.cov3D + (size_t)6 * i : nullptr, p, mf);
       if (p.visible) {
-        p.clamped = gv.clamped[i];
+        p.clamped = gv.clamped[r];
         // The blend backward accumulates RAW pixel moments of w = dL/dalpha * (opacity * G) per Gaussian
         //   ds = [S w dx, S w dy, S w dx^2, S w dx dy, S w dy^2, S w, dL/dr, dL/dg, dL/db];
         // the per-Gaussian constants are applied once here instead of once per (warp, Gaussian) in the blend kernel:
@@ -623,16 +639,19 @@ k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out
       float v = 0.f;
 #pragma unroll
       for (int w = 0; w < kPT / 32; ++w) v += s_pose[w][threadIdx.x];
-      gv.pose_part[(size_t)blockIdx.x * 16 + threadIdx.x] = v;
+      gv.pose_part[((size_t)blockIdx.y * gridDim.x + blockIdx.x) * 16 + threadIdx.x] = v;
     }
   }
   if (bulk_out && threadIdx.x == 0) bulk_wait_read();   // shared memory must outlive the bulk stores reading it
 }
 
-// Pose-gradient partials [nblocks][16] -> 16 column sums (one CTA per column, deterministic order) ...
+// Pose-gradient partials [V][nblocks][16] -> 16 column sums per view (grid (16, V), one CTA per column, deterministic
+// order) ...
 __global__ void __launch_bounds__(256) k_pose_reduce(const float* __restrict__ part, int nblocks, float* __restrict__ acc16) {
   __shared__ float s[256];
   const int c = blockIdx.x;
+  part += (size_t)blockIdx.y * nblocks * 16;
+  acc16 += 16 * blockIdx.y;
   float v0 = 0.f, v1 = 0.f, v2 = 0.f, v3 = 0.f;
   int b = threadIdx.x;
   for (; b + 768 < nblocks; b += 1024) {
@@ -651,8 +670,12 @@ __global__ void __launch_bounds__(256) k_pose_reduce(const float* __restrict__ p
   if (threadIdx.x == 0) acc16[c] = s[0];
 }
 // ... and the chain to dL/dP[7] (utils/pose_utils.py quad2rotation + normalisation backward).
+//     (one CTA per view)
 __global__ void k_pose_finalize(const float* __restrict__ acc16, const float* pose, float* dpose) {
-  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  if (threadIdx.x != 0) return;
+  acc16 += 16 * blockIdx.x;
+  pose += 7 * blockIdx.x;
+  dpose += 7 * blockIdx.x;
   float acc[16];
   for (int c = 0; c < 16; ++c) acc[c] = acc16[c];
   float dp[7];
@@ -729,6 +752,9 @@ static int ensure_attrs() {
 }
 
 extern "C" GSB_API uint32_t* gsb_status_device(void* geom, int32_t P) { return geom ? geom_view(geom, P).status : nullptr; }
+extern "C" GSB_API uint32_t* gsb_status_device_batch(void* geom, int32_t P, int32_t V) {
+  return geom ? geom_view(geom, P, V).status : nullptr;      // the status words precede the tile arrays
+}
 
 static CamArgs cam_args(const GsbCamera* cam, const GsbGaussians* g) {
   CamArgs a;
@@ -738,38 +764,65 @@ static CamArgs cam_args(const GsbCamera* cam, const GsbGaussians* g) {
   return a;
 }
 
-extern "C" GSB_API int gsb_preprocess_ex(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt,
-                                         void* geom, size_t geom_bytes, int32_t* radii, uint32_t* status_host,
-                                         gsb_stream_t stream_) {
-  cudaStream_t st = (cudaStream_t)stream_;
+// A batch of V views shares cam (intrinsics, background) and g (the Gaussians); with V > 1 the poses come from
+// g->pose as a [V, 7] table.  V = 1 is the single-view forward.
+static int batch_args(int V, const GsbCamera* cam, const GsbGaussians* g) {
+  GSB_REQUIRE(V >= 1 && V <= 65535, "V must be in 1..65535 (grid y)");
+  GSB_REQUIRE(cam && g && g->P >= 0, "null camera / gaussians");
+  GSB_REQUIRE((long long)V * g->P < 0x7fffffffLL, "V * P must be below 2^31");
+  GSB_REQUIRE(cam->width > 0 && cam->height > 0 && (long long)V * frame_tiles(cam->width, cam->height) < 0x7fffffffLL,
+              "V * tiles must be below 2^31");
+  GSB_REQUIRE(V == 1 || (g->pose && g->raw_params), "a batch needs raw parameters and a [V, 7] pose table");
+  return GSB_OK;
+}
+
+static int preprocess_views(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, int V, void* geom,
+                            size_t geom_bytes, int32_t* radii, uint32_t* status_host, cudaStream_t st) {
+  int rc = batch_args(V, cam, g);
+  if (rc) return rc;
   InPtrs in;
-  int rc = make_inptrs(cam, g, in);
+  rc = make_inptrs(cam, g, in);
   if (rc) return rc;
   rc = apply_filter(filt, g, in);
   if (rc) return rc;
   GSB_REQUIRE(geom && (radii || g->P == 0), "null buffer");
   const int P = g->P;
-  GeomView gv = geom_view(geom, P);
+  const int ntiles = frame_tiles(cam->width, cam->height);
+  GeomView gv = geom_view(geom, P, V, ntiles);
   if (gv.total > geom_bytes) { gsb_set_error("geom buffer too small"); return GSB_ERR_CAPACITY; }
   rc = ensure_attrs();
   if (rc) return rc;
-  const int ntiles = ((cam->width + kBlock - 1) / kBlock) * ((cam->height + kBlock - 1) / kBlock);
   gsb_count_launch(1);
-  k_setup_cam<<<1, 32, 0, st>>>(gv.cam, cam_args(cam, g));
+  k_setup_cam<<<V, 32, 0, st>>>(gv.cam, cam_args(cam, g));
   // aux (the per-forward counters) sits immediately before tcount: one memset clears both
-  GSB_CUDA(cudaMemsetAsync(gv.aux, 0, (size_t)((char*)gv.tcount - (char*)gv.aux) + (size_t)ntiles * 4, st));
+  GSB_CUDA(cudaMemsetAsync(gv.aux, 0, (size_t)((char*)gv.tcount - (char*)gv.aux) + (size_t)V * ntiles * 4, st));
   if (P > 0) {
     const int nb = (P + kPT - 1) / kPT;
     ProfScope ps(GSB_K_PREPROCESS, st, 2);
-    (in.mip.on ? k_preprocess<true> : k_preprocess<false>)<<<nb, kPT, kPrepSmem, st>>>(in, gv, radii);
-    rc = gsb_launch_big_rects(P, gv, nullptr, cam->width, cam->height, cam->exact_cull, 0u, st);   // count mode
+    (in.mip.on ? k_preprocess<true> : k_preprocess<false>)<<<dim3(nb, V), kPT, kPrepSmem, st>>>(in, gv, radii);
+    rc = gsb_launch_big_rects(P, V, gv, nullptr, cam->width, cam->height, cam->exact_cull, 0u, st);   // count mode
     if (rc) return rc;
   }
-  rc = gsb_launch_tile_scan(gv, ntiles, st);
+  rc = gsb_launch_tile_scan(gv, V * ntiles, st);
   if (rc) return rc;
   if (status_host) GSB_CUDA(cudaMemcpyAsync(status_host, gv.status, 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   GSB_CUDA(cudaGetLastError());
   return GSB_OK;
+}
+
+extern "C" GSB_API int gsb_preprocess_ex(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt,
+                                         void* geom, size_t geom_bytes, int32_t* radii, uint32_t* status_host,
+                                         gsb_stream_t stream) {
+  return preprocess_views(cam, g, filt, 1, geom, geom_bytes, radii, status_host, (cudaStream_t)stream);
+}
+
+extern "C" GSB_API int gsb_preprocess_batch(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt,
+                                            int32_t V, const float* poses7, void* geom, size_t geom_bytes,
+                                            int32_t* radii, uint32_t* status_host, gsb_stream_t stream) {
+  GSB_REQUIRE(g && poses7, "gsb_preprocess_batch: null gaussians / poses");
+  GsbGaussians gb = *g;
+  gb.pose = poses7;
+  return preprocess_views(cam, &gb, filt, V, geom, geom_bytes, radii, status_host, (cudaStream_t)stream);
 }
 
 extern "C" GSB_API int gsb_preprocess(const GsbCamera* cam, const GsbGaussians* g, void* geom, size_t geom_bytes,
@@ -777,31 +830,66 @@ extern "C" GSB_API int gsb_preprocess(const GsbCamera* cam, const GsbGaussians* 
   return gsb_preprocess_ex(cam, g, nullptr, geom, geom_bytes, radii, status_host, stream);
 }
 
-extern "C" GSB_API int gsb_render(const GsbCamera* cam, int32_t P, void* geom, void* binning, size_t binning_bytes,
-                          int64_t R, void* image, float* out_color, uint32_t* status_host, gsb_stream_t stream_) {
-  cudaStream_t st = (cudaStream_t)stream_;
+static int render_views(const GsbCamera* cam, int32_t P, int V, void* geom, void* binning, size_t binning_bytes,
+                        int64_t R, void* image, float* out_color, uint32_t* status_host, cudaStream_t st) {
   GSB_REQUIRE(cam && geom && binning && image && out_color, "null buffer");
   GSB_REQUIRE(R >= 0 && R < (int64_t)0x7fffffff, "R out of range");
+  GSB_REQUIRE(V >= 1 && V <= 65535 && P >= 0 && (long long)V * P < 0x7fffffffLL, "bad V / P");
   const int W = cam->width, H = cam->height;
-  GeomView gv = geom_view(geom, P);
-  BinView bv = bin_view(binning, R, W, H);
+  GeomView gv = geom_view(geom, P, V, frame_tiles(W, H));
+  BinView bv = bin_view(binning, R, W, H, V);
   if (bv.total > binning_bytes) { gsb_set_error("binning buffer too small"); return GSB_ERR_CAPACITY; }
-  ImgView iv = img_view(image, W, H);
-  int rc = gsb_launch_binning(P, gv, bv, W, H, cam->exact_cull, (uint32_t)R, st);
+  ImgView iv = img_view(image, W, H, V);
+  int rc = gsb_launch_binning(P, V, gv, bv, W, H, cam->exact_cull, (uint32_t)R, st);
   if (rc) return rc;
-  rc = gsb_launch_blend_fwd(gv, bv, iv, cam->bg, W, H, out_color, st);
+  rc = gsb_launch_blend_fwd(gv, bv, iv, cam->bg, W, H, V, out_color, st);
   if (rc) return rc;
   if (status_host) GSB_CUDA(cudaMemcpyAsync(status_host, gv.status, 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   GSB_CUDA(cudaGetLastError());
   return GSB_OK;
 }
 
+extern "C" GSB_API int gsb_render(const GsbCamera* cam, int32_t P, void* geom, void* binning, size_t binning_bytes,
+                          int64_t R, void* image, float* out_color, uint32_t* status_host, gsb_stream_t stream) {
+  return render_views(cam, P, 1, geom, binning, binning_bytes, R, image, out_color, status_host, (cudaStream_t)stream);
+}
+
+extern "C" GSB_API int gsb_render_batch(const GsbCamera* cam, int32_t P, int32_t V, void* geom, void* binning,
+                                        size_t binning_bytes, int64_t R, void* image, float* out_color,
+                                        uint32_t* status_host, gsb_stream_t stream) {
+  return render_views(cam, P, V, geom, binning, binning_bytes, R, image, out_color, status_host, (cudaStream_t)stream);
+}
+
+static int backward_views(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, const GsbDensifyStats* stats,
+                          int V, void* geom, void* binning, int64_t R, void* image, const float* dL_dout,
+                          const GsbGrads* grads, cudaStream_t st);
+
 extern "C" GSB_API int gsb_backward_stats(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt,
                                           const GsbDensifyStats* stats, void* geom, void* binning, int64_t R, void* image,
-                                          const float* dL_dout, const GsbGrads* grads, gsb_stream_t stream_) {
-  cudaStream_t st = (cudaStream_t)stream_;
+                                          const float* dL_dout, const GsbGrads* grads, gsb_stream_t stream) {
+  return backward_views(cam, g, filt, stats, 1, geom, binning, R, image, dL_dout, grads, (cudaStream_t)stream);
+}
+
+extern "C" GSB_API int gsb_backward_pose_batch(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt,
+                                               int32_t V, const float* poses7, void* geom, void* binning, int64_t R,
+                                               void* image, const float* dL_dout, float* dpose7, gsb_stream_t stream) {
+  GSB_REQUIRE(g && poses7 && dpose7, "gsb_backward_pose_batch: null gaussians / poses / dpose");
+  GsbGaussians gb = *g;
+  gb.pose = poses7;
+  GsbGrads gr;
+  memset(&gr, 0, sizeof(gr));
+  gr.dL_dpose = dpose7;
+  return backward_views(cam, &gb, filt, nullptr, V, geom, binning, R, image, dL_dout, &gr, (cudaStream_t)stream);
+}
+
+// Per-Gaussian gradients and densification statistics are single-view only (V = 1); a batch computes dL/dpose per view.
+static int backward_views(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, const GsbDensifyStats* stats,
+                          int V, void* geom, void* binning, int64_t R, void* image, const float* dL_dout,
+                          const GsbGrads* grads, cudaStream_t st) {
+  int rc = batch_args(V, cam, g);
+  if (rc) return rc;
   InPtrs in;
-  int rc = make_inptrs(cam, g, in);
+  rc = make_inptrs(cam, g, in);
   if (rc) return rc;
   rc = apply_filter(filt, g, in);
   if (rc) return rc;
@@ -811,24 +899,24 @@ extern "C" GSB_API int gsb_backward_stats(const GsbCamera* cam, const GsbGaussia
     GSB_REQUIRE((stats->radii && stats->grad_accum && stats->denom && stats->max_radii2D) || g->P == 0,
                 "GsbDensifyStats: null buffer");
   const int P = g->P, W = cam->width, H = cam->height;
-  GeomView gv = geom_view(geom, P);
-  BinView bv = bin_view(binning, R, W, H);
-  ImgView iv = img_view(image, W, H);
+  GeomView gv = geom_view(geom, P, V, frame_tiles(W, H));
+  BinView bv = bin_view(binning, R, W, H, V);
+  ImgView iv = img_view(image, W, H, V);
   rc = ensure_attrs();
   if (rc) return rc;
   if (P == 0) {
-    if (grads->dL_dpose) GSB_CUDA(cudaMemsetAsync(grads->dL_dpose, 0, 7 * 4, st));
+    if (grads->dL_dpose) GSB_CUDA(cudaMemsetAsync(grads->dL_dpose, 0, (size_t)V * 7 * 4, st));
     return GSB_OK;
   }
-  GSB_CUDA(cudaMemsetAsync(gv.dacc, 0, (size_t)P * kDaccSlots * 8, st));
-  GSB_CUDA(cudaMemsetAsync(gv.dscale, 0, 4, st));
+  GSB_CUDA(cudaMemsetAsync(gv.dacc, 0, (size_t)V * P * kDaccSlots * 8, st));
+  GSB_CUDA(cudaMemsetAsync(gv.dscale, 0, (size_t)V * 4, st));
   // tracking mode (render.py:99-170): only dL/dpose is wanted -> the blend backward reduces 8 values instead of 9.
   // Not with the 2D Mip filter: o_eff depends on Sigma2 and so on the pose, whose gradient then needs S w (slot 5).
   const bool pose_only = !in.mip.on2d && g->pose && grads->dL_dpose && !grads->dL_dmeans3D && !grads->dL_dmeans2D && !grads->dL_dscales &&
                          !grads->dL_drotations && !grads->dL_dopacities && !grads->dL_dsh_dc && !grads->dL_dsh_rest &&
                          !grads->dL_dcolors && !grads->dL_dcov3D && gsb_option_blend_version() == 2 &&
                          gsb_option_stage_bulk() == 1;
-  rc = gsb_launch_blend_bwd(gv, bv, iv, cam->bg, W, H, dL_dout, pose_only, st);
+  rc = gsb_launch_blend_bwd(gv, bv, iv, cam->bg, W, H, V, dL_dout, pose_only, st);
   if (rc) return rc;
   OutPtrs out;
   out.dmeans = grads->dL_dmeans3D; out.dmeans2D = grads->dL_dmeans2D; out.dscales = grads->dL_dscales;
@@ -844,10 +932,10 @@ extern "C" GSB_API int gsb_backward_stats(const GsbCamera* cam, const GsbGaussia
   { ProfScope ps(GSB_K_PREPROCESS_BWD, st, g->pose ? 3 : 1);
     auto kern = in.mip.on ? (stats ? k_preprocess_bwd<true, true> : k_preprocess_bwd<true, false>)
                           : (stats ? k_preprocess_bwd<false, true> : k_preprocess_bwd<false, false>);
-    kern<<<nb, kPT, kPrepSmem, st>>>(in, gv, pose_only ? 1 : 0, out, sp);
+    kern<<<dim3(nb, V), kPT, kPrepSmem, st>>>(in, gv, pose_only ? 1 : 0, out, sp);
     if (g->pose) {
-      k_pose_reduce<<<16, 256, 0, st>>>(gv.pose_part, nb, gv.pose_acc);
-      k_pose_finalize<<<1, 32, 0, st>>>(gv.pose_acc, g->pose, grads->dL_dpose);
+      k_pose_reduce<<<dim3(16, V), 256, 0, st>>>(gv.pose_part, nb, gv.pose_acc);
+      k_pose_finalize<<<V, 32, 0, st>>>(gv.pose_acc, g->pose, grads->dL_dpose);
     } }
   GSB_CUDA(cudaGetLastError());
   return GSB_OK;

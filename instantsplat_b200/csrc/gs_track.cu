@@ -16,15 +16,26 @@ namespace {
 constexpr int kLT = 256;
 
 // sums[0] += sum |img - gt| * mask, sums[1] += sum mask;  dL_dimg = sign(img - gt) * mask (unnormalised)
+// Grid y = view: view v reads img, gt and writes dL at v * n and adds into sums[2v..2v+1].  Thread k always takes the
+// elements in groups of four (4k..4k+3, then the n % 4 tail), whatever the alignment of the pointers: the split into
+// blocks and threads -- and so the float partial sums -- depends only on n and the grid, so a view of a batch, a slice
+// of a caller's tensor and a fresh copy of it give the same bits.  Alignment only selects 128-bit or scalar accesses.
 __global__ void __launch_bounds__(kLT) k_l1_mask(size_t n, const float* __restrict__ img, const float* __restrict__ gt,
                                                  float thr, double* __restrict__ sums, float* __restrict__ dL) {
   __shared__ float red[2][kLT / 32];
   float s_abs = 0.f, s_m = 0.f;
   const size_t n4 = n >> 2;
+  img += n * blockIdx.y; gt += n * blockIdx.y; dL += n * blockIdx.y; sums += 2 * blockIdx.y;
   const bool vec = ((((uintptr_t)img | (uintptr_t)gt | (uintptr_t)dL) & 15) == 0);
-  for (size_t k = (size_t)blockIdx.x * kLT + threadIdx.x; k < (vec ? n4 : 0); k += (size_t)gridDim.x * kLT) {
-    const float4 a = __ldg(reinterpret_cast<const float4*>(img) + k), b = __ldg(reinterpret_cast<const float4*>(gt) + k);
-    const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
+  for (size_t k = (size_t)blockIdx.x * kLT + threadIdx.x; k < n4; k += (size_t)gridDim.x * kLT) {
+    float av[4], bv[4];
+    if (vec) {
+      const float4 a = __ldg(reinterpret_cast<const float4*>(img) + k), b = __ldg(reinterpret_cast<const float4*>(gt) + k);
+      av[0] = a.x; av[1] = a.y; av[2] = a.z; av[3] = a.w; bv[0] = b.x; bv[1] = b.y; bv[2] = b.z; bv[3] = b.w;
+    } else {
+#pragma unroll
+      for (int u = 0; u < 4; ++u) { av[u] = __ldg(img + 4 * k + u); bv[u] = __ldg(gt + 4 * k + u); }
+    }
     float g[4];
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
@@ -33,9 +44,14 @@ __global__ void __launch_bounds__(kLT) k_l1_mask(size_t n, const float* __restri
       s_m += m;
       g[u] = m * (d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f));
     }
-    reinterpret_cast<float4*>(dL)[k] = make_float4(g[0], g[1], g[2], g[3]);
+    if (vec) {
+      reinterpret_cast<float4*>(dL)[k] = make_float4(g[0], g[1], g[2], g[3]);
+    } else {
+#pragma unroll
+      for (int u = 0; u < 4; ++u) dL[4 * k + u] = g[u];
+    }
   }
-  for (size_t e = (vec ? 4 * n4 : 0) + (size_t)blockIdx.x * kLT + threadIdx.x; e < n; e += (size_t)gridDim.x * kLT) {
+  for (size_t e = 4 * n4 + (size_t)blockIdx.x * kLT + threadIdx.x; e < n; e += (size_t)gridDim.x * kLT) {
     const float m = img[e] > thr ? 1.f : 0.f, d = img[e] - gt[e];
     s_abs += fabsf(d) * m;
     s_m += m;
@@ -59,11 +75,16 @@ __global__ void __launch_bounds__(kLT) k_l1_mask(size_t n, const float* __restri
 
 struct TrackArgs {
   float* pose; const float* dpose_raw; const double* sums; float* m; float* v; float* best; float* loss_out;
+  int64_t loss_stride;
   float lr_q, lr_T, b1, b2, eps, wd, bc1, bc2_sqrt;
 };
 
+// one CTA per view: view w steps pose[7w..], keeps its candidate in best[8w..] and writes its loss at loss_out[w * stride]
 __global__ void k_track_step(TrackArgs a) {
-  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  if (threadIdx.x != 0) return;
+  const int w = blockIdx.x;
+  a.pose += 7 * w; a.dpose_raw += 7 * w; a.sums += 2 * w; a.m += 7 * w; a.v += 7 * w; a.best += 8 * w;
+  if (a.loss_out) a.loss_out += a.loss_stride * w;
   const double cnt = a.sums[1];
   const float inv = cnt > 0.0 ? (float)(1.0 / cnt) : 0.f;
   const float loss = cnt > 0.0 ? (float)(a.sums[0] / cnt) : 0.f;
@@ -156,15 +177,41 @@ extern "C" GSB_API int gsb_mip_filter3d(int32_t P, const float* xyz, int32_t n_v
   return GSB_OK;
 }
 
-extern "C" GSB_API int gsb_l1_mask_fwd_bwd(int32_t C, int32_t H, int32_t W, const float* img, const float* gt,
-                                           float threshold, double* sums, float* dL_dimg, gsb_stream_t stream_) {
+extern "C" GSB_API int gsb_l1_mask_fwd_bwd_batch(int32_t V, int32_t C, int32_t H, int32_t W, const float* img,
+                                                 const float* gt, float threshold, double* sums, float* dL_dimg,
+                                                 gsb_stream_t stream_) {
   cudaStream_t st = (cudaStream_t)stream_;
-  GSB_REQUIRE(C > 0 && H > 0 && W > 0 && img && gt && sums && dL_dimg, "gsb_l1_mask_fwd_bwd: bad argument");
+  GSB_REQUIRE(V >= 1 && V <= 65535 && C > 0 && H > 0 && W > 0 && img && gt && sums && dL_dimg,
+              "gsb_l1_mask_fwd_bwd: bad argument");
   const size_t n = (size_t)C * H * W;
   const int max_blocks = 8 * gsb_sm_count();
   const int blocks = (int)((n / 4 + kLT - 1) / kLT < (size_t)max_blocks ? (n / 4 + kLT - 1) / kLT + 1 : max_blocks);
   ProfScope ps(GSB_K_LOSS_FWD, st);
-  k_l1_mask<<<blocks, kLT, 0, st>>>(n, img, gt, threshold, sums, dL_dimg);
+  k_l1_mask<<<dim3(blocks, V), kLT, 0, st>>>(n, img, gt, threshold, sums, dL_dimg);
+  GSB_CUDA(cudaGetLastError());
+  return GSB_OK;
+}
+
+extern "C" GSB_API int gsb_l1_mask_fwd_bwd(int32_t C, int32_t H, int32_t W, const float* img, const float* gt,
+                                           float threshold, double* sums, float* dL_dimg, gsb_stream_t stream) {
+  return gsb_l1_mask_fwd_bwd_batch(1, C, H, W, img, gt, threshold, sums, dL_dimg, stream);
+}
+
+extern "C" GSB_API int gsb_track_step_batch(int32_t V, float* pose7, const float* dpose7_raw, const double* sums2,
+                                            float* exp_avg7, float* exp_avg_sq7, float* best8, float* loss_out,
+                                            int64_t loss_stride, int32_t step, float lr_q, float lr_T, float beta1,
+                                            float beta2, float eps, float weight_decay, gsb_stream_t stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  GSB_REQUIRE(V >= 1 && V <= 65535 && pose7 && dpose7_raw && sums2 && exp_avg7 && exp_avg_sq7 && best8 && step >= 1,
+              "gsb_track_step: bad argument");
+  TrackArgs a;
+  a.pose = pose7; a.dpose_raw = dpose7_raw; a.sums = sums2; a.m = exp_avg7; a.v = exp_avg_sq7; a.best = best8;
+  a.loss_out = loss_out; a.loss_stride = loss_stride;
+  a.lr_q = lr_q; a.lr_T = lr_T; a.b1 = beta1; a.b2 = beta2; a.eps = eps; a.wd = weight_decay;
+  a.bc1 = (float)(1.0 - pow((double)beta1, (double)step));
+  a.bc2_sqrt = (float)sqrt(1.0 - pow((double)beta2, (double)step));
+  ProfScope ps(GSB_K_ADAM, st);
+  k_track_step<<<V, 32, 0, st>>>(a);
   GSB_CUDA(cudaGetLastError());
   return GSB_OK;
 }
@@ -172,17 +219,7 @@ extern "C" GSB_API int gsb_l1_mask_fwd_bwd(int32_t C, int32_t H, int32_t W, cons
 extern "C" GSB_API int gsb_track_step(float* pose7, const float* dpose7_raw, const double* sums2, float* exp_avg7,
                                       float* exp_avg_sq7, float* best8, float* loss_out, int32_t step, float lr_q,
                                       float lr_T, float beta1, float beta2, float eps, float weight_decay,
-                                      gsb_stream_t stream_) {
-  cudaStream_t st = (cudaStream_t)stream_;
-  GSB_REQUIRE(pose7 && dpose7_raw && sums2 && exp_avg7 && exp_avg_sq7 && best8 && step >= 1, "gsb_track_step: bad argument");
-  TrackArgs a;
-  a.pose = pose7; a.dpose_raw = dpose7_raw; a.sums = sums2; a.m = exp_avg7; a.v = exp_avg_sq7; a.best = best8;
-  a.loss_out = loss_out;
-  a.lr_q = lr_q; a.lr_T = lr_T; a.b1 = beta1; a.b2 = beta2; a.eps = eps; a.wd = weight_decay;
-  a.bc1 = (float)(1.0 - pow((double)beta1, (double)step));
-  a.bc2_sqrt = (float)sqrt(1.0 - pow((double)beta2, (double)step));
-  ProfScope ps(GSB_K_ADAM, st);
-  k_track_step<<<1, 32, 0, st>>>(a);
-  GSB_CUDA(cudaGetLastError());
-  return GSB_OK;
+                                      gsb_stream_t stream) {
+  return gsb_track_step_batch(1, pose7, dpose7_raw, sums2, exp_avg7, exp_avg_sq7, best8, loss_out, 0, step, lr_q, lr_T,
+                              beta1, beta2, eps, weight_decay, stream);
 }

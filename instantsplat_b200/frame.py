@@ -123,17 +123,26 @@ class Frame:
     """Scratch of forwards at one (device, P, W, H): the geometry buffer (which holds the status words), radii, the
     image buffer, the rendered colour [3, H, W], and a binning buffer of `cap` instances (0: none yet).
 
+    views: scratch of a batch of that many views of the same Gaussians and intrinsics (the *_batch methods,
+    gsb_preprocess_batch and friends); radii is then [views, P] and color [views, 3, H, W].  None: one view.
+
     host_status arguments are the caller's pinned 8-word slots (or None): the library copies the status words there
     after the phase."""
 
-    def __init__(self, device, P, W, H):
+    def __init__(self, device, P, W, H, views=None):
         L = _lib.lib()
-        self.P, self.W, self.H = P, W, H
-        self.geom = torch.empty(L.gsb_geom_bytes(P), dtype=torch.uint8, device=device)
-        self.radii = torch.empty(P, dtype=torch.int32, device=device)
-        self.image = torch.empty(L.gsb_image_bytes(W, H), dtype=torch.uint8, device=device)
-        self.color = torch.empty(3, H, W, dtype=torch.float32, device=device)
-        self._so = L.gsb_status_device(self.geom.data_ptr(), P) - self.geom.data_ptr()
+        self.P, self.W, self.H, self.views = P, W, H, 1 if views is None else int(views)
+        if views is None:
+            geom_bytes, image_bytes = L.gsb_geom_bytes(P), L.gsb_image_bytes(W, H)
+            self.radii = torch.empty(P, dtype=torch.int32, device=device)
+            self.color = torch.empty(3, H, W, dtype=torch.float32, device=device)
+        else:
+            geom_bytes, image_bytes = L.gsb_geom_bytes_batch(P, views, W, H), L.gsb_image_bytes_batch(W, H, views)
+            self.radii = torch.empty(views, P, dtype=torch.int32, device=device)
+            self.color = torch.empty(views, 3, H, W, dtype=torch.float32, device=device)
+        self.geom = torch.empty(geom_bytes, dtype=torch.uint8, device=device)
+        self.image = torch.empty(image_bytes, dtype=torch.uint8, device=device)
+        self._so = L.gsb_status_device_batch(self.geom.data_ptr(), P, self.views) - self.geom.data_ptr()
         self.binning, self.cap = None, 0
 
     @property
@@ -147,7 +156,7 @@ class Frame:
 
     def alloc_binning(self, cap: int, round_to: int = 1) -> None:
         """A new binning buffer of `cap` instances, its byte size rounded up to a multiple of round_to."""
-        nbytes = (_lib.lib().gsb_binning_bytes(cap, self.W, self.H) + round_to - 1) // round_to * round_to
+        nbytes = (_lib.lib().gsb_binning_bytes_batch(cap, self.W, self.H, self.views) + round_to - 1) // round_to * round_to
         self.binning = torch.empty(nbytes, dtype=torch.uint8, device=self.geom.device)
         self.cap = cap
 
@@ -178,3 +187,24 @@ class Frame:
         check(_lib.lib().gsb_blend_stats(ctypes.byref(cam), self.P, self.geom.data_ptr(), self.binning.data_ptr(),
                                          self.cap, self.image.data_ptr(), self.color.data_ptr(), dL_dimage.data_ptr(),
                                          stats.data_ptr(), _lib.stream_ptr()), "gsb_blend_stats")
+
+    # ---- a batch of views (views > 1; gsb200.h "batched tracking") ----------------------------------------------
+    def preprocess_batch(self, cam, g, poses7, host_status=None, filt=None) -> None:
+        """poses7: contiguous fp32 [views, 7] device tensor; g holds raw parameters (its pose is not used)."""
+        check(_lib.lib().gsb_preprocess_batch(ctypes.byref(cam), ctypes.byref(g), _f(filt), self.views,
+                                              poses7.data_ptr(), self.geom.data_ptr(), self.geom.numel(),
+                                              self.radii.data_ptr(), _p(host_status), _lib.stream_ptr()),
+              "gsb_preprocess_batch")
+
+    def render_batch(self, cam, host_status=None) -> None:
+        check(_lib.lib().gsb_render_batch(ctypes.byref(cam), self.P, self.views, self.geom.data_ptr(),
+                                          self.binning.data_ptr(), self.binning.numel(), self.cap,
+                                          self.image.data_ptr(), self.color.data_ptr(), _p(host_status),
+                                          _lib.stream_ptr()), "gsb_render_batch")
+
+    def backward_pose_batch(self, cam, g, poses7, dL_dimage, dpose7, filt=None) -> None:
+        """dL_dimage [views, 3, H, W] -> dpose7 [views, 7] (pose gradients only)."""
+        check(_lib.lib().gsb_backward_pose_batch(ctypes.byref(cam), ctypes.byref(g), _f(filt), self.views,
+                                                 poses7.data_ptr(), self.geom.data_ptr(), self.binning.data_ptr(),
+                                                 self.cap, self.image.data_ptr(), dL_dimage.data_ptr(),
+                                                 dpose7.data_ptr(), _lib.stream_ptr()), "gsb_backward_pose_batch")
