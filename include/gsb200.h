@@ -232,7 +232,14 @@ GSB_API int gsb_track_step(float* pose7, const float* dpose7_raw, const double* 
  * truncated (memory-safe, as in gsb_render).
  *
  * Sizes: geom grows by ~145 bytes per (view, Gaussian), the image buffer and out_color by V frames, binning by
- * 8 bytes per tile and view; at V = 1 each is at least the single-view size. */
+ * 8 bytes per tile and view; at V = 1 each is at least the single-view size.
+ *
+ * Batched training (several views per optimizer step, JointTrainer.step_batch): gsb_backward_batch writes the
+ * per-Gaussian gradients of all V views SUMMED in view order -- for every element ((g_0 + g_1) + g_2) + ... in fp32,
+ * bit-identical to V single-view backward calls whose outputs are added in that order -- plus dL/dpose per view.  It
+ * stages each Gaussian slice once and loops over the views inside one launch; no per-view gradient copy is written.
+ * gsb_loss_forward_batch / gsb_loss_backward_batch are the training loss on V images, each view's sums and dL/dimg
+ * exactly those of gsb_loss_forward / gsb_loss_backward on it.  Densification statistics stay single-view. */
 GSB_API size_t gsb_geom_bytes_batch(int32_t P, int32_t V, int32_t width, int32_t height);
 GSB_API size_t gsb_binning_bytes_batch(int64_t R, int32_t width, int32_t height, int32_t V);
 GSB_API size_t gsb_image_bytes_batch(int32_t width, int32_t height, int32_t V);
@@ -252,6 +259,21 @@ GSB_API int gsb_render_batch(const GsbCamera* cam, int32_t P, int32_t V, void* g
 GSB_API int gsb_backward_pose_batch(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, int32_t V,
                                     const float* poses7, void* geom, void* binning, int64_t R, void* image,
                                     const float* dL_dout, float* dpose7, gsb_stream_t stream);
+/* gsb_backward_ex for the batch with every per-Gaussian gradient of `grads` summed over the V views (see above);
+ * dL_dout [V, 3, H, W], dpose7 [V, 7] (grads->dL_dpose is ignored).  Needs SH colours and scale / rotation (no
+ * dL_dcolors / dL_dcov3D); the 2D and 3D Mip filters of filt apply to every view.  V = 1 gives gsb_backward_ex's bits. */
+GSB_API int gsb_backward_batch(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, int32_t V,
+                               const float* poses7, void* geom, void* binning, int64_t R, void* image,
+                               const float* dL_dout, const GsbGrads* grads, float* dpose7, gsb_stream_t stream);
+/* gsb_loss_forward / gsb_loss_backward on V images img [V, C, H, W]: view v's target is the [C, H, W] block
+ * gt + gt_row[v] * C*H*W (gt_row: device int32 [V], so that one captured launch serves any choice of targets).
+ * sums [V, 2] (double, caller zeroes), maps [3, V, C, H, W]; dL_dimg [V, C, H, W], each view scaled by 1/N with
+ * N = C*H*W as in gsb_loss_backward (a mean over views is the caller's factor). */
+GSB_API int gsb_loss_forward_batch(int32_t V, int32_t C, int32_t H, int32_t W, const float* img, const float* gt,
+                                   const int32_t* gt_row, double* sums, float* maps, gsb_stream_t stream);
+GSB_API int gsb_loss_backward_batch(int32_t V, int32_t C, int32_t H, int32_t W, const float* img, const float* gt,
+                                    const int32_t* gt_row, const float* maps, float lambda_dssim, float* dL_dimg,
+                                    gsb_stream_t stream);
 /* gsb_l1_mask_fwd_bwd on V images [V, C, H, W] at once; sums [V, 2] (double, caller zeroes). */
 GSB_API int gsb_l1_mask_fwd_bwd_batch(int32_t V, int32_t C, int32_t H, int32_t W, const float* img, const float* gt,
                                       float threshold, double* sums, float* dL_dimg, gsb_stream_t stream);

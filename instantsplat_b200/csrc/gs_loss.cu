@@ -116,9 +116,14 @@ __device__ __forceinline__ float2 bcast(float w) { return make_float2(w, w); }
 // (two float2 accumulators) and E[ab] (scalar).  Horizontal: thread -> (row, 4 adjacent columns), inputs fetched
 // with seven 128-bit shared loads.  Vertical: thread -> (column, 2 adjacent rows).
 // img planes [BC][H][W].  maps (optional) [3][BC][H][W].  sums[0] += sum|a-b| (if do_l1), sums[1] += sum ssim.
+// kViews: a batch of views of C planes each (BC = V * C): plane z = v * C + c of img1 is compared with plane
+// gt_row[v] * C + c of img2, and view v's sums go to sums[2v], sums[2v + 1].  Every plane keeps the single-view CTA
+// split, so each view's partials are those of the single-view call.
+template <bool kViews = false>
 __global__ void __launch_bounds__(256, 4)
 k_ssim_fwd(int H, int W, const float* __restrict__ img1, const float* __restrict__ img2,
-           double* __restrict__ sums, float* __restrict__ maps, size_t plane_total, int do_l1) {
+           double* __restrict__ sums, float* __restrict__ maps, size_t plane_total, int do_l1, int C = 1,
+           const int32_t* __restrict__ gt_row = nullptr) {
   __shared__ __align__(16) float2 sAB[EH][EWP];
   __shared__ __align__(16) float2 sH1[EH][HS];     // {E_h[a], E_h[b]}
   __shared__ __align__(16) float2 sH2[EH][HS];     // {E_h[a^2], E_h[b^2]}
@@ -126,10 +131,16 @@ k_ssim_fwd(int H, int W, const float* __restrict__ img1, const float* __restrict
   __shared__ float red[8];
   const int bc = blockIdx.z;
   const int x0 = blockIdx.x * TW, y0 = blockIdx.y * TH;
+  size_t gt_plane = bc;
+  if constexpr (kViews) {
+    const int v = bc / C;
+    gt_plane = (size_t)__ldg(gt_row + v) * C + (bc - v * C);
+    sums += 2 * v;
+  }
   {
     HaloRegs ha, hb;
     halo_load(ha, img1 + (size_t)bc * H * W, H, W, x0, y0);
-    halo_load(hb, img2 + (size_t)bc * H * W, H, W, x0, y0);
+    halo_load(hb, img2 + gt_plane * H * W, H, W, x0, y0);
     halo_store2(ha, hb, sAB);
   }
   __syncthreads();
@@ -215,11 +226,14 @@ k_ssim_fwd(int H, int W, const float* __restrict__ img1, const float* __restrict
 }
 
 // out = ssim_scale * (conv(m_mu) + 2 x conv(m_s1) + y conv(m_s12)) [* *dyn_scale] + l1_scale * sign(x-y)
-// The first two maps travel as one float2 through both filter passes.
+// The first two maps travel as one float2 through both filter passes.  kViews: y from plane gt_row[v] * C + c of img2
+// (as in k_ssim_fwd<true>).
+template <bool kViews = false>
 __global__ void __launch_bounds__(256, 5)
 k_ssim_bwd(int H, int W, const float* __restrict__ img1, const float* __restrict__ img2,
            const float* __restrict__ maps, size_t plane_total, float ssim_scale,
-           const float* __restrict__ dyn_scale, float l1_scale, float* __restrict__ out) {
+           const float* __restrict__ dyn_scale, float l1_scale, float* __restrict__ out, int C = 1,
+           const int32_t* __restrict__ gt_row = nullptr) {
   __shared__ __align__(16) float2 sM12[EH][EWP];
   __shared__ __align__(16) float sM3[EH][EWP];
   __shared__ __align__(16) float2 sH12[EH][HS];
@@ -227,6 +241,11 @@ k_ssim_bwd(int H, int W, const float* __restrict__ img1, const float* __restrict
   const int bc = blockIdx.z;
   const int x0 = blockIdx.x * TW, y0 = blockIdx.y * TH;
   const size_t pbase = (size_t)bc * H * W;
+  size_t gbase = pbase;
+  if constexpr (kViews) {
+    const int v = bc / C;
+    gbase = ((size_t)__ldg(gt_row + v) * C + (bc - v * C)) * H * W;
+  }
   {
     HaloRegs h0, h1, h2;
     halo_load(h0, maps + pbase, H, W, x0, y0);
@@ -295,7 +314,7 @@ k_ssim_bwd(int H, int W, const float* __restrict__ img1, const float* __restrict
     const int x = x0 + tx, y = y0 + ty + o;
     if (x < W && y < H) {
       size_t off = pbase + (size_t)y * W + x;
-      float xv = img1[off], yv = img2[off];
+      float xv = img1[off], yv = img2[gbase + (size_t)y * W + x];
       float g = sc * (g12[o].x + 2.f * xv * g12[o].y + yv * g3[o]);
       if (l1_scale != 0.f) {
         float df = xv - yv;
@@ -367,4 +386,44 @@ extern "C" GSB_API int gsb_loss_backward(int32_t C, int32_t H, int32_t W, const 
                                                      (float)((1.0 - (double)lambda_dssim) / N), dL_dimg);
   gsb_prof_end(slot, (cudaStream_t)stream);
   return check(cudaGetLastError(), "k_loss_bwd");
+}
+
+// The loss of V views [V, C, H, W] in one launch each: view v against target plane block gt_row[v] of gt (device int32
+// [V]), its sums at sums[2v] and sums[2v + 1], its dL/dimg scaled by the single-view 1/N (N = C H W).
+extern "C" GSB_API int gsb_loss_forward_batch(int32_t V, int32_t C, int32_t H, int32_t W, const float* img,
+                                              const float* gt, const int32_t* gt_row, double* sums, float* maps,
+                                              gsb_stream_t stream) {
+  if (V <= 0 || V > 65535 / (C > 0 ? C : 1) || C <= 0 || H <= 0 || W <= 0 || !img || !gt || !gt_row || !sums || !maps) {
+    gsb_set_error("gsb_loss_forward_batch: bad argument");
+    return GSB_ERR_INVALID;
+  }
+  if (ensure_window()) return check(cudaGetLastError(), "window upload");
+  dim3 grid((W + TW - 1) / TW, (H + TH - 1) / TH, V * C);
+  gsb_count_launch(1);
+  int slot = gsb_prof_begin(GSB_K_LOSS_FWD, (cudaStream_t)stream);
+  k_ssim_fwd<true><<<grid, 256, 0, (cudaStream_t)stream>>>(H, W, img, gt, sums, maps, (size_t)V * C * H * W, 1, C,
+                                                            gt_row);
+  gsb_prof_end(slot, (cudaStream_t)stream);
+  return check(cudaGetLastError(), "k_loss_fwd_batch");
+}
+
+extern "C" GSB_API int gsb_loss_backward_batch(int32_t V, int32_t C, int32_t H, int32_t W, const float* img,
+                                               const float* gt, const int32_t* gt_row, const float* maps,
+                                               float lambda_dssim, float* dL_dimg, gsb_stream_t stream) {
+  if (V <= 0 || V > 65535 / (C > 0 ? C : 1) || C <= 0 || H <= 0 || W <= 0 || !img || !gt || !gt_row || !maps ||
+      !dL_dimg) {
+    gsb_set_error("gsb_loss_backward_batch: bad argument");
+    return GSB_ERR_INVALID;
+  }
+  if (ensure_window()) return check(cudaGetLastError(), "window upload");
+  const double N = (double)C * H * W;
+  dim3 grid((W + TW - 1) / TW, (H + TH - 1) / TH, V * C);
+  gsb_count_launch(1);
+  int slot = gsb_prof_begin(GSB_K_LOSS_BWD, (cudaStream_t)stream);
+  k_ssim_bwd<true><<<grid, 256, 0, (cudaStream_t)stream>>>(H, W, img, gt, maps, (size_t)V * C * H * W,
+                                                            (float)(-(double)lambda_dssim / N), nullptr,
+                                                            (float)((1.0 - (double)lambda_dssim) / N), dL_dimg, C,
+                                                            gt_row);
+  gsb_prof_end(slot, (cudaStream_t)stream);
+  return check(cudaGetLastError(), "k_loss_bwd_batch");
 }

@@ -162,16 +162,33 @@ GS_HD void sh_to_rgb(int D, const float* sh_dc, const float* sh_rest, float x, f
   }
 }
 
+// d/dsh store of sh_to_rgb_bwd: kAcc adds the value to what is there, rounded once (never contracted into an FMA), so
+// that a sum over views is the sum of the single-view values
+template <bool kAcc>
+GS_HD void sh_put(float& o, float v) {
+  if constexpr (kAcc) {
+#if defined(__CUDA_ARCH__)
+    o = __fadd_rn(o, v);
+#else
+    o = o + v;
+#endif
+  } else {
+    o = v;
+  }
+}
+
 // Backward of sh_to_rgb: writes d/dsh (dc: 3, rest: 3*(K-1) for the K active coeffs; inactive
 // ones are left untouched) and returns dL/ddir.  ALIAS-SAFE: d_rest may be the same memory as
 // sh_rest (each channel's coefficients are read into registers before that channel is written).
+// kAcc: add d/dsh to d_dc / d_rest instead (which must then not alias sh_rest).
+template <bool kAcc = false>
 GS_HD void sh_to_rgb_bwd(int D, const float* sh_rest, float x, float y, float z, const float* dL,
                          float* d_dc, float* d_rest, float* ddir) {
   float gx = 0.f, gy = 0.f, gz = 0.f;
   float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
   for (int ch = 0; ch < 3; ++ch) {
     float g = dL[ch];
-    d_dc[ch] = SH_C0 * g;
+    sh_put<kAcc>(d_dc[ch], SH_C0 * g);
     if (D > 0) {
       const float* s = sh_rest + ch;
       float* o = d_rest + ch;
@@ -193,16 +210,17 @@ GS_HD void sh_to_rgb_bwd(int D, const float* sh_rest, float x, float y, float z,
           dz += SH_C3_1 * c10 * xy + SH_C3_2 * c11 * 8.f * yz +
                 SH_C3_3 * c12 * (6.f * zz - 3.f * xx - 3.f * yy) + SH_C3_4 * c13 * 8.f * xz +
                 SH_C3_5 * c14 * (xx - yy);
-          o[24] = SH_C3_0 * y * (3.f * xx - yy) * g; o[27] = SH_C3_1 * xy * z * g;
-          o[30] = SH_C3_2 * y * (4.f * zz - xx - yy) * g;
-          o[33] = SH_C3_3 * z * (2.f * zz - 3.f * xx - 3.f * yy) * g;
-          o[36] = SH_C3_4 * x * (4.f * zz - xx - yy) * g; o[39] = SH_C3_5 * z * (xx - yy) * g;
-          o[42] = SH_C3_6 * x * (xx - 3.f * yy) * g;
+          sh_put<kAcc>(o[24], SH_C3_0 * y * (3.f * xx - yy) * g); sh_put<kAcc>(o[27], SH_C3_1 * xy * z * g);
+          sh_put<kAcc>(o[30], SH_C3_2 * y * (4.f * zz - xx - yy) * g);
+          sh_put<kAcc>(o[33], SH_C3_3 * z * (2.f * zz - 3.f * xx - 3.f * yy) * g);
+          sh_put<kAcc>(o[36], SH_C3_4 * x * (4.f * zz - xx - yy) * g); sh_put<kAcc>(o[39], SH_C3_5 * z * (xx - yy) * g);
+          sh_put<kAcc>(o[42], SH_C3_6 * x * (xx - 3.f * yy) * g);
         }
-        o[9] = SH_C2_0 * xy * g; o[12] = SH_C2_1 * yz * g; o[15] = SH_C2_2 * (2.f * zz - xx - yy) * g;
-        o[18] = SH_C2_3 * xz * g; o[21] = SH_C2_4 * (xx - yy) * g;
+        sh_put<kAcc>(o[9], SH_C2_0 * xy * g); sh_put<kAcc>(o[12], SH_C2_1 * yz * g);
+        sh_put<kAcc>(o[15], SH_C2_2 * (2.f * zz - xx - yy) * g);
+        sh_put<kAcc>(o[18], SH_C2_3 * xz * g); sh_put<kAcc>(o[21], SH_C2_4 * (xx - yy) * g);
       }
-      o[0] = -SH_C1 * y * g; o[3] = SH_C1 * z * g; o[6] = -SH_C1 * x * g;
+      sh_put<kAcc>(o[0], -SH_C1 * y * g); sh_put<kAcc>(o[3], SH_C1 * z * g); sh_put<kAcc>(o[6], -SH_C1 * x * g);
       gx += dx * g; gy += dy * g; gz += dz * g;
     }
   }
@@ -474,7 +492,8 @@ struct GaussGrad {
   float dcolor[3];      // dL/drgb after the clamp mask (colors_precomp path)
 };
 
-template <bool kMip = false>
+// kAcc: the SH gradient is added to d_sh_dc / d_sh_rest (sh_to_rgb_bwd<true>); everything else is unchanged
+template <bool kMip = false, bool kAcc = false>
 GS_HD void project_bwd(const CamConst& c, const GaussIn& in, const Proj& p, const float* sh_rest,
                        bool use_sh, bool cov_pre, const float* ds, GaussGrad& g, float* d_sh_dc,
                        float* d_sh_rest, float* pose_acc, const Mip mf = Mip()) {
@@ -489,7 +508,7 @@ GS_HD void project_bwd(const CamConst& c, const GaussIn& in, const Proj& p, cons
     float inv = 1.f / sqrtf(vx * vx + vy * vy + vz * vz);
     float dx = vx * inv, dy = vy * inv, dz = vz * inv;
     float ddir[3];
-    sh_to_rgb_bwd(c.D, sh_rest, dx, dy, dz, dL, d_sh_dc, d_sh_rest, ddir);
+    sh_to_rgb_bwd<kAcc>(c.D, sh_rest, dx, dy, dz, dL, d_sh_dc, d_sh_rest, ddir);
     float dot = dx * ddir[0] + dy * ddir[1] + dz * ddir[2];
     dmc[0] += (ddir[0] - dx * dot) * inv;
     dmc[1] += (ddir[1] - dy * dot) * inv;

@@ -11,7 +11,8 @@
 //   k_blend_fwd2       (gs_blend.cu) one CTA per 16x16 tile, TMA-staged slab chunks, two pixels per lane
 //   k_blend_bwd2       (gs_blend.cu) back-to-front replay, 9 gradients per (warp, Gaussian) reduced in-warp
 //   k_preprocess_bwd   analytic backward to the model's own tensors + in-kernel pose-gradient
-//                      reduction; k_pose_finalize chains it to dL/dP[7]
+//                      reduction; k_pose_finalize chains it to dL/dP[7].  <., false, true>: the gradients of a batch
+//                      of views summed in view order, inputs staged once per Gaussian slice (gsb_backward_batch)
 //
 // Reference behaviour: SURVEY.md Appendix A; call site gaussian_renderer/__init__.py:60-135.
 #include <string.h>
@@ -248,6 +249,9 @@ __device__ __forceinline__ void stage_out(float* __restrict__ dst, const float* 
 constexpr int kSmXyz = 0, kSmSc = 3 * kPT, kSmQ = 6 * kPT, kSmOp = 10 * kPT, kSmSh = 11 * kPT;
 constexpr int kSmFloats = 11 * kPT + kRowPad * kPT;
 constexpr size_t kPrepSmem = sizeof(CamConst) + 16 + (size_t)kSmFloats * 4;
+// The view-summing backward (k_preprocess_bwd<., false, true>) keeps the staged SH rows as inputs for every view and adds
+// each view's SH gradient into a second region of the same layout behind them.
+constexpr size_t kPrepSmemViews = kPrepSmem + (size_t)kRowPad * kPT * 4;
 
 __device__ __forceinline__ void copy_in(float* sm, const float* __restrict__ src, int n, bool vec) {
   if (vec) {
@@ -475,12 +479,185 @@ struct StatsPtrs {
   const int32_t* radii; float* accum; float* denom; float* max_r;
 };
 
+// The CTA's gradient rows (staging layout; SH rows at `sh`) -> the gradient tensors.  All threads call; returns whether
+// the stores were bulk copies, which read shared memory until bulk_wait_read().  Used by views_bwd; the single-view
+// instances keep the same code inline, which keeps their SASS the one measured before the view-summing instance.
+__device__ __forceinline__ bool store_block_grads(const InPtrs& in, const OutPtrs& out, const float* sm, const float* sh,
+                                                  int first, int nv, int M, bool use_sh, bool vec) {
+  // Full CTA, aligned, split SH layout: every gradient array of the CTA leaves as one bulk store (shared -> global)
+  // issued by one thread; the generic path below covers ragged / unaligned / packed cases.
+  const bool bulk_out = vec && nv == kPT && !in.sh_packed && M == 16;
+  if (bulk_out) tma_store_fence();
+  __syncthreads();
+  if (bulk_out) {
+    if (threadIdx.x == 0) {
+      constexpr uint32_t B3 = 3 * kPT * 4, B4 = 4 * kPT * 4, B1 = kPT * 4, BR = 45 * kPT * 4;
+      if (out.dmeans) bulk_s2g(out.dmeans + (size_t)3 * first, sm + kSmXyz, B3);
+      if (out.dscales) bulk_s2g(out.dscales + (size_t)3 * first, sm + kSmSc, B3);
+      if (out.drots) bulk_s2g(out.drots + (size_t)4 * first, sm + kSmQ, B4);
+      if (out.dopac) bulk_s2g(out.dopac + first, sm + kSmOp, B1);
+      if (use_sh && out.dsh_dc) {
+        bulk_s2g(out.dsh_dc + (size_t)3 * first, sh, B3);
+        if (out.dsh_rest) bulk_s2g(out.dsh_rest + (size_t)45 * first, sh + 3 * kPT, BR);
+      }
+      bulk_commit();
+    }
+  } else {
+    if (out.dmeans) copy_out(out.dmeans + (size_t)3 * first, sm + kSmXyz, 3 * nv, vec);
+    if (out.dscales) copy_out(out.dscales + (size_t)3 * first, sm + kSmSc, 3 * nv, vec);
+    if (out.drots) copy_out(out.drots + (size_t)4 * first, sm + kSmQ, 4 * nv, vec);
+    if (out.dopac) copy_out(out.dopac + first, sm + kSmOp, nv, vec);
+    if (use_sh && out.dsh_dc) {
+      if (in.sh_packed) {
+        stage_out(out.dsh_dc + (size_t)3 * M * first, sh, 3 * M * nv, 3 * M, kRowPad, 0, vec);
+      } else {
+        copy_out(out.dsh_dc + (size_t)3 * first, sh, 3 * nv, vec);
+        if (M > 1 && out.dsh_rest)
+          copy_out(out.dsh_rest + (size_t)3 * (M - 1) * first, sh + 3 * kPT, 3 * (M - 1) * nv, vec);
+      }
+    }
+  }
+  return bulk_out;
+}
+
+// The CTA's pose-gradient partials pa[16] (one set per thread): warp shuffle, then across the 8 warps; dst[16].
+// All threads call (one barrier).
+__device__ __forceinline__ void block_pose_partials(const float* pa, float (*s_pose)[16], float* dst) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int k = 0; k < 16; ++k) {
+    float v = pa[k];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (lane == 0) s_pose[warp][k] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x < 16) {
+    float v = 0.f;
+#pragma unroll
+    for (int w = 0; w < kPT / 32; ++w) v += s_pose[w][threadIdx.x];
+    dst[threadIdx.x] = v;
+  }
+}
+
+// k_preprocess_bwd<kMip, false, true>: the per-Gaussian gradients of `nviews` views, summed.  For every Gaussian and
+// gradient element the result is ((g_0 + g_1) + g_2) + ..., where g_v is what the single-view instance computes for
+// view v from that view's moments (record v * P + i, fixed-point unit gv.dscale[v]) and camera constants (gv.cam[v]).
+// The view-independent inputs are staged once by the caller; the running sums start at -0 (so the first view adds
+// exactly its own bits) and every view adds with __fadd_rn, which is never contracted into an FMA.  A view in which
+// the Gaussian has no moments adds the +0 the single-view call writes.  SH sums live in shared memory behind the
+// staged rows (kPrepSmemViews); the others in registers.  View v's pose partials go to pose_part row (v, CTA), the
+// layout of grid y = view, so k_pose_reduce / k_pose_finalize are unchanged.  Not for densification statistics.
+template <bool kMip>
+__device__ __forceinline__ void views_bwd(const InPtrs& in, const GeomView& gv, int pose_only_layout,
+                                          const OutPtrs& out, int nviews, CamConst* cam, float* sm,
+                                          float (*s_pose)[16], int first, int nv, bool use_sh, bool vec) {
+  const int t = threadIdx.x, i = first + t;
+  const int D = cam->D, M = cam->M;
+  const ShRows sr = sh_rows(in.sh_packed, M);
+  const float* row_rest = sm + kSmSh + sr.rest_off + sr.rest_stride * t;
+  float* const acc = sm + kSmFloats;
+  float* const acc_dc = acc + sr.dc_stride * t;
+  float* const acc_rest = acc + sr.rest_off + sr.rest_stride * t;
+  const int nrest = 3 * (M - 1), nact = 3 * ((D + 1) * (D + 1) - 1);
+  float am[3], asc[3], aq[4], aop = -0.f, a2d[2];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) am[k] = asc[k] = -0.f;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) aq[k] = -0.f;
+  a2d[0] = a2d[1] = -0.f;
+  if (t < nv) {
+    acc_dc[0] = acc_dc[1] = acc_dc[2] = -0.f;
+    for (int k = 0; k < nrest; ++k) acc_rest[k] = -0.f;
+  }
+  for (int v = 0; v < nviews; ++v) {
+    if (v > 0) {
+      __syncthreads();                                     // view v - 1's camera and pose partials are consumed
+      const uint32_t* s = reinterpret_cast<const uint32_t*>(gv.cam + v);
+      uint32_t* d = reinterpret_cast<uint32_t*>(cam);
+      for (int k = threadIdx.x; k < (int)(sizeof(CamConst) / 4); k += blockDim.x) d[k] = s[k];
+      __syncthreads();
+    }
+    const size_t r = (size_t)v * in.P + i;
+    float pa[16];
+#pragma unroll
+    for (int k = 0; k < 16; ++k) pa[k] = 0.f;
+    GaussGrad gg;
+    gg.dm[0] = gg.dm[1] = gg.dm[2] = 0.f; gg.dsc[0] = gg.dsc[1] = gg.dsc[2] = 0.f;
+    gg.dq[0] = gg.dq[1] = gg.dq[2] = gg.dq[3] = 0.f; gg.dop = 0.f;
+    gg.dmeans2D[0] = gg.dmeans2D[1] = 0.f;
+    if (t < nv) {
+      float ds[kDaccSlots];
+#pragma unroll
+      for (int k = 0; k < kDaccSlots; ++k) ds[k] = 0.f;
+      if (gv.tiles[r] > 0) {
+        const unsigned long long* a = gv.dacc + r * kDaccSlots;
+        const float extent = gv.rec[3 * r + 2].w, inv_m = fix_inv_m(gv.dscale + v);
+        const double unit[3] = {1.0 / (double)fix_scale(5, extent, inv_m), 1.0 / (double)fix_scale(0, extent, inv_m),
+                                1.0 / (double)fix_scale(2, extent, inv_m)};
+#pragma unroll
+        for (int k = 0; k < kDaccSlots; ++k) ds[k] = fix_decode(a[k], unit[fix_exp(k) - 2]);
+      }
+      if (pose_only_layout) { ds[8] = ds[5]; ds[5] = 0.f; }
+      bool any = false;
+#pragma unroll
+      for (int k = 0; k < 9; ++k) any |= (ds[k] != 0.f);
+      bool has = false;
+      if (any && gv.tiles[r] > 0) {
+        GaussIn g;
+        read_gauss(sm, t, in.scales != nullptr, g);
+        Proj p;
+        const Mip mf = kMip ? gauss_mip(in, i) : Mip();
+        project_geometry<kMip>(*cam, g, in.cov3D ? in.cov3D + (size_t)6 * i : nullptr, p, mf);
+        if (p.visible) {
+          p.clamped = gv.clamped[r];
+          const float sx = ds[0], sy = ds[1];                // as in the single-view instance
+          ds[0] = -(p.A * sx + p.B * sy);
+          ds[1] = -(p.C * sy + p.B * sx);
+          ds[2] *= -0.5f;
+          ds[3] = -ds[3];
+          ds[4] *= -0.5f;
+          ds[5] = p.opacity > 0.f ? ds[5] / p.opacity : 0.f;
+          project_bwd<kMip, true>(*cam, g, p, row_rest, use_sh, in.cov3D != nullptr, ds, gg, acc_dc, acc_rest, pa, mf);
+          has = use_sh;
+        }
+      }
+      if (!has)
+        for (int k = 0; k < 3; ++k) acc_dc[k] = __fadd_rn(acc_dc[k], 0.f);
+      for (int k = has ? nact : 0; k < nrest; ++k) acc_rest[k] = __fadd_rn(acc_rest[k], 0.f);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) { am[k] = __fadd_rn(am[k], gg.dm[k]); asc[k] = __fadd_rn(asc[k], gg.dsc[k]); }
+#pragma unroll
+      for (int k = 0; k < 4; ++k) aq[k] = __fadd_rn(aq[k], gg.dq[k]);
+      aop = __fadd_rn(aop, gg.dop);
+      a2d[0] = __fadd_rn(a2d[0], gg.dmeans2D[0]);
+      a2d[1] = __fadd_rn(a2d[1], gg.dmeans2D[1]);
+    }
+    if (cam->pose_on) block_pose_partials(pa, s_pose, gv.pose_part + ((size_t)v * gridDim.x + blockIdx.x) * 16);
+  }
+  if (t < nv) {
+    sm[kSmXyz + 3 * t] = am[0]; sm[kSmXyz + 3 * t + 1] = am[1]; sm[kSmXyz + 3 * t + 2] = am[2];
+    sm[kSmSc + 3 * t] = asc[0]; sm[kSmSc + 3 * t + 1] = asc[1]; sm[kSmSc + 3 * t + 2] = asc[2];
+    *reinterpret_cast<float4*>(sm + kSmQ + 4 * t) = make_float4(aq[0], aq[1], aq[2], aq[3]);
+    sm[kSmOp + t] = aop;
+    if (out.dmeans2D) {
+      out.dmeans2D[3 * (size_t)i] = a2d[0];
+      out.dmeans2D[3 * (size_t)i + 1] = a2d[1];
+      out.dmeans2D[3 * (size_t)i + 2] = 0.f;
+    }
+  }
+  const bool bulk_out = store_block_grads(in, out, sm, acc, first, nv, M, use_sh, vec);
+  if (bulk_out && threadIdx.x == 0) bulk_wait_read();
+}
+
 #ifndef GSB_PBWD_MINB
 #define GSB_PBWD_MINB 4
 #endif
-template <bool kMip, bool kStats>
-__global__ void __launch_bounds__(kPT, GSB_PBWD_MINB)
-k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out, StatsPtrs stats) {
+// kViews: one CTA per Gaussian slice for a whole batch of `nviews` views (grid y = 1) -- the gradients of every view,
+// summed in view order; see views_bwd below.  The other instances take grid y = view and ignore nviews.
+template <bool kMip, bool kStats, bool kViews = false>
+__global__ void __launch_bounds__(kPT, kViews ? 3 : GSB_PBWD_MINB)
+k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out, StatsPtrs stats, const int nviews) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   CamConst* cam = reinterpret_cast<CamConst*>(smem_raw);
   float* sm = reinterpret_cast<float*>(smem_raw + ((sizeof(CamConst) + 15) / 16) * 16);
@@ -501,6 +678,10 @@ k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out
   stage_block_inputs(in, first, nv, use_sh, D, M, sm, &s_bar);
   const int t = threadIdx.x;
   const int i = first + t;
+  if constexpr (kViews) {
+    views_bwd<kMip>(in, gv, pose_only_layout, out, nviews, cam, sm, s_pose, first, nv, use_sh, vec);
+    return;
+  }
   const size_t r = (size_t)blockIdx.y * in.P + i;          // record id (grid y = view, as in k_preprocess)
   float pa[16];
 #pragma unroll
@@ -746,6 +927,8 @@ static int ensure_attrs() {
     for (auto k : {k_preprocess_bwd<false, false>, k_preprocess_bwd<true, false>, k_preprocess_bwd<false, true>,
                    k_preprocess_bwd<true, true>})
       GSB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPrepSmem));
+    for (auto k : {k_preprocess_bwd<false, false, true>, k_preprocess_bwd<true, false, true>})
+      GSB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPrepSmemViews));
     if (dev >= 0 && dev < 64) done[dev] = true;
   }
   return GSB_OK;
@@ -862,7 +1045,7 @@ extern "C" GSB_API int gsb_render_batch(const GsbCamera* cam, int32_t P, int32_t
 
 static int backward_views(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, const GsbDensifyStats* stats,
                           int V, void* geom, void* binning, int64_t R, void* image, const float* dL_dout,
-                          const GsbGrads* grads, cudaStream_t st);
+                          const GsbGrads* grads, cudaStream_t st, bool sum_views = false);
 
 extern "C" GSB_API int gsb_backward_stats(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt,
                                           const GsbDensifyStats* stats, void* geom, void* binning, int64_t R, void* image,
@@ -882,10 +1065,27 @@ extern "C" GSB_API int gsb_backward_pose_batch(const GsbCamera* cam, const GsbGa
   return backward_views(cam, &gb, filt, nullptr, V, geom, binning, R, image, dL_dout, &gr, (cudaStream_t)stream);
 }
 
-// Per-Gaussian gradients and densification statistics are single-view only (V = 1); a batch computes dL/dpose per view.
+extern "C" GSB_API int gsb_backward_batch(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, int32_t V,
+                                          const float* poses7, void* geom, void* binning, int64_t R, void* image,
+                                          const float* dL_dout, const GsbGrads* grads, float* dpose7,
+                                          gsb_stream_t stream) {
+  GSB_REQUIRE(g && poses7 && grads && dpose7, "gsb_backward_batch: null gaussians / poses / grads / dpose");
+  GSB_REQUIRE(!g->colors_precomp && !g->cov3D_precomp && !grads->dL_dcolors && !grads->dL_dcov3D,
+              "gsb_backward_batch: SH colours and scale / rotation only (no precomputed colours or covariances)");
+  GsbGaussians gb = *g;
+  gb.pose = poses7;
+  GsbGrads gr = *grads;
+  gr.dL_dpose = dpose7;
+  return backward_views(cam, &gb, filt, nullptr, V, geom, binning, R, image, dL_dout, &gr, (cudaStream_t)stream, true);
+}
+
+// dL/dpose is computed per view.  sum_views (gsb_backward_batch): the per-Gaussian gradients are those of all V views,
+// summed in view order, bit-identical to V single-view calls added in that order (k_preprocess_bwd<., false, true>).
+// Otherwise a batch (V > 1) writes no per-Gaussian gradient (gsb_backward_pose_batch).  Densification statistics are
+// single-view only.
 static int backward_views(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, const GsbDensifyStats* stats,
                           int V, void* geom, void* binning, int64_t R, void* image, const float* dL_dout,
-                          const GsbGrads* grads, cudaStream_t st) {
+                          const GsbGrads* grads, cudaStream_t st, bool sum_views) {
   int rc = batch_args(V, cam, g);
   if (rc) return rc;
   InPtrs in;
@@ -895,6 +1095,7 @@ static int backward_views(const GsbCamera* cam, const GsbGaussians* g, const Gsb
   if (rc) return rc;
   GSB_REQUIRE(geom && binning && image && dL_dout && grads, "null buffer");
   if (g->pose) GSB_REQUIRE(grads->dL_dpose != nullptr, "dL_dpose required when pose is fused");
+  GSB_REQUIRE(!stats || (V == 1 && !sum_views), "densification statistics are single-view only");
   if (stats)
     GSB_REQUIRE((stats->radii && stats->grad_accum && stats->denom && stats->max_radii2D) || g->P == 0,
                 "GsbDensifyStats: null buffer");
@@ -930,9 +1131,14 @@ static int backward_views(const GsbCamera* cam, const GsbGaussians* g, const Gsb
   sp.denom = stats ? stats->denom : nullptr; sp.max_r = stats ? stats->max_radii2D : nullptr;
   const int nb = (P + kPT - 1) / kPT;
   { ProfScope ps(GSB_K_PREPROCESS_BWD, st, g->pose ? 3 : 1);
-    auto kern = in.mip.on ? (stats ? k_preprocess_bwd<true, true> : k_preprocess_bwd<true, false>)
-                          : (stats ? k_preprocess_bwd<false, true> : k_preprocess_bwd<false, false>);
-    kern<<<dim3(nb, V), kPT, kPrepSmem, st>>>(in, gv, pose_only ? 1 : 0, out, sp);
+    if (sum_views) {
+      (in.mip.on ? k_preprocess_bwd<true, false, true> : k_preprocess_bwd<false, false, true>)
+          <<<nb, kPT, kPrepSmemViews, st>>>(in, gv, pose_only ? 1 : 0, out, sp, V);
+    } else {
+      auto kern = in.mip.on ? (stats ? k_preprocess_bwd<true, true> : k_preprocess_bwd<true, false>)
+                            : (stats ? k_preprocess_bwd<false, true> : k_preprocess_bwd<false, false>);
+      kern<<<dim3(nb, V), kPT, kPrepSmem, st>>>(in, gv, pose_only ? 1 : 0, out, sp, 1);
+    }
     if (g->pose) {
       k_pose_reduce<<<dim3(16, V), 256, 0, st>>>(gv.pose_part, nb, gv.pose_acc);
       k_pose_finalize<<<V, 32, 0, st>>>(gv.pose_acc, g->pose, grads->dL_dpose);

@@ -208,3 +208,11 @@ class Frame:
                                                  poses7.data_ptr(), self.geom.data_ptr(), self.binning.data_ptr(),
                                                  self.cap, self.image.data_ptr(), dL_dimage.data_ptr(),
                                                  dpose7.data_ptr(), _lib.stream_ptr()), "gsb_backward_pose_batch")
+
+    def backward_batch(self, cam, g, poses7, dL_dimage, grads, dpose7, filt=None) -> None:
+        """dL_dimage [views, 3, H, W] -> every per-Gaussian gradient of `grads` summed over the views in view order
+        (bit-identical to single-view backwards added in that order), and dpose7 [views, 7]."""
+        check(_lib.lib().gsb_backward_batch(ctypes.byref(cam), ctypes.byref(g), _f(filt), self.views, poses7.data_ptr(),
+                                            self.geom.data_ptr(), self.binning.data_ptr(), self.cap,
+                                            self.image.data_ptr(), dL_dimage.data_ptr(), ctypes.byref(grads),
+                                            dpose7.data_ptr(), _lib.stream_ptr()), "gsb_backward_batch")

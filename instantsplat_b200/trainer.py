@@ -15,10 +15,14 @@ training views sharded round-robin (view v -> rank v mod G); per step every rank
 its views, gradients are summed with one all-reduce over NVLink and scaled by 1/G inside the Adam
 kernel, so all replicas stay bit-identical.  An "iteration" in the reported iters/s is one VIEW
 (one reference iteration); one optimizer step consumes G views.
+
+One GPU, V views per optimizer step (`JointTrainer.step_batch(views)`, DESIGN.md section 4.10): the same semantics as
+G = V ranks, computed by one view-batched forward, loss and backward whose per-Gaussian gradients are summed over the
+views in view order, and one Adam launch with grad_scale = 1/V.
 """
 from __future__ import annotations
 
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 import torch
@@ -125,6 +129,18 @@ def adam_step_sizes(cfg, iteration: int, opt_step: int, lag: Dict[str, int]) -> 
         t = max(1, opt_step - lag.get(name, 0))
         out[name] = lr * ((1 - b2 ** t) ** 0.5 / (1 - b1 ** t))
     return out
+
+
+def batch_events(cfg, before: int, V: int) -> Dict[str, object]:
+    """What one optimizer step over V views does to the schedules, starting from `before` views consumed (step() with
+    G ranks, JointTrainer.step_batch with V views): the new iteration count; whether it crosses an SH-degree step
+    (oneupSHdegree) or a 3D-filter recompute (not within the last 100 iterations); whether Adam steps (not at or
+    after cfg.iterations).  The learning rates are those of the new iteration (adam_step_sizes).  step() writes the
+    same rules out inline (it is left as it was); keep the two alike."""
+    it = before + V
+    return dict(iteration=it, sh_up=it // cfg.sh_increase_interval > before // cfg.sh_increase_interval,
+                mip=it // cfg.mip_filter3d_interval > before // cfg.mip_filter3d_interval and it < cfg.iterations - 100,
+                do_opt=it < cfg.iterations)
 
 
 def L_sig_words():
@@ -246,6 +262,7 @@ class JointTrainer:
             self.densify_generator = torch.Generator(device=self.dev).manual_seed(int(c.densify_seed))
             self.white_background = bool((scene.bg == 1).all())
         self.densified_at, self.reset_at = [], []
+        self._batch = None            # step_batch's scratch for the view count of its last call (_batch_scratch)
 
     # ------------------------------------------------------------------------------------------
     def view(self, flat: torch.Tensor, name: str) -> torch.Tensor:
@@ -304,8 +321,8 @@ class JointTrainer:
                          self.poses[view])
 
     # ------------------------------------------------------------------------------------------
-    def _size_binning(self, R: int) -> None:
-        self.frame.alloc_binning(capacity(R, self.headroom))
+    def _size_binning(self, R: int, fr: Optional[Frame] = None) -> None:
+        (self.frame if fr is None else fr).alloc_binning(capacity(R, self.headroom))
 
     def _launch_forward(self, view: int) -> None:
         """Enqueue the forward without ever waiting for the GPU: the instance count R stays on the device; the
@@ -323,15 +340,19 @@ class JointTrainer:
         self.frame.render(cam, self.host_status[1])
         self._keep = (cam, g)
 
-    def _settle(self) -> bool:
+    def _settle(self, batch=None) -> bool:
         """Wait for the status words of the last forward's preprocess phase (early in the stream: the GPU still has
         the rest of the iteration queued, so this never starves it).  Returns True if the binning buffer was big
-        enough; otherwise grows it (the device skipped the optimizer update by itself) and returns False."""
+        enough; otherwise grows it (the device skipped the optimizer update by itself) and returns False.
+        batch: step_batch's scratch, whose frame made that forward (None: self.frame).  Each frame counts its forwards
+        in its own status words and copies them to its own pinned slot, so a serial number is only ever compared with
+        the count of the frame that wrote it."""
+        fr = self.frame if batch is None else batch.frame
+        hs = self.host_status if batch is None else batch.host_status
         if self._polling:
             # graph replay: no host-visible event inside the graph, so watch the pinned status words for this forward's
             # serial number (written by the tile scan, copied by the memcpy node right behind it)
-            want = self._fwd_count & 0x7FFFFFFF
-            hs = self.host_status
+            want = (self._fwd_count if batch is None else batch.fwd_count) & 0x7FFFFFFF
             n = 0
             while (int(hs[0, ST_SEQ]) & 0x7FFFFFFF) != want:
                 n += 1
@@ -339,17 +360,17 @@ class JointTrainer:
                     raise _lib.GsbError("graph replay: the forward's status words never arrived")
         else:
             self._ev_pre.synchronize()
-        R = read_R(self.host_status[0])
+        R = read_R(hs[0])
         self.last_R = R
-        if R > self.cap:
+        if R > fr.cap:
             self.overflows += 1
-            self._size_binning(R)
+            self._size_binning(R, fr)
             return False
-        if R > 0.85 * self.cap:                        # grow ahead of need
-            self._size_binning(R)
+        if R > 0.85 * fr.cap:                          # grow ahead of need
+            self._size_binning(R, fr)
         return True
 
-    def _settled(self, enqueue, local: bool = False) -> None:
+    def _settled(self, enqueue, local: bool = False, batch=None) -> None:
         """enqueue() launches a forward, possibly with the rest of an iteration; then wait for its instance count.  When
         the binning buffer was too small, the device has skipped the optimizer update by itself (gated on the overflow
         word, summed over the ranks in multi-GPU mode), so parameters and moments are untouched, and _settle has grown
@@ -357,7 +378,7 @@ class JointTrainer:
         ranks cannot know yet; they stop loudly.  local: only this rank's forward, which any rank may repeat."""
         for _ in range(2):
             enqueue()
-            if self._settle():
+            if self._settle(batch):
                 return
             if self.world_size > 1 and not local:
                 raise _lib.GsbError(f"rank {self.rank}: {self.last_R} instances exceeded the binning capacity; the "
@@ -441,10 +462,10 @@ class JointTrainer:
         self._advance(skip)
         self._launch_adam(grad_scale, skip)
 
-    def _launch_adam(self, grad_scale: Optional[float] = None, skip=()) -> None:
+    def _launch_adam(self, grad_scale: Optional[float] = None, skip=(), skip_ptr=None) -> None:
         gs = 1.0 / self.world_size if grad_scale is None else grad_scale
-        launch_adam([self._adam_entry(name, gs) for name in self._stepped(skip)], self.flags, skip_ptr=self._skip_ptr(),
-                    step_sizes_dev=self._step_dev)
+        launch_adam([self._adam_entry(name, gs) for name in self._stepped(skip)], self.flags,
+                    skip_ptr=self._skip_ptr() if skip_ptr is None else skip_ptr, step_sizes_dev=self._step_dev)
 
     def _skip_ptr(self):
         """Device word that makes the optimizer kernels skip the update: the forward's overflow status
@@ -609,11 +630,172 @@ class JointTrainer:
                 self._advance()        # once per iteration: a repeat after an overflow takes the same step
             enqueue = self._replay if self.use_graph and self.cap > 0 else self._enqueue_iteration
             self._settled(lambda: enqueue(view, gt, do_opt, stats))
-        # crossing a multiple of the interval (with G ranks `iteration` advances by G per step)
+        # crossing a multiple of the interval (with G ranks `iteration` advances by G per step).  The SH-degree, do_opt
+        # and 3D-filter rules of this method are also written out in batch_events (step_batch); keep the two alike.
         if self.filt is not None and self.iteration // c.mip_filter3d_interval > before // c.mip_filter3d_interval and \
                 self.iteration < c.iterations - 100:
             self.compute_filter_3D()
             self.mip_recomputed_at.append(self.iteration)
+
+    # ---- several views per optimizer step on one GPU (DESIGN.md section 4.10) ----------------------------------
+    def step_batch(self, views: Sequence[int], gts: Optional[torch.Tensor] = None) -> None:
+        """One optimizer step over the V views `views` (distinct indices into the pose table), with the semantics of
+        step() on V ranks: `iteration` advances by V, and the SH-degree, learning-rate and Mip-filter schedules fire
+        when it crosses their points; every view is rendered at its own pose row, its loss is train.py's on its target
+        (gts[k] for views[k], or the trainer's own targets when gts is None); the per-Gaussian gradients are summed in
+        the order of `views`, each view's dL/dpose lands in its row of pose_grad (the other rows are zero); one Adam
+        step with grad_scale = 1/V over the six tensors and the whole pose table (skipped at the last iteration).
+        step_batch([v]) equals step(v) bit for bit.  The per-view losses stay on the device (batch_loss_values()).
+
+        With use_graph, the captured graph is keyed on the address of the targets: pass gts=None (the trainer's own
+        targets) or the same held buffer on every call.  A fresh tensor per call (or a non-contiguous one, which is
+        copied) makes every call capture a new graph, and beyond 64 graphs the cache, step()'s graphs included, is
+        cleared."""
+        if self.world_size > 1:
+            raise _lib.GsbError("step_batch needs world_size == 1 (batches on several GPUs are not implemented)")
+        if self._stats is not None:
+            raise _lib.GsbError("step_batch does not densify: the densification statistics are single-view "
+                                "(OptimConfig.densify=True needs step())")
+        views = [int(v) for v in views]
+        V = len(views)
+        if V == 0:
+            raise ValueError("step_batch: no views")
+        if len(set(views)) != V:
+            raise ValueError(f"step_batch: duplicate views in {views} (each view owns one pose row)")
+        if any(not 0 <= v < self.n_views for v in views):
+            raise ValueError(f"step_batch: views {views} out of range 0..{self.n_views - 1}")
+        if gts is None:
+            if self.gt is None:
+                raise ValueError("step_batch: no targets (the trainer has no gt_images and gts is None)")
+            target, rows = self.gt, views
+        else:
+            dev = self.dev if self.dev.index is not None else torch.device(self.dev.type, torch.cuda.current_device())
+            if not isinstance(gts, torch.Tensor) or tuple(gts.shape) != (V, 3, self.H, self.W) or \
+                    gts.dtype != torch.float32 or gts.device != dev:
+                raise ValueError(f"step_batch: gts must be a float32 tensor of shape {(V, 3, self.H, self.W)} on {dev}, "
+                                 f"got {getattr(gts, 'dtype', type(gts))} {tuple(getattr(gts, 'shape', ()))} on "
+                                 f"{getattr(gts, 'device', None)}")
+            target, rows = gts.contiguous(), list(range(V))
+        c = self.cfg
+        b = self._batch_scratch(V)
+        # the view ids and target rows reach the (possibly captured) iteration through device memory
+        b.sel.copy_(torch.tensor([views, rows], dtype=torch.int64, pin_memory=True), non_blocking=True)
+        ev = batch_events(c, self.iteration, V)
+        self.iteration = ev["iteration"]
+        if ev["sh_up"]:
+            self.active_sh_degree = min(self.active_sh_degree + 1, c.max_sh_degree)     # oneupSHdegree
+        do_opt = ev["do_opt"]
+        if do_opt:
+            self._advance()            # once per step: a repeat after an overflow takes the same step
+        enqueue = self._replay_batch if self.use_graph and b.frame.cap > 0 else self._enqueue_batch
+        self._settled(lambda: enqueue(b, target, do_opt), batch=b)
+        b.stepped = True
+        if self.filt is not None and ev["mip"]:
+            self.compute_filter_3D()
+            self.mip_recomputed_at.append(self.iteration)
+
+    def batch_loss_values(self) -> torch.Tensor:
+        """loss_value() of each view of the last step_batch call, [V] on the device (views in the call's order)."""
+        if self._batch is None or not self._batch.stepped:
+            raise _lib.GsbError("batch_loss_values: no step_batch call since the trainer was built, resized or restored")
+        s = self._batch.sums
+        n = 3 * self.H * self.W
+        lam = self.cfg.lambda_dssim
+        return (1.0 - lam) * s[:, 0] / n + lam * (1.0 - s[:, 1] / n)
+
+    class _BatchScratch:
+        """step_batch's buffers for V views: the batch Frame with its own pinned status slot (its forwards have their own
+        serial numbers, see _settle), sel [2, V] (view ids, target rows; uploaded per call), the gathered poses and their
+        gradients [V, 7], dL/dimage, loss maps and per-view loss sums."""
+
+        def __init__(self, dev, P, W, H, V):
+            self.V = V
+            self.frame = Frame(dev, P, W, H, views=V)
+            self.frame.status.zero_()          # the forward serial number lives in these words
+            self.fwd_count = 0
+            self.stepped = False
+            self.host_status = torch.zeros(2, ST_WORDS, dtype=torch.int32).pin_memory()   # [0] preprocess, [1] render
+            self.sel = torch.zeros(2, V, dtype=torch.int64, device=dev)
+            self.rows = torch.zeros(V, dtype=torch.int32, device=dev)
+            self.poses = torch.zeros(V, 7, dtype=torch.float32, device=dev)
+            self.dpose = torch.zeros(V, 7, dtype=torch.float32, device=dev)
+            self.dL = torch.empty_like(self.frame.color)
+            self.maps = torch.empty(3, V, 3, H, W, dtype=torch.float32, device=dev)
+            self.sums = torch.zeros(V, 2, dtype=torch.float64, device=dev)
+
+    def _batch_scratch(self, V: int) -> "_BatchScratch":
+        """The scratch for V views; one set is held at a time (a call with another V replaces it, and with it the
+        graphs captured over it)."""
+        if self._batch is None or self._batch.V != V:
+            self._batch = None
+            self._graphs = {k: g for k, g in self._graphs.items() if k[0] != "batch"}
+            self._batch = self._BatchScratch(self.dev, self.P, self.W, self.H, V)
+        return self._batch
+
+    def _enqueue_batch(self, b: "_BatchScratch", target: torch.Tensor, do_opt: bool) -> None:
+        """One step_batch iteration with no wait, launched eagerly or captured into a graph: gather the pose rows,
+        forward, loss, backward summed over the views, scatter dL/dpose into pose_grad, the test hook, and (do_opt)
+        the update, gated on the batch's binning-overflow word."""
+        L = _lib.lib()
+        st = _lib.stream_ptr()
+        fr, V = b.frame, b.V
+        idx = b.sel[0]
+        b.rows.copy_(b.sel[1])
+        with torch.no_grad():          # a restored pose table may carry requires_grad from the checkpoint's Parameter
+            torch.index_select(self.poses, 0, idx, out=b.poses)
+        cam = self.ident.camera(self.active_sh_degree, 16, self.exact_cull)
+        p = self.params
+        g = gaussians(self.P, *(self.view(p, n) for n in ("xyz", "rotation", "scaling", "opacity", "f_dc", "f_rest")),
+                      b.poses)
+        fr.preprocess_batch(cam, g, b.poses, b.host_status[0], self.filt)
+        if not torch.cuda.is_current_stream_capturing():
+            b.fwd_count += 1
+            self._polling = False
+            self._ev_pre.record()
+            if fr.cap == 0:                           # very first forward: size the buffer from the real count
+                self._ev_pre.synchronize()
+                self._size_binning(read_R(b.host_status[0]), fr)
+        fr.render_batch(cam, b.host_status[1])
+        b.sums.zero_()
+        check(L.gsb_loss_forward_batch(V, 3, self.H, self.W, fr.color.data_ptr(), target.data_ptr(),
+                                       b.rows.data_ptr(), b.sums.data_ptr(), b.maps.data_ptr(), st),
+              "gsb_loss_forward_batch")
+        check(L.gsb_loss_backward_batch(V, 3, self.H, self.W, fr.color.data_ptr(), target.data_ptr(),
+                                        b.rows.data_ptr(), b.maps.data_ptr(), float(self.cfg.lambda_dssim),
+                                        b.dL.data_ptr(), st), "gsb_loss_backward_batch")
+        gr = GsbGrads()
+        gd = self.grads
+        gr.dL_dmeans3D = self.view(gd, "xyz").data_ptr()
+        gr.dL_dscales = self.view(gd, "scaling").data_ptr()
+        gr.dL_drotations = self.view(gd, "rotation").data_ptr()
+        gr.dL_dopacities = self.view(gd, "opacity").data_ptr()
+        gr.dL_dsh_dc = self.view(gd, "f_dc").data_ptr()
+        gr.dL_dsh_rest = self.view(gd, "f_rest").data_ptr()
+        fr.backward_batch(cam, g, b.poses, b.dL, gr, b.dpose, self.filt)
+        self.pose_grad.zero_()
+        with torch.no_grad():
+            self.pose_grad.index_copy_(0, idx, b.dpose)
+        if self._after_backward is not None:
+            self._after_backward()
+        if do_opt:
+            self._launch_adam(1.0 / V, skip_ptr=fr.word(ST_OVERFLOW).data_ptr())
+
+    def _replay_batch(self, b: "_BatchScratch", target: torch.Tensor, do_opt: bool) -> None:
+        """Replay (capturing on first use) the CUDA graph of _enqueue_batch: one graph per (V, target buffer, do_opt,
+        active SH degree, capacity, exact_cull) serves every choice of views (they are read from b.sel)."""
+        key = ("batch", b.V, target.data_ptr(), do_opt, self.active_sh_degree, b.frame.cap, self.exact_cull)
+        g = self._graphs.get(key)
+        if g is None:
+            if len(self._graphs) > 64:
+                self._graphs.clear()
+            torch.cuda.synchronize()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self._enqueue_batch(b, target, do_opt)
+            self._graphs[key] = g
+        b.fwd_count += 1
+        self._polling = True
+        g.replay()
 
     # ---- densify / prune / opacity reset on the flat buffers (SURVEY.md section 8 row f4) -----------------------
     # Semantics of scene/gaussian_model.py: prune_points (:359-374) keeps the surviving rows of every
@@ -644,6 +826,7 @@ class JointTrainer:
             self._stats = torch.zeros(3, new_P, dtype=torch.float32, device=self.dev) if stats is None else \
                 stats.contiguous()
         self.frame = Frame(self.dev, new_P, self.W, self.H)   # the next forward sizes its binning buffer
+        self._batch = None
         self._mip_setup()
         self._keep = None
         self._graphs.clear()
