@@ -239,7 +239,8 @@ GSB_API int gsb_track_step(float* pose7, const float* dpose7_raw, const double* 
  * bit-identical to V single-view backward calls whose outputs are added in that order -- plus dL/dpose per view.  It
  * stages each Gaussian slice once and loops over the views inside one launch; no per-view gradient copy is written.
  * gsb_loss_forward_batch / gsb_loss_backward_batch are the training loss on V images, each view's sums and dL/dimg
- * exactly those of gsb_loss_forward / gsb_loss_backward on it.  Densification statistics stay single-view. */
+ * exactly those of gsb_loss_forward / gsb_loss_backward on it.  gsb_backward_batch_stats also accumulates the
+ * densification statistics of the batch's first views; batched tracking (gsb_backward_pose_batch) takes none. */
 GSB_API size_t gsb_geom_bytes_batch(int32_t P, int32_t V, int32_t width, int32_t height);
 GSB_API size_t gsb_binning_bytes_batch(int64_t R, int32_t width, int32_t height, int32_t V);
 GSB_API size_t gsb_image_bytes_batch(int32_t width, int32_t height, int32_t V);
@@ -265,6 +266,17 @@ GSB_API int gsb_backward_pose_batch(const GsbCamera* cam, const GsbGaussians* g,
 GSB_API int gsb_backward_batch(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, int32_t V,
                                const float* poses7, void* geom, void* binning, int64_t R, void* image,
                                const float* dL_dout, const GsbGrads* grads, float* dpose7, gsb_stream_t stream);
+/* gsb_backward_batch that also accumulates the densification statistics (train.py:197-199) of views 0 .. n_stats-1,
+ * in view order: for each such view v and every Gaussian with radii[v*P + i] > 0, grad_accum += |dL/dmeans2D[:2]| of
+ * view v's own loss (not of the sum), denom += 1, max_radii2D = max(max_radii2D, radii[v*P + i]).  stats->radii is
+ * the batch's [V, P] radii (gsb_preprocess_batch); the other three are [P].  The result is bit-identical to n_stats
+ * gsb_backward_stats calls made in view order; nothing is counted when the batch's binning capacity was exceeded
+ * (status word 1).  n_stats must be in 0..V and stats non-NULL when n_stats > 0 (else GSB_ERR_INVALID);
+ * gsb_backward_batch is this with stats = NULL and n_stats = 0. */
+GSB_API int gsb_backward_batch_stats(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, int32_t V,
+                                     int32_t n_stats, const GsbDensifyStats* stats, const float* poses7, void* geom,
+                                     void* binning, int64_t R, void* image, const float* dL_dout,
+                                     const GsbGrads* grads, float* dpose7, gsb_stream_t stream);
 /* gsb_loss_forward / gsb_loss_backward on V images img [V, C, H, W]: view v's target is the [C, H, W] block
  * gt + gt_row[v] * C*H*W (gt_row: device int32 [V], so that one captured launch serves any choice of targets).
  * sums [V, 2] (double, caller zeroes), maps [3, V, C, H, W]; dL_dimg [V, C, H, W], each view scaled by 1/N with

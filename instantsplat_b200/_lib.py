@@ -79,7 +79,8 @@ EXPORTS = ("gsb_geom_bytes", "gsb_binning_bytes", "gsb_image_bytes", "gsb_prepro
            "gsb_preprocess_ex", "gsb_backward_ex", "gsb_mip_filter3d", "gsb_backward_stats",
            "gsb_geom_bytes_batch", "gsb_binning_bytes_batch", "gsb_image_bytes_batch", "gsb_status_device_batch",
            "gsb_preprocess_batch", "gsb_render_batch", "gsb_backward_pose_batch", "gsb_l1_mask_fwd_bwd_batch",
-           "gsb_track_step_batch", "gsb_backward_batch", "gsb_loss_forward_batch", "gsb_loss_backward_batch")
+           "gsb_track_step_batch", "gsb_backward_batch", "gsb_loss_forward_batch", "gsb_loss_backward_batch",
+           "gsb_backward_batch_stats")
 KERNEL_IDS = ("preprocess", "sort_depth", "scan", "duplicate", "sort_tile", "gather", "blend_fwd", "blend_bwd",
               "preprocess_bwd", "loss_fwd", "loss_bwd", "adam")
 
@@ -157,10 +158,14 @@ def lib() -> ctypes.CDLL:
     L.gsb_track_step_batch.argtypes = [i32, vp, vp, vp, vp, vp, vp, vp, i64, i32] + [ctypes.c_float] * 6 + [vp]
     L.gsb_backward_batch.argtypes = [ctypes.POINTER(GsbCamera), ctypes.POINTER(GsbGaussians), ctypes.POINTER(GsbFilter),
                                      i32, vp, vp, vp, i64, vp, vp, ctypes.POINTER(GsbGrads), vp, vp]
+    L.gsb_backward_batch_stats.argtypes = [ctypes.POINTER(GsbCamera), ctypes.POINTER(GsbGaussians),
+                                           ctypes.POINTER(GsbFilter), i32, i32, ctypes.POINTER(GsbDensifyStats), vp, vp,
+                                           vp, i64, vp, vp, ctypes.POINTER(GsbGrads), vp, vp]
     L.gsb_loss_forward_batch.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
     L.gsb_loss_backward_batch.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, ctypes.c_float, vp, vp]
     for f in ("gsb_preprocess_batch", "gsb_render_batch", "gsb_backward_pose_batch", "gsb_l1_mask_fwd_bwd_batch",
-              "gsb_track_step_batch", "gsb_backward_batch", "gsb_loss_forward_batch", "gsb_loss_backward_batch"):
+              "gsb_track_step_batch", "gsb_backward_batch", "gsb_loss_forward_batch", "gsb_loss_backward_batch",
+              "gsb_backward_batch_stats"):
         getattr(L, f).restype = ctypes.c_int
     L.gsb_adam_step_gated.argtypes = [i32, ctypes.POINTER(GsbAdamTensor), vp, vp, vp]
     L.gsb_adam_step_gated.restype = ctypes.c_int

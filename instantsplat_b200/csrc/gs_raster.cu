@@ -11,8 +11,9 @@
 //   k_blend_fwd2       (gs_blend.cu) one CTA per 16x16 tile, TMA-staged slab chunks, two pixels per lane
 //   k_blend_bwd2       (gs_blend.cu) back-to-front replay, 9 gradients per (warp, Gaussian) reduced in-warp
 //   k_preprocess_bwd   analytic backward to the model's own tensors + in-kernel pose-gradient
-//                      reduction; k_pose_finalize chains it to dL/dP[7].  <., false, true>: the gradients of a batch
-//                      of views summed in view order, inputs staged once per Gaussian slice (gsb_backward_batch)
+//                      reduction; k_pose_finalize chains it to dL/dP[7].  <., ., true>: the gradients of a batch
+//                      of views summed in view order, inputs staged once per Gaussian slice, and (<., true, true>)
+//                      the densification statistics of its first views (gsb_backward_batch_stats)
 //
 // Reference behaviour: SURVEY.md Appendix A; call site gaussian_renderer/__init__.py:60-135.
 #include <string.h>
@@ -547,11 +548,19 @@ __device__ __forceinline__ void block_pose_partials(const float* pa, float (*s_p
 // exactly its own bits) and every view adds with __fadd_rn, which is never contracted into an FMA.  A view in which
 // the Gaussian has no moments adds the +0 the single-view call writes.  SH sums live in shared memory behind the
 // staged rows (kPrepSmemViews); the others in registers.  View v's pose partials go to pose_part row (v, CTA), the
-// layout of grid y = view, so k_pose_reduce / k_pose_finalize are unchanged.  Not for densification statistics.
-template <bool kMip>
+// layout of grid y = view, so k_pose_reduce / k_pose_finalize are unchanged.
+// kStats (k_preprocess_bwd<., true, true>): the densification statistics of views 0 .. nstats-1 as well, each view
+// adding what one single-view kStats call on it adds (train.py:197-199): where radii[v * P + i] > 0, its own
+// |dL/dmeans2D[:2]|, one view and its radius.  The three running values are loaded once, kept in registers across the
+// view loop and stored once; the norm is written out as the single-view instance compiles sqrtf(dx*dx + dy*dy) (an
+// FMUL of dy, one FFMA of dx, IEEE sqrt) and added with __fadd_rn in view order, so the result is bit-identical to
+// nstats single-view calls made in view order.  Nothing is counted after a binning overflow (the caller repeats the
+// step).
+template <bool kMip, bool kStats>
 __device__ __forceinline__ void views_bwd(const InPtrs& in, const GeomView& gv, int pose_only_layout,
-                                          const OutPtrs& out, int nviews, CamConst* cam, float* sm,
-                                          float (*s_pose)[16], int first, int nv, bool use_sh, bool vec) {
+                                          const OutPtrs& out, const StatsPtrs& stats, int nviews, int nstats,
+                                          CamConst* cam, float* sm, float (*s_pose)[16], int first, int nv,
+                                          bool use_sh, bool vec) {
   const int t = threadIdx.x, i = first + t;
   const int D = cam->D, M = cam->M;
   const ShRows sr = sh_rows(in.sh_packed, M);
@@ -569,6 +578,12 @@ __device__ __forceinline__ void views_bwd(const InPtrs& in, const GeomView& gv, 
   if (t < nv) {
     acc_dc[0] = acc_dc[1] = acc_dc[2] = -0.f;
     for (int k = 0; k < nrest; ++k) acc_rest[k] = -0.f;
+  }
+  bool count = false;
+  float s_acc = 0.f, s_den = 0.f, s_max = 0.f;
+  if constexpr (kStats) {
+    count = t < nv && nstats > 0 && gv.status[kStOverflow] == 0u;
+    if (count) { s_acc = stats.accum[i]; s_den = stats.denom[i]; s_max = stats.max_r[i]; }
   }
   for (int v = 0; v < nviews; ++v) {
     if (v > 0) {
@@ -632,6 +647,17 @@ __device__ __forceinline__ void views_bwd(const InPtrs& in, const GeomView& gv, 
       aop = __fadd_rn(aop, gg.dop);
       a2d[0] = __fadd_rn(a2d[0], gg.dmeans2D[0]);
       a2d[1] = __fadd_rn(a2d[1], gg.dmeans2D[1]);
+      if constexpr (kStats) {
+        if (count && v < nstats) {
+          const int rad = stats.radii[r];
+          if (rad > 0) {
+            const float dx = gg.dmeans2D[0], dy = gg.dmeans2D[1];
+            s_acc = __fadd_rn(s_acc, __fsqrt_rn(__fmaf_rn(dx, dx, __fmul_rn(dy, dy))));
+            s_den = __fadd_rn(s_den, 1.f);
+            s_max = fmaxf(s_max, (float)rad);
+          }
+        }
+      }
     }
     if (cam->pose_on) block_pose_partials(pa, s_pose, gv.pose_part + ((size_t)v * gridDim.x + blockIdx.x) * 16);
   }
@@ -646,6 +672,9 @@ __device__ __forceinline__ void views_bwd(const InPtrs& in, const GeomView& gv, 
       out.dmeans2D[3 * (size_t)i + 2] = 0.f;
     }
   }
+  if constexpr (kStats) {
+    if (count) { stats.accum[i] = s_acc; stats.denom[i] = s_den; stats.max_r[i] = s_max; }
+  }
   const bool bulk_out = store_block_grads(in, out, sm, acc, first, nv, M, use_sh, vec);
   if (bulk_out && threadIdx.x == 0) bulk_wait_read();
 }
@@ -654,10 +683,12 @@ __device__ __forceinline__ void views_bwd(const InPtrs& in, const GeomView& gv, 
 #define GSB_PBWD_MINB 4
 #endif
 // kViews: one CTA per Gaussian slice for a whole batch of `nviews` views (grid y = 1) -- the gradients of every view,
-// summed in view order; see views_bwd below.  The other instances take grid y = view and ignore nviews.
+// summed in view order, and (kStats) the statistics of its first `nstats` views; see views_bwd above.  The other
+// instances take grid y = view and ignore nviews and nstats.
 template <bool kMip, bool kStats, bool kViews = false>
 __global__ void __launch_bounds__(kPT, kViews ? 3 : GSB_PBWD_MINB)
-k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out, StatsPtrs stats, const int nviews) {
+k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out, StatsPtrs stats, const int nviews,
+                 const int nstats) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   CamConst* cam = reinterpret_cast<CamConst*>(smem_raw);
   float* sm = reinterpret_cast<float*>(smem_raw + ((sizeof(CamConst) + 15) / 16) * 16);
@@ -679,7 +710,8 @@ k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out
   const int t = threadIdx.x;
   const int i = first + t;
   if constexpr (kViews) {
-    views_bwd<kMip>(in, gv, pose_only_layout, out, nviews, cam, sm, s_pose, first, nv, use_sh, vec);
+    views_bwd<kMip, kStats>(in, gv, pose_only_layout, out, stats, nviews, nstats, cam, sm, s_pose, first, nv, use_sh,
+                            vec);
     return;
   }
   const size_t r = (size_t)blockIdx.y * in.P + i;          // record id (grid y = view, as in k_preprocess)
@@ -927,7 +959,8 @@ static int ensure_attrs() {
     for (auto k : {k_preprocess_bwd<false, false>, k_preprocess_bwd<true, false>, k_preprocess_bwd<false, true>,
                    k_preprocess_bwd<true, true>})
       GSB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPrepSmem));
-    for (auto k : {k_preprocess_bwd<false, false, true>, k_preprocess_bwd<true, false, true>})
+    for (auto k : {k_preprocess_bwd<false, false, true>, k_preprocess_bwd<true, false, true>,
+                   k_preprocess_bwd<false, true, true>, k_preprocess_bwd<true, true, true>})
       GSB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPrepSmemViews));
     if (dev >= 0 && dev < 64) done[dev] = true;
   }
@@ -1045,7 +1078,7 @@ extern "C" GSB_API int gsb_render_batch(const GsbCamera* cam, int32_t P, int32_t
 
 static int backward_views(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, const GsbDensifyStats* stats,
                           int V, void* geom, void* binning, int64_t R, void* image, const float* dL_dout,
-                          const GsbGrads* grads, cudaStream_t st, bool sum_views = false);
+                          const GsbGrads* grads, cudaStream_t st, bool sum_views = false, int n_stats = 1);
 
 extern "C" GSB_API int gsb_backward_stats(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt,
                                           const GsbDensifyStats* stats, void* geom, void* binning, int64_t R, void* image,
@@ -1065,10 +1098,13 @@ extern "C" GSB_API int gsb_backward_pose_batch(const GsbCamera* cam, const GsbGa
   return backward_views(cam, &gb, filt, nullptr, V, geom, binning, R, image, dL_dout, &gr, (cudaStream_t)stream);
 }
 
-extern "C" GSB_API int gsb_backward_batch(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, int32_t V,
-                                          const float* poses7, void* geom, void* binning, int64_t R, void* image,
-                                          const float* dL_dout, const GsbGrads* grads, float* dpose7,
-                                          gsb_stream_t stream) {
+extern "C" GSB_API int gsb_backward_batch_stats(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt,
+                                                int32_t V, int32_t n_stats, const GsbDensifyStats* stats,
+                                                const float* poses7, void* geom, void* binning, int64_t R, void* image,
+                                                const float* dL_dout, const GsbGrads* grads, float* dpose7,
+                                                gsb_stream_t stream) {
+  GSB_REQUIRE(n_stats >= 0 && n_stats <= V, "gsb_backward_batch_stats: n_stats must be in 0..V");
+  GSB_REQUIRE(stats || n_stats == 0, "gsb_backward_batch_stats: n_stats > 0 needs statistics");
   GSB_REQUIRE(g && poses7 && grads && dpose7, "gsb_backward_batch: null gaussians / poses / grads / dpose");
   GSB_REQUIRE(!g->colors_precomp && !g->cov3D_precomp && !grads->dL_dcolors && !grads->dL_dcov3D,
               "gsb_backward_batch: SH colours and scale / rotation only (no precomputed colours or covariances)");
@@ -1076,16 +1112,26 @@ extern "C" GSB_API int gsb_backward_batch(const GsbCamera* cam, const GsbGaussia
   gb.pose = poses7;
   GsbGrads gr = *grads;
   gr.dL_dpose = dpose7;
-  return backward_views(cam, &gb, filt, nullptr, V, geom, binning, R, image, dL_dout, &gr, (cudaStream_t)stream, true);
+  return backward_views(cam, &gb, filt, stats, V, geom, binning, R, image, dL_dout, &gr, (cudaStream_t)stream, true,
+                        n_stats);
 }
 
-// dL/dpose is computed per view.  sum_views (gsb_backward_batch): the per-Gaussian gradients are those of all V views,
-// summed in view order, bit-identical to V single-view calls added in that order (k_preprocess_bwd<., false, true>).
-// Otherwise a batch (V > 1) writes no per-Gaussian gradient (gsb_backward_pose_batch).  Densification statistics are
-// single-view only.
+extern "C" GSB_API int gsb_backward_batch(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, int32_t V,
+                                          const float* poses7, void* geom, void* binning, int64_t R, void* image,
+                                          const float* dL_dout, const GsbGrads* grads, float* dpose7,
+                                          gsb_stream_t stream) {
+  return gsb_backward_batch_stats(cam, g, filt, V, 0, nullptr, poses7, geom, binning, R, image, dL_dout, grads, dpose7,
+                                  stream);
+}
+
+// dL/dpose is computed per view.  sum_views (gsb_backward_batch_stats): the per-Gaussian gradients are those of all V
+// views, summed in view order, bit-identical to V single-view calls added in that order (k_preprocess_bwd<., ., true>),
+// and with stats the densification statistics of views 0 .. n_stats-1 (stats->radii: the batch's [V, P] radii).
+// Otherwise a batch (V > 1) writes no per-Gaussian gradient and takes no statistics (gsb_backward_pose_batch), and a
+// single view counts its statistics when stats is given.
 static int backward_views(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, const GsbDensifyStats* stats,
                           int V, void* geom, void* binning, int64_t R, void* image, const float* dL_dout,
-                          const GsbGrads* grads, cudaStream_t st, bool sum_views) {
+                          const GsbGrads* grads, cudaStream_t st, bool sum_views, int n_stats) {
   int rc = batch_args(V, cam, g);
   if (rc) return rc;
   InPtrs in;
@@ -1095,7 +1141,7 @@ static int backward_views(const GsbCamera* cam, const GsbGaussians* g, const Gsb
   if (rc) return rc;
   GSB_REQUIRE(geom && binning && image && dL_dout && grads, "null buffer");
   if (g->pose) GSB_REQUIRE(grads->dL_dpose != nullptr, "dL_dpose required when pose is fused");
-  GSB_REQUIRE(!stats || (V == 1 && !sum_views), "densification statistics are single-view only");
+  GSB_REQUIRE(!stats || V == 1 || sum_views, "densification statistics of a batch need the view-summing backward");
   if (stats)
     GSB_REQUIRE((stats->radii && stats->grad_accum && stats->denom && stats->max_radii2D) || g->P == 0,
                 "GsbDensifyStats: null buffer");
@@ -1132,12 +1178,14 @@ static int backward_views(const GsbCamera* cam, const GsbGaussians* g, const Gsb
   const int nb = (P + kPT - 1) / kPT;
   { ProfScope ps(GSB_K_PREPROCESS_BWD, st, g->pose ? 3 : 1);
     if (sum_views) {
-      (in.mip.on ? k_preprocess_bwd<true, false, true> : k_preprocess_bwd<false, false, true>)
-          <<<nb, kPT, kPrepSmemViews, st>>>(in, gv, pose_only ? 1 : 0, out, sp, V);
+      const bool count = stats && n_stats > 0;
+      auto kern = in.mip.on ? (count ? k_preprocess_bwd<true, true, true> : k_preprocess_bwd<true, false, true>)
+                            : (count ? k_preprocess_bwd<false, true, true> : k_preprocess_bwd<false, false, true>);
+      kern<<<nb, kPT, kPrepSmemViews, st>>>(in, gv, pose_only ? 1 : 0, out, sp, V, count ? n_stats : 0);
     } else {
       auto kern = in.mip.on ? (stats ? k_preprocess_bwd<true, true> : k_preprocess_bwd<true, false>)
                             : (stats ? k_preprocess_bwd<false, true> : k_preprocess_bwd<false, false>);
-      kern<<<dim3(nb, V), kPT, kPrepSmem, st>>>(in, gv, pose_only ? 1 : 0, out, sp, 1);
+      kern<<<dim3(nb, V), kPT, kPrepSmem, st>>>(in, gv, pose_only ? 1 : 0, out, sp, 1, 0);
     }
     if (g->pose) {
       k_pose_reduce<<<dim3(16, V), 256, 0, st>>>(gv.pose_part, nb, gv.pose_acc);

@@ -209,10 +209,13 @@ class Frame:
                                                  self.cap, self.image.data_ptr(), dL_dimage.data_ptr(),
                                                  dpose7.data_ptr(), _lib.stream_ptr()), "gsb_backward_pose_batch")
 
-    def backward_batch(self, cam, g, poses7, dL_dimage, grads, dpose7, filt=None) -> None:
+    def backward_batch(self, cam, g, poses7, dL_dimage, grads, dpose7, filt=None, stats=None, n_stats=0) -> None:
         """dL_dimage [views, 3, H, W] -> every per-Gaussian gradient of `grads` summed over the views in view order
-        (bit-identical to single-view backwards added in that order), and dpose7 [views, 7]."""
-        check(_lib.lib().gsb_backward_batch(ctypes.byref(cam), ctypes.byref(g), _f(filt), self.views, poses7.data_ptr(),
-                                            self.geom.data_ptr(), self.binning.data_ptr(), self.cap,
-                                            self.image.data_ptr(), dL_dimage.data_ptr(), ctypes.byref(grads),
-                                            dpose7.data_ptr(), _lib.stream_ptr()), "gsb_backward_batch")
+        (bit-identical to single-view backwards added in that order), and dpose7 [views, 7].  stats: densify_stats(...)
+        over this frame's [views, P] radii, or None; the same launch accumulates the statistics of views 0..n_stats-1,
+        bit-identical to single-view backwards with statistics made in view order."""
+        check(_lib.lib().gsb_backward_batch_stats(ctypes.byref(cam), ctypes.byref(g), _f(filt), self.views, int(n_stats),
+                                                  None if stats is None else ctypes.byref(stats), poses7.data_ptr(),
+                                                  self.geom.data_ptr(), self.binning.data_ptr(), self.cap,
+                                                  self.image.data_ptr(), dL_dimage.data_ptr(), ctypes.byref(grads),
+                                                  dpose7.data_ptr(), _lib.stream_ptr()), "gsb_backward_batch_stats")

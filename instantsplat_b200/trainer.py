@@ -95,6 +95,10 @@ class OptimConfig:
     densify_clone_split = False
     scene_extent = None
     densify_seed = 0                 # seed of the generator the split samples are drawn from
+    # step_batch with densify (DESIGN.md section 4.10): the statistics of every view of a batch, and the densify / reset
+    # events of the iterations a batch covers fired once at its end.  Off: step_batch refuses densify=True, so that a
+    # run configured for train.py's per-iteration schedule does not move its events by switching to step_batch.
+    densify_batches = False
 
 
 def lr_schedules(args, spatial_lr_scale):
@@ -141,6 +145,28 @@ def batch_events(cfg, before: int, V: int) -> Dict[str, object]:
     return dict(iteration=it, sh_up=it // cfg.sh_increase_interval > before // cfg.sh_increase_interval,
                 mip=it // cfg.mip_filter3d_interval > before // cfg.mip_filter3d_interval and it < cfg.iterations - 100,
                 do_opt=it < cfg.iterations)
+
+
+def batch_densify_events(cfg, before: int, V: int, white_background: bool) -> Dict[str, object]:
+    """The densification schedule of one optimizer step over V views starting from `before` views consumed
+    (JointTrainer.step_batch with densify): view k of the batch stands for iteration before + 1 + k.
+      n_stats: how many leading views count their statistics (those whose iteration is < densify_until_iter);
+      densify: some covered iteration j is a densify point of step() (densify_from_iter < j < densify_until_iter,
+               j % densification_interval == 0);
+      reset: some covered j < densify_until_iter is an opacity reset (j % opacity_reset_interval == 0, or a white
+             background and j == densify_from_iter);
+      size_threshold: the screen-size limit of the densify, that of the last densify point covered (cfg.size_threshold
+             when it is past opacity_reset_interval, else None); None without a densify.
+    Each event fires at most once per step.  With V = 1 these are the rules step() writes out inline; keep them alike."""
+    its = range(before + 1, before + V + 1)
+    dens = [j for j in its if cfg.densify_from_iter < j < cfg.densify_until_iter and j % cfg.densification_interval == 0]
+    reset = any(j < cfg.densify_until_iter and (j % cfg.opacity_reset_interval == 0 or
+                                                (white_background and j == cfg.densify_from_iter)) for j in its)
+    size = None
+    if dens and dens[-1] > cfg.opacity_reset_interval:
+        size = cfg.size_threshold
+    return dict(n_stats=min(max(cfg.densify_until_iter - 1 - before, 0), V), densify=bool(dens), reset=reset,
+                size_threshold=size)
 
 
 def L_sig_words():
@@ -263,6 +289,7 @@ class JointTrainer:
             self.white_background = bool((scene.bg == 1).all())
         self.densified_at, self.reset_at = [], []
         self._batch = None            # step_batch's scratch for the view count of its last call (_batch_scratch)
+        self._batch_sums = None       # per-view loss sums of the last step_batch (batch_loss_values)
 
     # ------------------------------------------------------------------------------------------
     def view(self, flat: torch.Tensor, name: str) -> torch.Tensor:
@@ -647,15 +674,20 @@ class JointTrainer:
         step with grad_scale = 1/V over the six tensors and the whole pose table (skipped at the last iteration).
         step_batch([v]) equals step(v) bit for bit.  The per-view losses stay on the device (batch_loss_values()).
 
+        With OptimConfig.densify, cfg.densify_batches must be set: each view whose iteration is below densify_until_iter
+        adds its own statistics (batch_densify_events), and the densify / opacity-reset events of the iterations the
+        step covers run once, after the step's backward and before its Adam step, eagerly.  step_batch([v]) then still
+        equals step(v) bit for bit.
+
         With use_graph, the captured graph is keyed on the address of the targets: pass gts=None (the trainer's own
         targets) or the same held buffer on every call.  A fresh tensor per call (or a non-contiguous one, which is
         copied) makes every call capture a new graph, and beyond 64 graphs the cache, step()'s graphs included, is
         cleared."""
         if self.world_size > 1:
             raise _lib.GsbError("step_batch needs world_size == 1 (batches on several GPUs are not implemented)")
-        if self._stats is not None:
-            raise _lib.GsbError("step_batch does not densify: the densification statistics are single-view "
-                                "(OptimConfig.densify=True needs step())")
+        if self._stats is not None and not self.cfg.densify_batches:
+            raise _lib.GsbError("step_batch with OptimConfig.densify=True needs OptimConfig.densify_batches=True: it "
+                                "moves the densify and opacity-reset events to batch boundaries (or use step())")
         views = [int(v) for v in views]
         V = len(views)
         if V == 0:
@@ -680,25 +712,48 @@ class JointTrainer:
         b = self._batch_scratch(V)
         # the view ids and target rows reach the (possibly captured) iteration through device memory
         b.sel.copy_(torch.tensor([views, rows], dtype=torch.int64, pin_memory=True), non_blocking=True)
+        de = dict(n_stats=0, densify=False, reset=False, size_threshold=None)
+        if self._stats is not None:
+            de = batch_densify_events(c, self.iteration, V, self.white_background)
+        n_stats = de["n_stats"]
         ev = batch_events(c, self.iteration, V)
         self.iteration = ev["iteration"]
         if ev["sh_up"]:
             self.active_sh_degree = min(self.active_sh_degree + 1, c.max_sh_degree)     # oneupSHdegree
         do_opt = ev["do_opt"]
-        if do_opt:
-            self._advance()            # once per step: a repeat after an overflow takes the same step
-        enqueue = self._replay_batch if self.use_graph and b.frame.cap > 0 else self._enqueue_batch
-        self._settled(lambda: enqueue(b, target, do_opt), batch=b)
-        b.stepped = True
+        if de["densify"] or de["reset"]:
+            # as in step(): densify / reset between the backward and the optimizer step, eagerly; the replaced tensors
+            # take no step.  densify_and_prune rebuilds the buffers and drops the batch scratch (b stays alive here).
+            self._settled(lambda: self._enqueue_batch(b, target, False, n_stats), batch=b)
+            skip = set()
+            if de["densify"]:
+                self.densify_and_prune(c.densify_grad_threshold, c.min_opacity, self.scene_extent, de["size_threshold"],
+                                       c.densify_clone_split, self.densify_generator)
+                self.densified_at.append(self.iteration)
+                skip.update(name for name, _ in SEGMENTS)
+            if de["reset"]:
+                self.reset_opacity()
+                self.reset_at.append(self.iteration)
+                skip.add("opacity")
+            if do_opt:
+                skip = [name for name, _ in SEGMENTS if name in skip]
+                self._advance(skip)
+                self._launch_adam(1.0 / V, skip, skip_ptr=b.frame.word(ST_OVERFLOW).data_ptr())
+        else:
+            if do_opt:
+                self._advance()        # once per step: a repeat after an overflow takes the same step
+            enqueue = self._replay_batch if self.use_graph and b.frame.cap > 0 else self._enqueue_batch
+            self._settled(lambda: enqueue(b, target, do_opt, n_stats), batch=b)
+        self._batch_sums = b.sums
         if self.filt is not None and ev["mip"]:
             self.compute_filter_3D()
             self.mip_recomputed_at.append(self.iteration)
 
     def batch_loss_values(self) -> torch.Tensor:
         """loss_value() of each view of the last step_batch call, [V] on the device (views in the call's order)."""
-        if self._batch is None or not self._batch.stepped:
+        if self._batch_sums is None:
             raise _lib.GsbError("batch_loss_values: no step_batch call since the trainer was built, resized or restored")
-        s = self._batch.sums
+        s = self._batch_sums
         n = 3 * self.H * self.W
         lam = self.cfg.lambda_dssim
         return (1.0 - lam) * s[:, 0] / n + lam * (1.0 - s[:, 1] / n)
@@ -713,7 +768,6 @@ class JointTrainer:
             self.frame = Frame(dev, P, W, H, views=V)
             self.frame.status.zero_()          # the forward serial number lives in these words
             self.fwd_count = 0
-            self.stepped = False
             self.host_status = torch.zeros(2, ST_WORDS, dtype=torch.int32).pin_memory()   # [0] preprocess, [1] render
             self.sel = torch.zeros(2, V, dtype=torch.int64, device=dev)
             self.rows = torch.zeros(V, dtype=torch.int32, device=dev)
@@ -732,10 +786,11 @@ class JointTrainer:
             self._batch = self._BatchScratch(self.dev, self.P, self.W, self.H, V)
         return self._batch
 
-    def _enqueue_batch(self, b: "_BatchScratch", target: torch.Tensor, do_opt: bool) -> None:
+    def _enqueue_batch(self, b: "_BatchScratch", target: torch.Tensor, do_opt: bool, n_stats: int = 0) -> None:
         """One step_batch iteration with no wait, launched eagerly or captured into a graph: gather the pose rows,
-        forward, loss, backward summed over the views, scatter dL/dpose into pose_grad, the test hook, and (do_opt)
-        the update, gated on the batch's binning-overflow word."""
+        forward, loss, backward summed over the views (and the densification statistics of views 0..n_stats-1),
+        scatter dL/dpose into pose_grad, the test hook, and (do_opt) the update, gated on the batch's binning-overflow
+        word."""
         L = _lib.lib()
         st = _lib.stream_ptr()
         fr, V = b.frame, b.V
@@ -771,7 +826,10 @@ class JointTrainer:
         gr.dL_dopacities = self.view(gd, "opacity").data_ptr()
         gr.dL_dsh_dc = self.view(gd, "f_dc").data_ptr()
         gr.dL_dsh_rest = self.view(gd, "f_rest").data_ptr()
-        fr.backward_batch(cam, g, b.poses, b.dL, gr, b.dpose, self.filt)
+        st = None
+        if n_stats > 0:
+            st = densify_stats(fr.radii, self._stats[0], self._stats[1], self._stats[2])
+        fr.backward_batch(cam, g, b.poses, b.dL, gr, b.dpose, self.filt, st, n_stats)
         self.pose_grad.zero_()
         with torch.no_grad():
             self.pose_grad.index_copy_(0, idx, b.dpose)
@@ -780,10 +838,10 @@ class JointTrainer:
         if do_opt:
             self._launch_adam(1.0 / V, skip_ptr=fr.word(ST_OVERFLOW).data_ptr())
 
-    def _replay_batch(self, b: "_BatchScratch", target: torch.Tensor, do_opt: bool) -> None:
+    def _replay_batch(self, b: "_BatchScratch", target: torch.Tensor, do_opt: bool, n_stats: int = 0) -> None:
         """Replay (capturing on first use) the CUDA graph of _enqueue_batch: one graph per (V, target buffer, do_opt,
-        active SH degree, capacity, exact_cull) serves every choice of views (they are read from b.sel)."""
-        key = ("batch", b.V, target.data_ptr(), do_opt, self.active_sh_degree, b.frame.cap, self.exact_cull)
+        active SH degree, capacity, exact_cull, n_stats) serves every choice of views (they are read from b.sel)."""
+        key = ("batch", b.V, target.data_ptr(), do_opt, self.active_sh_degree, b.frame.cap, self.exact_cull, n_stats)
         g = self._graphs.get(key)
         if g is None:
             if len(self._graphs) > 64:
@@ -791,7 +849,7 @@ class JointTrainer:
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                self._enqueue_batch(b, target, do_opt)
+                self._enqueue_batch(b, target, do_opt, n_stats)
             self._graphs[key] = g
         b.fwd_count += 1
         self._polling = True
@@ -827,6 +885,7 @@ class JointTrainer:
                 stats.contiguous()
         self.frame = Frame(self.dev, new_P, self.W, self.H)   # the next forward sizes its binning buffer
         self._batch = None
+        self._batch_sums = None
         self._mip_setup()
         self._keep = None
         self._graphs.clear()
