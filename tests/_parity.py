@@ -16,7 +16,8 @@ Protocol (BASELINE.json north_star: render <= 1e-4 max abs per pixel, gradients 
    (deep in a list, behind low transmittance, seen through an edge tile).  The oracle computes the truth in fp64, so
    the per-row metric does not measure the oracle's own fp32 rounding.
 4. Every forward's tile lists are checked exactly on all tiles (tests/_binning.py `check_lists`), not only on the
-   compared ones.
+   compared ones, and its per-pixel state on the compared, unflagged pixels: final_T within IMG_TOL of the oracle's,
+   and the last contributor (n_contrib) exactly.
 5. Every case appends its numbers to a report that conftest.py writes at the end of the session.
 """
 import math
@@ -26,6 +27,7 @@ import torch
 from oracle import gs_oracle as O
 
 import _binning as BL
+import _blend as BD
 
 DEV = "cuda"
 NAMES = ("xyz", "rotation", "scaling", "opacity", "f_dc", "f_rest")
@@ -150,7 +152,8 @@ def compare_fused(name, sc, view, deg, bg, gt=None, tiles=None, names=None, reco
     m2c = torch.zeros(sc.P, 3, device=DEV, requires_grad=True)
     img_c, radii_c = I.rasterize_fused(pc["xyz"], pc["rotation"], pc["scaling"], pc["opacity"], pc["f_dc"],
                                        pc["f_rest"], pose_c, m2c, settings_for(sc, deg, bg))
-    lists = BL.check_lists(BL.decode(img_c.grad_fn.st))
+    lists_c = BL.decode(img_c.grad_fn.st)
+    lists = BL.check_lists(lists_c)
     mask = None
     if tiles is not None:
         gx = (sc.width + 15) // 16
@@ -164,6 +167,14 @@ def compare_fused(name, sc, view, deg, bg, gt=None, tiles=None, names=None, reco
                tiles_compared=(len(tiles) if tiles is not None else ((sc.width + 15) // 16) * ((sc.height + 15) // 16)),
                **st)
     rec["lists"] = lists
+    # per-pixel state of the forward: final_T, and n_contrib as the id of the last contributor (the kernel's culled
+    # lists and the oracle's rect lists number their entries differently)
+    ft_c, nc_c = BD.decode_image(img_c.grad_fn.st)
+    sel = ~amb if mask is None else mask & ~amb
+    last_c = BD.last_contributor(lists_c["ids"].cpu(), lists_c["ranges"].cpu(), nc_c, sc.width)
+    last_o = BD.last_contributor(aux["gids"], aux["ranges"], aux["n_contrib"], sc.width)
+    rec["final_T_max_abs_err"] = float((ft_c.double() - aux["final_T"].double()).abs()[sel].max())
+    rec["n_contrib_mismatch"] = int((last_c != last_o)[sel].sum())
     rec["radii_mismatch_frac"] = float((radii_c.cpu() != radii_o).float().mean())
     # ---- weights
     if gt is not None:
@@ -208,6 +219,8 @@ def compare_fused(name, sc, view, deg, bg, gt=None, tiles=None, names=None, reco
     if record:
         REPORT.append(rec)
     assert_image(st, name)
+    assert rec["final_T_max_abs_err"] <= IMG_TOL, f"{name}: final_T differs from the oracle's: {rec}"
+    assert rec["n_contrib_mismatch"] == 0, f"{name}: the last contributor differs on {rec['n_contrib_mismatch']} pixels"
     assert rec["radii_mismatch_frac"] < 2e-3, rec
     bad = {k: v for k, v in ge.items() if not v < GRAD_TOL}
     assert not bad, f"{name}: gradient relative errors over {GRAD_TOL}: {bad} (all: {ge})"
