@@ -296,6 +296,22 @@ GSB_API int gsb_track_step_batch(int32_t V, float* pose7, const float* dpose7_ra
                                  float lr_q, float lr_T, float beta1, float beta2, float eps, float weight_decay,
                                  gsb_stream_t stream);
 
+/* ---- evaluation metrics (train.py:256-290 training_report, metrics.py:55-84) ----
+ * img [V, C, H, W]; view v is compared with block gt_row[v] of gt (gt + gt_row[v] * C*H*W, gt_row: device int32 [V]).
+ * mode: GSB_METRIC_CLAMP (both clamped to [0,1], train.py training_report) or GSB_METRIC_PNG8 (both through
+ * save_image's 8-bit quantisation uint8(clamp(x*255 + 0.5, 0, 255)) and to_tensor's /255, render.py -> metrics.py).
+ * out [V, 2 + C] doubles: sum|a-b|, sum of the SSIM map (the training loss's SSIM), per-channel sum (a-b)^2.
+ * Every CTA writes its partial sums to scratch (at least gsb_image_metrics_scratch_bytes(V, C, H, W) bytes) and a
+ * second kernel adds each view's partials in a fixed order: no atomics, and view v's result is bit-identical across
+ * runs, whatever V is and whichever views share the batch.  V * C must not exceed 65535; an unknown mode or a short
+ * scratch is GSB_ERR_INVALID. */
+#define GSB_METRIC_CLAMP 1
+#define GSB_METRIC_PNG8 2
+GSB_API size_t gsb_image_metrics_scratch_bytes(int32_t V, int32_t C, int32_t H, int32_t W);
+GSB_API int gsb_image_metrics_batch(int32_t V, int32_t C, int32_t H, int32_t W, const float* img, const float* gt,
+                                    const int32_t* gt_row, int32_t mode, double* out, void* scratch,
+                                    size_t scratch_bytes, gsb_stream_t stream);
+
 /* Per-point Adam (scene/per_point_adam.py:34-98), n tensors in one launch. */
 typedef struct GsbAdamTensor {
   float* param;

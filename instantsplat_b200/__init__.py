@@ -18,3 +18,4 @@ from .trainer import CHECKPOINT_KEY, JointTrainer, OptimConfig, read_checkpoint 
 from .model import GaussianModel, PipelineDefaults, SimpleGaussianModel, optimization_defaults  # noqa: F401
 from .knn import distCUDA2  # noqa: F401
 from .densify import cameras_extent, densify_plan  # noqa: F401
+from .evaluation import image_metrics  # noqa: F401

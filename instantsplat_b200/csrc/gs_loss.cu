@@ -11,6 +11,9 @@
 // per thread horizontally from 128-bit shared loads, 2 outputs per thread vertically), so HBM
 // traffic is the compulsory read of the two images plus the three partial-derivative maps written
 // for the backward.
+//
+// The evaluation metrics (gsb_image_metrics_batch: train.py's training_report, metrics.py) are the same forward on
+// clamped or 8-bit-quantised inputs, with per-CTA partial sums and a fixed-order reduction instead of atomics.
 #include <cuda_runtime.h>
 #include <stdio.h>
 
@@ -66,12 +69,29 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
   return r;   // valid in thread 0
 }
 
+// What the forward compares: the pixel values as they are (the training loss), clamped to [0, 1] (train.py's
+// training_report), or through torchvision's save_image and to_tensor (render.py -> metrics.py):
+// uint8(clamp(x * 255 + 0.5, 0, 255)) / 255 in fp32, truncating, so exact ties round up.
+enum { kInRaw = 0, kInClamp = GSB_METRIC_CLAMP, kInPng8 = GSB_METRIC_PNG8 };
+
+template <int kIn>
+__device__ __forceinline__ float metric_input(float x) {
+  if constexpr (kIn == kInClamp) return fminf(fmaxf(x, 0.f), 1.f);
+  if constexpr (kIn == kInPng8) {
+    const float q = truncf(fminf(fmaxf(__fadd_rn(__fmul_rn(x, 255.f), 0.5f), 0.f), 255.f));
+    return __fdiv_rn(q, 255.f);
+  }
+  return x;
+}
+
 // Stage the (TH+10) x (TW+10) halo of TWO planes into shared memory as interleaved float2 {a, b} (zero 'same'
 // padding): one warp per row, lanes along x (two coalesced accesses per row and plane).  Fully unrolled with all
-// global loads issued before the first shared store, so a lane has 16 loads in flight.
+// global loads issued before the first shared store, so a lane has 16 loads in flight.  kIn: metric_input applied to
+// every loaded pixel (the padding stays zero).
 constexpr int kRowsPerWarp = (EH + 7) / 8;   // 4
 struct HaloRegs { float a[kRowsPerWarp], b[kRowsPerWarp]; };
 
+template <int kIn = kInRaw>
 __device__ __forceinline__ void halo_load(HaloRegs& h, const float* __restrict__ src, int H, int W, int x0, int y0) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int xa = x0 - HALO + lane, xb = xa + 32;
@@ -83,8 +103,8 @@ __device__ __forceinline__ void halo_load(HaloRegs& h, const float* __restrict__
     const int y = y0 + r - HALO;
     const bool yin = r < EH && y >= 0 && y < H;
     const float* row = src + (size_t)(yin ? y : 0) * W;
-    h.a[i] = (yin && xa_in) ? __ldg(row + xa) : 0.f;
-    h.b[i] = (yin && xb_in) ? __ldg(row + xb) : 0.f;
+    h.a[i] = (yin && xa_in) ? metric_input<kIn>(__ldg(row + xa)) : 0.f;
+    h.b[i] = (yin && xb_in) ? metric_input<kIn>(__ldg(row + xb)) : 0.f;
   }
 }
 // dst[r][x] = {p.(x), q.(x)}
@@ -119,11 +139,15 @@ __device__ __forceinline__ float2 bcast(float w) { return make_float2(w, w); }
 // kViews: a batch of views of C planes each (BC = V * C): plane z = v * C + c of img1 is compared with plane
 // gt_row[v] * C + c of img2, and view v's sums go to sums[2v], sums[2v + 1].  Every plane keeps the single-view CTA
 // split, so each view's partials are those of the single-view call.
-template <bool kViews = false>
+// kIn != kInRaw (evaluation metrics, needs kViews): both planes go through metric_input<kIn>, and instead of adding
+// to `sums` with atomics every CTA writes its own {sum|a-b|, sum ssim, sum (a-b)^2} (CTA sums in fp32, as above) to
+// sums[3 * cta], cta = (bc * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x; k_metrics_reduce adds them up.
+template <bool kViews = false, int kIn = kInRaw>
 __global__ void __launch_bounds__(256, 4)
 k_ssim_fwd(int H, int W, const float* __restrict__ img1, const float* __restrict__ img2,
            double* __restrict__ sums, float* __restrict__ maps, size_t plane_total, int do_l1, int C = 1,
            const int32_t* __restrict__ gt_row = nullptr) {
+  static_assert(kIn == kInRaw || kViews, "the metric forward is the view-batched one");
   __shared__ __align__(16) float2 sAB[EH][EWP];
   __shared__ __align__(16) float2 sH1[EH][HS];     // {E_h[a], E_h[b]}
   __shared__ __align__(16) float2 sH2[EH][HS];     // {E_h[a^2], E_h[b^2]}
@@ -135,12 +159,13 @@ k_ssim_fwd(int H, int W, const float* __restrict__ img1, const float* __restrict
   if constexpr (kViews) {
     const int v = bc / C;
     gt_plane = (size_t)__ldg(gt_row + v) * C + (bc - v * C);
-    sums += 2 * v;
+    if constexpr (kIn == kInRaw) sums += 2 * v;
+    else sums += 3 * (((size_t)bc * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x);
   }
   {
     HaloRegs ha, hb;
-    halo_load(ha, img1 + (size_t)bc * H * W, H, W, x0, y0);
-    halo_load(hb, img2 + gt_plane * H * W, H, W, x0, y0);
+    halo_load<kIn>(ha, img1 + (size_t)bc * H * W, H, W, x0, y0);
+    halo_load<kIn>(hb, img2 + gt_plane * H * W, H, W, x0, y0);
     halo_store2(ha, hb, sAB);
   }
   __syncthreads();
@@ -195,7 +220,7 @@ k_ssim_fwd(int H, int W, const float* __restrict__ img1, const float* __restrict
       }
     }
   }
-  float ssim_v = 0.f, l1_v = 0.f;
+  float ssim_v = 0.f, l1_v = 0.f, sq_v = 0.f;
 #pragma unroll
   for (int o = 0; o < 2; ++o) {
     const int x = x0 + tx, y = y0 + ty + o;
@@ -214,7 +239,21 @@ k_ssim_fwd(int H, int W, const float* __restrict__ img1, const float* __restrict
         maps[2 * plane_total + off] = 2.f * A1 * inv;                             // d/dE[xy]
       }
       if (do_l1) { const float2 c = sAB[ty + o + HALO][tx + HALO]; l1_v += fabsf(c.x - c.y); }
+      if constexpr (kIn != kInRaw) {
+        const float2 c = sAB[ty + o + HALO][tx + HALO];
+        const float d = c.x - c.y;
+        sq_v = fmaf(d, d, sq_v);
+      }
     }
+  }
+  if constexpr (kIn != kInRaw) {
+    const float s = block_sum(ssim_v, red);
+    __syncthreads();
+    const float l = block_sum(l1_v, red);
+    __syncthreads();
+    const float q = block_sum(sq_v, red);
+    if (threadIdx.x == 0) { sums[0] = (double)l; sums[1] = (double)s; sums[2] = (double)q; }
+    return;
   }
   float s = block_sum(ssim_v, red);
   if (threadIdx.x == 0) atomicAdd(sums + 1, (double)s);
@@ -325,6 +364,33 @@ k_ssim_bwd(int H, int W, const float* __restrict__ img1, const float* __restrict
   }
 }
 
+// One CTA per view: out[v] = {sum|a-b|, sum ssim, sum (a-b)^2 of each channel} from the view's C * T CTA partials
+// (T tiles per plane, laid out as k_ssim_fwd<true, kIn> writes them).  Every sum is taken in fp64 in one fixed order
+// (thread t adds items t, t + 256, ...; then a fixed tree), so a view's result depends on its own partials only.
+constexpr int kReduceThreads = 256;
+__global__ void __launch_bounds__(kReduceThreads)
+k_metrics_reduce(int C, int T, const double* __restrict__ partials, double* __restrict__ out) {
+  __shared__ double red[kReduceThreads];
+  const int v = blockIdx.x;
+  const double* p = partials + (size_t)v * C * T * 3;
+  for (int j = 0; j < 2 + C; ++j) {
+    // j = 0, 1: l1 / ssim over all C * T CTAs of the view; j >= 2: squared error over the T CTAs of channel j - 2
+    const int n = j < 2 ? C * T : T;
+    const double* q = j < 2 ? p + j : p + (size_t)(j - 2) * T * 3 + 2;
+    double s = 0.0;
+    for (int i = threadIdx.x; i < n; i += kReduceThreads) s += q[(size_t)3 * i];
+    red[threadIdx.x] = s;
+    __syncthreads();
+#pragma unroll
+    for (int o = kReduceThreads / 2; o > 0; o >>= 1) {
+      if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) out[(size_t)v * (2 + C) + j] = red[0];
+    __syncthreads();
+  }
+}
+
 int check(cudaError_t e, const char* what) {
   if (e == cudaSuccess) return GSB_OK;
   char buf[256];
@@ -426,4 +492,40 @@ extern "C" GSB_API int gsb_loss_backward_batch(int32_t V, int32_t C, int32_t H, 
                                                             gt_row);
   gsb_prof_end(slot, (cudaStream_t)stream);
   return check(cudaGetLastError(), "k_loss_bwd_batch");
+}
+
+// Evaluation metrics of V views (include/gsb200.h): k_ssim_fwd<true, mode> writes one partial per CTA to `scratch`,
+// k_metrics_reduce adds each view's partials in a fixed order into out[v].  No atomics, so every view's result is
+// bit-identical from run to run and whatever else is in the batch.
+extern "C" GSB_API size_t gsb_image_metrics_scratch_bytes(int32_t V, int32_t C, int32_t H, int32_t W) {
+  if (V <= 0 || C <= 0 || H <= 0 || W <= 0) return 0;
+  const size_t T = (size_t)((W + TW - 1) / TW) * ((H + TH - 1) / TH);
+  return (size_t)V * C * T * 3 * sizeof(double);
+}
+
+extern "C" GSB_API int gsb_image_metrics_batch(int32_t V, int32_t C, int32_t H, int32_t W, const float* img,
+                                               const float* gt, const int32_t* gt_row, int32_t mode, double* out,
+                                               void* scratch, size_t scratch_bytes, gsb_stream_t stream) {
+  if (V <= 0 || C <= 0 || V > 65535 / C || H <= 0 || W <= 0 || !img || !gt || !gt_row || !out || !scratch ||
+      (mode != GSB_METRIC_CLAMP && mode != GSB_METRIC_PNG8)) {
+    gsb_set_error("gsb_image_metrics_batch: bad argument");
+    return GSB_ERR_INVALID;
+  }
+  if (scratch_bytes < gsb_image_metrics_scratch_bytes(V, C, H, W)) {
+    gsb_set_error("gsb_image_metrics_batch: scratch smaller than gsb_image_metrics_scratch_bytes()");
+    return GSB_ERR_INVALID;
+  }
+  if (ensure_window()) return check(cudaGetLastError(), "window upload");
+  dim3 grid((W + TW - 1) / TW, (H + TH - 1) / TH, V * C);
+  double* part = static_cast<double*>(scratch);
+  cudaStream_t st = (cudaStream_t)stream;
+  gsb_count_launch(2);
+  if (mode == GSB_METRIC_CLAMP)
+    k_ssim_fwd<true, kInClamp><<<grid, 256, 0, st>>>(H, W, img, gt, part, nullptr, 0, 1, C, gt_row);
+  else
+    k_ssim_fwd<true, kInPng8><<<grid, 256, 0, st>>>(H, W, img, gt, part, nullptr, 0, 1, C, gt_row);
+  int rc = check(cudaGetLastError(), "k_metrics_fwd");
+  if (rc != GSB_OK) return rc;
+  k_metrics_reduce<<<V, kReduceThreads, 0, st>>>(C, (int)(grid.x * grid.y), part, out);
+  return check(cudaGetLastError(), "k_metrics_reduce");
 }

@@ -171,6 +171,39 @@ class PoseTracker:
             return best[:, 1:].clone(), best[:, 0].clone(), trace
         return best[:, 1:].clone(), best[:, 0].clone()
 
+    def evaluate_batch(self, poses: torch.Tensor, gts: torch.Tensor, mode: str = "png8",
+                       max_batch: Optional[int] = None):
+        """render.py -> metrics.py for V views: render each row of poses [V, 7] (render_batch) and measure it against
+        gts [V, 3, H, W] (evaluation.image_metrics; mode "png8" is the 8-bit round trip of save_image and readImages).
+        Same input checks as optimize_batch; max_batch: views per batched forward (None: all at once).  Returns
+        image_metrics' dict (fp64 device tensors); view v's values are those of evaluate_batch on it alone."""
+        from .evaluation import _mode, metric_sums, metrics_from_sums
+        m = _mode(mode)
+        p = self._poses(poses, "evaluate_batch")
+        V = p.shape[0]
+        if not isinstance(gts, torch.Tensor) or tuple(gts.shape) != (V, 3, self.H, self.W):
+            raise ValueError(f"evaluate_batch: expected gts of shape {(V, 3, self.H, self.W)}, got "
+                             f"{tuple(getattr(gts, 'shape', ()))}")
+        self._same_device(gts, "evaluate_batch")
+        if max_batch is not None and int(max_batch) < 1:
+            raise ValueError("evaluate_batch: max_batch must be >= 1")
+        if V == 0:
+            raise ValueError("evaluate_batch: no views")
+        step = V if max_batch is None else int(max_batch)
+        with torch.cuda.device(self.dev):
+            gts = gts.detach().to(self.dev).float().contiguous()
+            cam = self._cam()
+            sums, ovf = [], torch.zeros(1, dtype=torch.int32, device=self.dev)
+            for v0 in range(0, V, step):
+                v1 = min(V, v0 + step)
+                fr = self._frame_batch(v1 - v0)
+                self._forward_batch(fr, cam, self._gauss(p[v0:v1]), p[v0:v1], True)
+                ovf |= fr.word(ST_OVERFLOW)
+                sums.append(metric_sums(fr.color, gts[v0:v1], list(range(v1 - v0)), m))
+            if int(ovf.item()):
+                raise _lib.GsbError("evaluate_batch: a tile list outgrew the binning buffer")
+            return metrics_from_sums(torch.cat(sums), self.H, self.W)
+
     def _optimize_views(self, poses, gts, num_iter, lr_T, lr_q, weight_decay, eta_min, threshold, return_trace):
         """One batched loop over poses.shape[0] views: (best [V, 8] on the host, trace [V, num_iter] or None)."""
         L = _lib.lib()

@@ -758,6 +758,81 @@ class JointTrainer:
         lam = self.cfg.lambda_dssim
         return (1.0 - lam) * s[:, 0] / n + lam * (1.0 - s[:, 1] / n)
 
+    # ---- evaluation (train.py:256-290 training_report; DESIGN.md section 4.11) ----------------------------------
+    def evaluate(self, views: Optional[Sequence[int]] = None, poses: Optional[torch.Tensor] = None,
+                 gts: Optional[torch.Tensor] = None, mode: str = "clamp",
+                 max_batch: Optional[int] = None) -> Dict[str, torch.Tensor]:
+        """training_report's loop: render views and measure them against their targets (evaluation.image_metrics).
+        views: indices into the pose table (None: every training view), each rendered at its pose row and compared
+        with gts[k] for views[k], or with the trainer's own target when gts is None.  poses [V, 7] with gts
+        [V, 3, H, W] instead: explicit poses (the test views at get_RT_test), not together with views.
+        Each chunk of up to max_batch views (None: all at once) is one batched forward as in a step (active SH
+        degree, Mip filters, exact_cull) with its own scratch, its binning buffer sized exactly from the preprocess
+        count, then one metrics call.  Returns image_metrics' dict over all views (fp64 device tensors); view k's
+        values do not depend on max_batch or on the other views.  Reads only the parameters, poses and targets and
+        writes no training state; the scratch is released on return."""
+        from .evaluation import _images, _mode, metric_sums, metrics_from_sums
+        if self.world_size > 1:
+            raise _lib.GsbError("evaluate needs world_size == 1 (evaluation on several GPUs is not implemented)")
+        m = _mode(mode)
+        if max_batch is not None and int(max_batch) < 1:
+            raise ValueError("evaluate: max_batch must be >= 1")
+        dev = self.dev if self.dev.index is not None else torch.device(self.dev.type, torch.cuda.current_device())
+        if poses is not None:
+            if views is not None:
+                raise ValueError("evaluate: pass views or poses, not both")
+            if not isinstance(poses, torch.Tensor) or poses.dim() != 2 or poses.shape[1] != 7 or \
+                    poses.dtype != torch.float32 or poses.device != dev:
+                raise ValueError(f"evaluate: poses must be a float32 [V, 7] tensor on {dev}, got "
+                                 f"{getattr(poses, 'dtype', type(poses))} {tuple(getattr(poses, 'shape', ()))} on "
+                                 f"{getattr(poses, 'device', None)}")
+            if gts is None:
+                raise ValueError("evaluate: explicit poses need their targets gts")
+            pose_rows = poses.detach().contiguous()
+            V = pose_rows.shape[0]
+        else:
+            views = list(range(self.n_views)) if views is None else [int(v) for v in views]
+            if any(not 0 <= v < self.n_views for v in views):
+                raise ValueError(f"evaluate: views {views} out of range 0..{self.n_views - 1}")
+            V = len(views)
+            if gts is None and self.gt is None:
+                raise ValueError("evaluate: no targets (the trainer has no gt_images and gts is None)")
+        if V == 0:
+            raise ValueError("evaluate: no views")
+        if gts is not None:
+            gts = _images(gts, "evaluate: gts", dev)
+            if tuple(gts.shape) != (V, 3, self.H, self.W):
+                raise ValueError(f"evaluate: gts must have shape {(V, 3, self.H, self.W)}, got {tuple(gts.shape)}")
+            target, rows = gts, list(range(V))
+        else:
+            target, rows = self.gt, views
+        if poses is None:
+            with torch.no_grad():      # a restored pose table may carry requires_grad from the checkpoint's Parameter
+                pose_rows = self.poses.detach()[torch.tensor(views, dtype=torch.int64, device=dev)].contiguous()
+        step = V if max_batch is None else int(max_batch)
+        cam = self.ident.camera(self.active_sh_degree, 16, self.exact_cull)
+        p = self.params
+        host_status = torch.zeros(ST_WORDS, dtype=torch.int32).pin_memory()
+        sums, ovf = [], torch.zeros(1, dtype=torch.int32, device=dev)
+        fr = None
+        for v0 in range(0, V, step):
+            v1 = min(V, v0 + step)
+            pr = pose_rows[v0:v1]
+            if fr is None or fr.views != v1 - v0:
+                fr = None
+                fr = Frame(dev, self.P, self.W, self.H, views=v1 - v0)
+            g = gaussians(self.P, *(self.view(p, n) for n in ("xyz", "rotation", "scaling", "opacity", "f_dc",
+                                                               "f_rest")), pr)
+            fr.preprocess_batch(cam, g, pr, host_status, self.filt)
+            torch.cuda.current_stream(dev).synchronize()
+            fr.alloc_binning(max(1, read_R(host_status)))
+            fr.render_batch(cam)
+            ovf |= fr.word(ST_OVERFLOW)
+            sums.append(metric_sums(fr.color, target, rows[v0:v1], m))
+        if int(ovf.item()):
+            raise _lib.GsbError("evaluate: a tile list outgrew the binning buffer sized from the preprocess count")
+        return metrics_from_sums(torch.cat(sums), self.H, self.W)
+
     class _BatchScratch:
         """step_batch's buffers for V views: the batch Frame with its own pinned status slot (its forwards have their own
         serial numbers, see _settle), sel [2, V] (view ids, target rows; uploaded per call), the gathered poses and their
