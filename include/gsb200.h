@@ -413,7 +413,8 @@ GSB_API int gsb_profile_collect(double* ms_sum, int64_t* count, int n_ids);
 GSB_API uint64_t gsb_launch_count(void);
 /* Tuning switches: "blend_version" = 1 (one pixel per lane, 8 warps per tile; the in-library cross-check) | 2 (two
  * pixels per lane; default); "stage_bulk" = 1 (slab chunks staged with cp.async.bulk/TMA +
- * mbarrier, double buffered; default) | 0. */
+ * mbarrier, double buffered; default) | 0; "blend_bwd_batch" = 1 (the v2 blend backward reduces its per-Gaussian
+ * moments in per-warp batches; default) | 0 (one warp butterfly per list entry: the bit-for-bit reference). */
 GSB_API int gsb_set_option(const char* name, int value);
 
 GSB_API const char* gsb_last_error(void);

@@ -27,11 +27,19 @@ constexpr float kLn2 = 0.6931471805599453f;
 #ifndef GSB_FWD_MINB
 #define GSB_FWD_MINB 8
 #endif
+#ifndef GSB_BWD_CHUNK
+#define GSB_BWD_CHUNK 192
+#endif
 #ifndef GSB_BWD_MINB
-#define GSB_BWD_MINB 8
+#define GSB_BWD_MINB 6
 #endif
 constexpr int kChunk1 = 256;           // v1 blend kernels: one entry per thread
-constexpr int kChunk = GSB_CHUNK;      // slab entries staged per step in the blend kernels
+constexpr int kChunk = GSB_CHUNK;      // slab entries staged per step in the forward (and the butterfly backward)
+// The batched backward (k_blend_bwd2<..., BATCH>) adds 15.2 KB of batch rows per CTA; with shorter chunks its CTA
+// (35.5 KB + 1 KB reserved) fits GSB_BWD_MINB = 6 times into an SM's 228 KB, and 6 x 128 threads x 80 registers
+// fit.  The butterfly instance keeps the forward's chunk and 8 CTAs / SM.
+constexpr int kChunkB = GSB_BWD_CHUNK;
+constexpr int kBwdMinBFly = 8;
 
 // ------------------------------------------------------------------------------------------
 // blend
@@ -364,10 +372,12 @@ constexpr int kThreads2 = 128;
 // byte count and issues cp.async.bulk.shared.global for the three slab arrays of the NEXT chunk
 // while the CTA blends the current one (double buffered).  SASS: UBLKCP + SYNCS.
 // ------------------------------------------------------------------------------------------
+template <int CH>
 struct SlabStage {
-  float4 s0[kChunk], s1[kChunk], s2[kChunk];     // record rows 0..2 of the chunk's entries: x,y,A',B' | C',o,qthr',id | r,g,b,-
+  float4 s0[CH], s1[CH], s2[CH];                 // record rows 0..2 of the chunk's entries: x,y,A',B' | C',o,qthr',id | r,g,b,-
 };
-constexpr int kIdRow = kChunk + 4;               // id chunk + up to 3 leading entries (bulk copies start 16-byte aligned)
+template <int CH>
+constexpr int id_row() { return CH + 4; }        // id chunk + up to 3 leading entries (bulk copies start 16-byte aligned)
 
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
@@ -383,10 +393,10 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 //   land(more)  wait until the oldest outstanding gather has landed (more: a younger one is in flight) + CTA barrier
 // Schedule used by the kernels: request(0), request(1), gather(0); then per chunk q: gather(q+1), request(q+2), land,
 // blend chunk q, CTA barrier.  Every buffer is rewritten only after the barrier that ends its last reader.
-template <bool BULK, int NT>
+template <bool BULK, int NT, int CH>
 struct Stager {
-  SlabStage* stg;                 // [2]
-  uint32_t (*sid)[kIdRow];        // [3]   (BULK only)
+  SlabStage<CH>* stg;             // [2]
+  uint32_t (*sid)[id_row<CH>()];  // [3]   (BULK only)
   uint64_t* bars;                 // [3]   (BULK only)
   const uint32_t* ids;
   const float4* rec;
@@ -411,7 +421,7 @@ struct Stager {
     }
   }
   __device__ __forceinline__ void gather(int q, size_t e, int cnt) {
-    SlabStage* st = &stg[q & 1];
+    SlabStage<CH>* st = &stg[q & 1];
     if (BULK) {
       mbar_wait(&bars[q % 3], (uint32_t)((q / 3) & 1));
       waited = q + 1;
@@ -452,10 +462,10 @@ k_blend_fwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids,
              float* __restrict__ out_color, float* __restrict__ final_T, uint32_t* __restrict__ n_contrib,
              unsigned long long* __restrict__ stats = nullptr) {
   unsigned int st_iter = 0, st_valid = 0;
-  __shared__ __align__(128) SlabStage stg[2];
-  __shared__ __align__(16) uint32_t sid[BULK ? 3 : 1][kIdRow];
+  __shared__ __align__(128) SlabStage<kChunk> stg[2];
+  __shared__ __align__(16) uint32_t sid[BULK ? 3 : 1][id_row<kChunk>()];
   __shared__ __align__(8) uint64_t bars[3];
-  Stager<BULK, kThreads2> sg{stg, sid, bars, ids, rec, 0, 0};
+  Stager<BULK, kThreads2, kChunk> sg{stg, sid, bars, ids, rec, 0, 0};
   sg.init();
   const int tile = view_tile(W, H, out_color, final_T, n_contrib);
   const int tx = blockIdx.x % gx, ty = blockIdx.x / gx;
@@ -486,7 +496,7 @@ k_blend_fwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids,
   for (int ci = 0; ci < nch; ++ci) {
     const int base = ci * kChunk;
     const int cnt = min(kChunk, n - base);
-    const SlabStage* cur = &stg[ci & 1];
+    const SlabStage<kChunk>* cur = &stg[ci & 1];
     if (ci + 1 < nch) {          // keep the pipeline full: records of chunk ci+1, ids of chunk ci+2
       sg.gather(ci + 1, c_e(ci + 1), c_n(ci + 1));
       if (ci + 2 < nch) sg.request(ci + 2, c_e(ci + 2), c_n(ci + 2));
@@ -560,24 +570,76 @@ k_blend_fwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids,
   }
 }
 
+// A batch row: the 32 lanes' values of one (entry, value), padded to 36 floats.  The row stores (lane L -> word
+// 36 r + L) hit 32 banks; so do the reduction's LDS.128 (lane t reads row t, and the 8 lanes of a phase start at
+// banks 4 t mod 32, 8 different 16-byte bank groups), and every address is a base plus an immediate.
+constexpr int kBatchRow = 36;
+
+// The sum of the 32 floats of a batch row, grouped as warp_reduce9 / warp_reduce8 group a value over the lanes: pairs
+// over lane bits 4, 3, 2, 1, 0 in that order.  Float addition is commutative, so only the grouping decides the bits
+// and the total equals the butterfly's bit for bit.
+__device__ __forceinline__ float batch_row_sum(const float* row) {
+  auto col = [&](int c) { return *reinterpret_cast<const float4*>(row + 4 * c); };
+  auto add = [](float4 a, float4 b) {
+    return make_float4(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y), __fadd_rn(a.z, b.z), __fadd_rn(a.w, b.w));
+  };
+  float4 q[4];
+#pragma unroll
+  for (int c = 0; c < 4; ++c) q[c] = add(col(c), col(c + 4));       // lane bit 4: lanes 4c.. and 4c+16..
+  q[0] = add(q[0], q[2]);                                            // lane bit 3
+  q[1] = add(q[1], q[3]);
+  q[0] = add(q[0], q[1]);                                            // lane bit 2
+  return __fadd_rn(__fadd_rn(q[0].x, q[0].z), __fadd_rn(q[0].y, q[0].w));   // lane bits 1, 0
+}
+
+// Reduces a warp's batch of n entries (rows[s * NV + i] = value i of entry s, one column per lane) and adds the
+// totals to the fixed-point accumulators: lane t < n * NV owns value t % NV of entry t / NV.  Lane s holds entry s's
+// accumulator index in idx and its extent in ext.  The first __syncwarp orders the lanes' row stores before these
+// reads, the second these reads before the next batch's stores.
+template <int NV, bool STATS>
+__device__ __forceinline__ void batch_flush(const float (*rows)[kBatchRow], int n, uint32_t idx, float ext,
+                                            unsigned long long* dacc, float inv_m, int lane) {
+  __syncwarp();
+  const int s = lane / NV, slot = lane - s * NV;
+  const uint32_t gi = __shfl_sync(0xffffffffu, idx, s);
+  const float e = __shfl_sync(0xffffffffu, ext, s);
+  if (lane < n * NV) {
+    const float total = batch_row_sum(rows[lane]);
+    if (!STATS) atomicAdd(dacc + (size_t)gi * kDaccSlots + slot, fix_encode(total, fix_scale(slot, e, inv_m)));
+  }
+  __syncwarp();
+}
+
 // POSE_ONLY (tracking mode, render.py:99-170: Gaussians frozen): dL/dopacity is not needed, so the moment S w is
 // dropped and dL/db takes its slot -- eight values, no ninth reduction chain, no scalar RED; k_preprocess_bwd is
 // told about the layout (dacc[5] = dL/db, dacc[8] unused).
-template <bool BULK, bool STATS = false, bool POSE_ONLY = false>
-__global__ void __launch_bounds__(kThreads2, GSB_BWD_MINB)
+//
+// BATCH (default): instead of one butterfly per list entry, every lane stores its NV values of the entry as one
+// column of the warp's batch rows (row s * NV + i = value i of the batch's entry s) and the warp walks on; when
+// NB = 3 entries are stored, and at the end of the list, lane t sums row t (batch_row_sum) and adds the total with
+// one fixed-point RED.  The rows need no staging memory, and the entry's accumulator index and extent are captured
+// in registers when it is stored, so a batch may span a chunk barrier.  !BATCH is the per-entry butterfly
+// (warp_reduce9 / warp_reduce8 + flush_fixed) with the forward's chunk and 8 CTAs / SM, selected by
+// gsb_set_option("blend_bwd_batch", 0): the bit-for-bit reference of the batched reduction.
+template <bool BULK, bool STATS = false, bool POSE_ONLY = false, bool BATCH = true>
+__global__ void __launch_bounds__(kThreads2, BATCH ? GSB_BWD_MINB : kBwdMinBFly)
 k_blend_bwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids, const float4* __restrict__ rec,
              const float* __restrict__ bg, int W, int H, int gx,
              const float* __restrict__ final_T, const uint32_t* __restrict__ n_contrib,
              const float* __restrict__ dL_dpix, unsigned long long* __restrict__ dacc,
              const uint32_t* __restrict__ dscale, unsigned long long* __restrict__ stats = nullptr) {
+  constexpr int CH = BATCH ? kChunkB : kChunk;
+  constexpr int NV = POSE_ONLY ? 8 : 9;                 // values per entry
+  constexpr int NB = 3;                                 // entries per batch: NB * NV <= 32 rows, one per lane
   unsigned int st_iter = 0, st_red = 0, st_valid = 0;
   const int tile = view_tile_bwd(W, H, dL_dpix, final_T, n_contrib, dscale);
   const float inv_m = fix_inv_m(dscale);
-  __shared__ __align__(128) SlabStage stg[2];
-  __shared__ __align__(16) uint32_t sid[BULK ? 3 : 1][kIdRow];
+  __shared__ __align__(128) SlabStage<CH> stg[2];
+  __shared__ __align__(16) uint32_t sid[BULK ? 3 : 1][id_row<CH>()];
   __shared__ __align__(8) uint64_t bars[3];
   __shared__ int s_bmax;
-  Stager<BULK, kThreads2> sg{stg, sid, bars, ids, rec, 0, 0};
+  __shared__ __align__(16) float s_batch[BATCH ? kThreads2 / 32 : 1][BATCH ? NB * NV : 1][kBatchRow];
+  Stager<BULK, kThreads2, CH> sg{stg, sid, bars, ids, rec, 0, 0};
   sg.init();
   const int tx = blockIdx.x % gx, ty = blockIdx.x / gx;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -613,10 +675,13 @@ k_blend_bwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids,
   const int bmax = s_bmax;
   float2 T = T_final;
   float2 acc_r = f2(0.f, 0.f), acc_g = f2(0.f, 0.f), acc_b = f2(0.f, 0.f);
-  const int nchunks = (bmax + kChunk - 1) / kChunk;
+  int nb = 0;                                           // BATCH: entries in the warp's batch
+  uint32_t b_idx = 0;                                   // BATCH: lane s < nb holds entry s's accumulator index
+  float b_ext = 0.f;                                    //        and fixed-point extent
+  const int nchunks = (bmax + CH - 1) / CH;
   // chunks are visited back to front; pipeline step q = 0 is the LAST chunk
-  auto c_e = [&](int q) { return (size_t)rg.x + (size_t)(nchunks - 1 - q) * kChunk; };
-  auto c_n = [&](int q) { return min(kChunk, bmax - (nchunks - 1 - q) * kChunk); };
+  auto c_e = [&](int q) { return (size_t)rg.x + (size_t)(nchunks - 1 - q) * CH; };
+  auto c_n = [&](int q) { return min(CH, bmax - (nchunks - 1 - q) * CH); };
   if (nchunks > 0) {
     sg.request(0, c_e(0), c_n(0));
     if (nchunks > 1) sg.request(1, c_e(1), c_n(1));
@@ -624,9 +689,9 @@ k_blend_bwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids,
   }
   for (int it = 0; it < nchunks; ++it) {
     const int ch = nchunks - 1 - it;
-    const int base = ch * kChunk;
-    const int cnt = min(kChunk, bmax - base);
-    const SlabStage* cur = &stg[it & 1];
+    const int base = ch * CH;
+    const int cnt = min(CH, bmax - base);
+    const SlabStage<CH>* cur = &stg[it & 1];
     if (it + 1 < nchunks) {
       sg.gather(it + 1, c_e(it + 1), c_n(it + 1));
       if (it + 2 < nchunks) sg.request(it + 2, c_e(it + 2), c_n(it + 2));
@@ -696,14 +761,27 @@ k_blend_bwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids,
           v[7] = dcol.x * dLg.x + dcol.y * dLg.y;
           v[8] = dcol.x * dLb.x + dcol.y * dLb.y;
           v[5] = POSE_ONLY ? v[8] : ws;                          // S w (or dL/db in the 8-value layout)
-          if (POSE_ONLY) warp_reduce8(v, lane); else warp_reduce9(v, lane);
-          if (!STATS)
-            flush_fixed(dacc + (size_t)__float_as_uint(e1.w) * kDaccSlots, v[0], v[8], c.w, inv_m, lane, !POSE_ONLY);
+          if constexpr (BATCH) {
+            float* col = &s_batch[warp][nb * NV][lane];
+#pragma unroll
+            for (int i = 0; i < NV; ++i) col[kBatchRow * i] = v[i];
+            if (lane == nb) { b_idx = __float_as_uint(e1.w); b_ext = c.w; }
+            if (++nb == NB) {
+              batch_flush<NV, STATS>(s_batch[warp], NB, b_idx, b_ext, dacc, inv_m, lane);
+              nb = 0;
+            }
+          } else {
+            if (POSE_ONLY) warp_reduce8(v, lane); else warp_reduce9(v, lane);
+            if (!STATS)
+              flush_fixed(dacc + (size_t)__float_as_uint(e1.w) * kDaccSlots, v[0], v[8], c.w, inv_m, lane, !POSE_ONLY);
+          }
         }
       }
     }
     __syncthreads();
   }
+  if constexpr (BATCH)
+    if (nb > 0) batch_flush<NV, STATS>(s_batch[warp], nb, b_idx, b_ext, dacc, inv_m, lane);
   sg.drain();
   if (STATS) {
 #pragma unroll
@@ -747,16 +825,18 @@ int gsb_launch_blend_bwd(const GeomView& gv, const BinView& bv, const ImgView& i
   const size_t nb = (n + kThreads - 1) / kThreads, max_blocks = 4 * (size_t)gsb_sm_count();
   k_abs_max<<<dim3((int)(nb < max_blocks ? nb : max_blocks), V), kThreads, 0, st>>>(n, dL_dout, gv.dscale);
   const int ver = gsb_option_blend_version(), bulk = gsb_option_stage_bulk();
+  const bool batch = gsb_option_blend_bwd_batch();
   unsigned long long* dacc = gv.dacc;
+  auto v2 = [&](auto kernel) {
+    kernel<<<grid, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, iv.final_T, iv.n_contrib, dL_dout, dacc,
+                                       gv.dscale, nullptr);
+  };
   if (pose_only)
-    k_blend_bwd2<true, false, true><<<grid, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, iv.final_T,
-                                                                iv.n_contrib, dL_dout, dacc, gv.dscale);
+    batch ? v2(k_blend_bwd2<true, false, true, true>) : v2(k_blend_bwd2<true, false, true, false>);
   else if (ver == 2 && bulk)
-    k_blend_bwd2<true><<<grid, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, iv.final_T,
-                                                   iv.n_contrib, dL_dout, dacc, gv.dscale);
+    batch ? v2(k_blend_bwd2<true, false, false, true>) : v2(k_blend_bwd2<true, false, false, false>);
   else if (ver == 2)
-    k_blend_bwd2<false><<<grid, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, iv.final_T,
-                                                    iv.n_contrib, dL_dout, dacc, gv.dscale);
+    batch ? v2(k_blend_bwd2<false, false, false, true>) : v2(k_blend_bwd2<false, false, false, false>);
   else
     k_blend_bwd<<<grid, kThreads, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, iv.final_T, iv.n_contrib,
                                            dL_dout, dacc, gv.dscale);

@@ -42,6 +42,7 @@ struct ProfScope {
 };
 int gsb_option_blend_version();
 int gsb_option_stage_bulk();
+int gsb_option_blend_bwd_batch();
 int gsb_sm_count();
 
 namespace gsb {

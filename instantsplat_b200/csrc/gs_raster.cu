@@ -86,7 +86,9 @@ extern "C" GSB_API uint64_t gsb_launch_count(void) { return g_launches.load(); }
 static std::atomic<int> g_blend_version{2};
 static std::atomic<int> g_stage_bulk{1};   // 1: slabs staged with cp.async.bulk (TMA) + mbarrier, 0: cooperative loads
 int gsb_option_blend_version() { return g_blend_version.load(std::memory_order_relaxed); }
+static std::atomic<int> g_blend_bwd_batch{1};   // 1: batched moment reduction, 0: per-entry butterfly (its reference)
 int gsb_option_stage_bulk() { return g_stage_bulk.load(std::memory_order_relaxed); }
+int gsb_option_blend_bwd_batch() { return g_blend_bwd_batch.load(std::memory_order_relaxed); }
 // SM count of the current device, cached per device: sizes the persistent and grid-stride launches (132 on an H100 SXM)
 int gsb_sm_count() {
   static std::atomic<int> sms[64];
@@ -102,6 +104,7 @@ int gsb_sm_count() {
 extern "C" GSB_API int gsb_set_option(const char* name, int value) {
   if (name && strcmp(name, "blend_version") == 0 && value >= 1 && value <= 2) { g_blend_version = value; return GSB_OK; }
   if (name && strcmp(name, "stage_bulk") == 0 && (value == 0 || value == 1)) { g_stage_bulk = value; return GSB_OK; }
+  if (name && strcmp(name, "blend_bwd_batch") == 0 && (value == 0 || value == 1)) { g_blend_bwd_batch = value; return GSB_OK; }
   gsb_set_error("gsb_set_option: unknown option or bad value");
   return GSB_ERR_INVALID;
 }
