@@ -139,8 +139,7 @@ def batch_events(cfg, before: int, V: int) -> Dict[str, object]:
     """What one optimizer step over V views does to the schedules, starting from `before` views consumed (step() with
     G ranks, JointTrainer.step_batch with V views): the new iteration count; whether it crosses an SH-degree step
     (oneupSHdegree) or a 3D-filter recompute (not within the last 100 iterations); whether Adam steps (not at or
-    after cfg.iterations).  The learning rates are those of the new iteration (adam_step_sizes).  step() writes the
-    same rules out inline (it is left as it was); keep the two alike."""
+    after cfg.iterations).  The learning rates are those of the new iteration (adam_step_sizes)."""
     it = before + V
     return dict(iteration=it, sh_up=it // cfg.sh_increase_interval > before // cfg.sh_increase_interval,
                 mip=it // cfg.mip_filter3d_interval > before // cfg.mip_filter3d_interval and it < cfg.iterations - 100,
@@ -149,7 +148,8 @@ def batch_events(cfg, before: int, V: int) -> Dict[str, object]:
 
 def batch_densify_events(cfg, before: int, V: int, white_background: bool) -> Dict[str, object]:
     """The densification schedule of one optimizer step over V views starting from `before` views consumed
-    (JointTrainer.step_batch with densify): view k of the batch stands for iteration before + 1 + k.
+    (JointTrainer.step_batch with densify, and step(), which densifies on one GPU only, with V = 1): view k of the
+    batch stands for iteration before + 1 + k.
       n_stats: how many leading views count their statistics (those whose iteration is < densify_until_iter);
       densify: some covered iteration j is a densify point of step() (densify_from_iter < j < densify_until_iter,
                j % densification_interval == 0);
@@ -157,7 +157,7 @@ def batch_densify_events(cfg, before: int, V: int, white_background: bool) -> Di
              background and j == densify_from_iter);
       size_threshold: the screen-size limit of the densify, that of the last densify point covered (cfg.size_threshold
              when it is past opacity_reset_interval, else None); None without a densify.
-    Each event fires at most once per step.  With V = 1 these are the rules step() writes out inline; keep them alike."""
+    Each event fires at most once per step.  With V = 1 these are train.py's per-iteration rules."""
     its = range(before + 1, before + V + 1)
     dens = [j for j in its if cfg.densify_from_iter < j < cfg.densify_until_iter and j % cfg.densification_interval == 0]
     reset = any(j < cfg.densify_until_iter and (j % cfg.opacity_reset_interval == 0 or
@@ -244,14 +244,13 @@ class JointTrainer:
         self._set_per_point_lr(scene.per_point_lr if self.cfg.pp_optimizer else None)
         self.gt = None if gt_images is None else gt_images.to(self.dev).float().contiguous()
         self.ident = IdentityView(self.W, self.H, scene.fovx, scene.fovy, scene.bg, self.dev)
-        self.frame = Frame(self.dev, P, self.W, self.H)     # scratch; its binning buffer is sized by the first forward
+        self._single = self._Slot(self.dev, P, self.W, self.H)   # step()'s forward; sized by the first forward
         self.headroom = 1.5
         self.filter_3D, self.filt, self.mip_recomputed_at = None, None, []
         self._mip_setup()
         self.dL_dimg = torch.empty_like(self.color)
         self.maps = torch.empty(3, 3, self.H, self.W, dtype=torch.float32, device=self.dev)
         self.sums = torch.zeros(2, dtype=torch.float64, device=self.dev)
-        self.host_status = torch.zeros(2, ST_WORDS, dtype=torch.int32).pin_memory()   # [0] after preprocess, [1] after render
         self._ev_pre = torch.cuda.Event()
         self._ovf = None
         self.flags = torch.zeros(8, dtype=torch.int32, device=self.dev)
@@ -267,8 +266,6 @@ class JointTrainer:
         self._graphs = {}
         self._after_backward = None   # test hook: called (and captured) between the backward and the optimizer step
         self._step_dev = torch.zeros(8, dtype=torch.float32, device=self.dev)   # every update's step sizes (_advance)
-        self.frame.status.zero_()     # the forward serial number lives in these words
-        self._fwd_count = 0
         self._polling = False
         self.iteration = 0            # reference iterations = views consumed (by all ranks)
         self.opt_step = 0
@@ -288,7 +285,7 @@ class JointTrainer:
             self.densify_generator = torch.Generator(device=self.dev).manual_seed(int(c.densify_seed))
             self.white_background = bool((scene.bg == 1).all())
         self.densified_at, self.reset_at = [], []
-        self._batch = None            # step_batch's scratch for the view count of its last call (_batch_scratch)
+        self._batch = None            # step_batch's slot for the view count of its last call (_batch_scratch)
         self._batch_sums = None       # per-view loss sums of the last step_batch (batch_loss_values)
 
     # ------------------------------------------------------------------------------------------
@@ -300,6 +297,16 @@ class JointTrainer:
     def my_views(self) -> List[int]:
         from .parallel import shard_views
         return shard_views(self.n_views, self.world_size, self.rank)
+
+    @property
+    def frame(self) -> Frame:
+        """The Frame of step() and render() (one view)."""
+        return self._single.frame
+
+    @property
+    def host_status(self) -> torch.Tensor:
+        """The pinned [2, ST_WORDS] status words of that frame's last forward: [0] after preprocess, [1] after render."""
+        return self._single.host_status
 
     @property
     def color(self) -> torch.Tensor:
@@ -342,44 +349,54 @@ class JointTrainer:
         mip_filter3d(self.view(self.params, "xyz"), self.poses, self.W, self.H, self.ident.tanfovx, self.ident.tanfovy,
                      out=self.filter_3D)
 
-    def _gauss(self, view: int) -> GsbGaussians:
+    def _gauss(self, poses: torch.Tensor) -> GsbGaussians:
+        """The Gaussians at a pose row [7] (or, for the batched entry points, rows [V, 7])."""
         p = self.params
         return gaussians(self.P, *(self.view(p, n) for n in ("xyz", "rotation", "scaling", "opacity", "f_dc", "f_rest")),
-                         self.poses[view])
+                         poses)
+
+    def _camera(self):
+        return self.ident.camera(self.active_sh_degree, 16, self.exact_cull)
 
     # ------------------------------------------------------------------------------------------
-    def _size_binning(self, R: int, fr: Optional[Frame] = None) -> None:
-        (self.frame if fr is None else fr).alloc_binning(capacity(R, self.headroom))
+    def _size_binning(self, R: int, slot: Optional["_Slot"] = None) -> None:
+        """A binning buffer for R instances plus headroom, in `slot`'s frame (None: step()'s)."""
+        (slot or self._single).frame.alloc_binning(capacity(R, self.headroom))
 
-    def _launch_forward(self, view: int) -> None:
-        """Enqueue the forward without ever waiting for the GPU: the instance count R stays on the device; the
-        host only provides a capacity (sized from the counts seen so far, +50 %) and reads R back lazily."""
-        cam, g = self.ident.camera(self.active_sh_degree, 16, self.exact_cull), self._gauss(view)
-        capturing = torch.cuda.is_current_stream_capturing()
-        self.frame.preprocess(cam, g, self.host_status[0], self.filt)
-        if not capturing:
-            self._fwd_count += 1
+    def _forward(self, slot: "_Slot", cam, g: GsbGaussians, poses: Optional[torch.Tensor] = None) -> None:
+        """Enqueue a forward of `slot`'s frame (poses: the [V, 7] rows of a batch slot) without ever waiting for the
+        GPU: the instance count R stays on the device; the host only provides a capacity (sized from the counts seen
+        so far, +50 %) and reads R back lazily."""
+        fr, hs = slot.frame, slot.host_status
+        if slot.V is None:
+            fr.preprocess(cam, g, hs[0], self.filt)
+        else:
+            fr.preprocess_batch(cam, g, poses, hs[0], self.filt)
+        if not torch.cuda.is_current_stream_capturing():
+            slot.fwd_count += 1
             self._polling = False
             self._ev_pre.record()
-            if self.cap == 0:                         # very first forward: size the buffer from the real count
+            if fr.cap == 0:                           # very first forward: size the buffer from the real count
                 self._ev_pre.synchronize()
-                self._size_binning(read_R(self.host_status[0]))
-        self.frame.render(cam, self.host_status[1])
+                self._size_binning(read_R(hs[0]), slot)
+        (fr.render if slot.V is None else fr.render_batch)(cam, hs[1])
+
+    def _launch_forward(self, view: int) -> None:
+        cam, g = self._camera(), self._gauss(self.poses[view])
+        self._forward(self._single, cam, g)
         self._keep = (cam, g)
 
-    def _settle(self, batch=None) -> bool:
-        """Wait for the status words of the last forward's preprocess phase (early in the stream: the GPU still has
-        the rest of the iteration queued, so this never starves it).  Returns True if the binning buffer was big
-        enough; otherwise grows it (the device skipped the optimizer update by itself) and returns False.
-        batch: step_batch's scratch, whose frame made that forward (None: self.frame).  Each frame counts its forwards
-        in its own status words and copies them to its own pinned slot, so a serial number is only ever compared with
-        the count of the frame that wrote it."""
-        fr = self.frame if batch is None else batch.frame
-        hs = self.host_status if batch is None else batch.host_status
+    def _settle(self, slot: Optional["_Slot"] = None) -> bool:
+        """Wait for the status words of the preprocess phase of `slot`'s last forward (None: step()'s slot; early in
+        the stream: the GPU still has the rest of the iteration queued, so this never starves it).  Returns True if the
+        binning buffer was big enough; otherwise grows it (the device skipped the optimizer update by itself) and
+        returns False."""
+        slot = slot or self._single
+        fr, hs = slot.frame, slot.host_status
         if self._polling:
             # graph replay: no host-visible event inside the graph, so watch the pinned status words for this forward's
             # serial number (written by the tile scan, copied by the memcpy node right behind it)
-            want = (self._fwd_count if batch is None else batch.fwd_count) & 0x7FFFFFFF
+            want = slot.fwd_count & 0x7FFFFFFF
             n = 0
             while (int(hs[0, ST_SEQ]) & 0x7FFFFFFF) != want:
                 n += 1
@@ -391,18 +408,19 @@ class JointTrainer:
         self.last_R = R
         if R > fr.cap:
             self.overflows += 1
-            self._size_binning(R, fr)
+            self._size_binning(R, slot)
             return False
         if R > 0.85 * fr.cap:                          # grow ahead of need
-            self._size_binning(R, fr)
+            self._size_binning(R, slot)
         return True
 
-    def _settled(self, enqueue, local: bool = False, batch=None) -> None:
+    def _settled(self, enqueue, local: bool = False, batch: Optional["_Slot"] = None) -> None:
         """enqueue() launches a forward, possibly with the rest of an iteration; then wait for its instance count.  When
         the binning buffer was too small, the device has skipped the optimizer update by itself (gated on the overflow
         word, summed over the ranks in multi-GPU mode), so parameters and moments are untouched, and _settle has grown
         the buffer: enqueue once more.  Several ranks cannot do that within a training iteration, because the other
-        ranks cannot know yet; they stop loudly.  local: only this rank's forward, which any rank may repeat."""
+        ranks cannot know yet; they stop loudly.  local: only this rank's forward, which any rank may repeat.
+        batch: the slot whose frame makes that forward (None: step()'s single-view slot)."""
         for _ in range(2):
             enqueue()
             if self._settle(batch):
@@ -428,6 +446,16 @@ class JointTrainer:
                                  self.maps.data_ptr(), st), "gsb_loss_forward")
         check(L.gsb_loss_backward(3, self.H, self.W, self.color.data_ptr(), gt.data_ptr(), self.maps.data_ptr(),
                                   float(self.cfg.lambda_dssim), self.dL_dimg.data_ptr(), st), "gsb_loss_backward")
+        gr = self._grads()
+        self.pose_grad.zero_()
+        gr.dL_dpose = self.pose_grad[view].data_ptr()
+        st = None
+        if stats:
+            st = densify_stats(self.frame.radii, self._stats[0], self._stats[1], self._stats[2])
+        self.frame.backward(cam, g, self.dL_dimg, gr, self.filt, st)
+
+    def _grads(self) -> GsbGrads:
+        """GsbGrads over the per-Gaussian segments of the flat gradient buffer (no pose gradient)."""
         gr = GsbGrads()
         gd = self.grads
         gr.dL_dmeans3D = self.view(gd, "xyz").data_ptr()
@@ -436,17 +464,16 @@ class JointTrainer:
         gr.dL_dopacities = self.view(gd, "opacity").data_ptr()
         gr.dL_dsh_dc = self.view(gd, "f_dc").data_ptr()
         gr.dL_dsh_rest = self.view(gd, "f_rest").data_ptr()
-        self.pose_grad.zero_()
-        gr.dL_dpose = self.pose_grad[view].data_ptr()
-        st = None
-        if stats:
-            st = densify_stats(self.frame.radii, self._stats[0], self._stats[1], self._stats[2])
-        self.frame.backward(cam, g, self.dL_dimg, gr, self.filt, st)
+        return gr
 
-    def loss_value(self) -> torch.Tensor:
+    def _loss(self, sums: torch.Tensor) -> torch.Tensor:
+        """train.py's loss (1 - lambda_dssim) L1 + lambda_dssim (1 - SSIM) from loss sums [..., 2] (L1, SSIM)."""
         n = 3 * self.H * self.W
         lam = self.cfg.lambda_dssim
-        return (1.0 - lam) * self.sums[0] / n + lam * (1.0 - self.sums[1] / n)
+        return (1.0 - lam) * sums[..., 0] / n + lam * (1.0 - sums[..., 1] / n)
+
+    def loss_value(self) -> torch.Tensor:
+        return self._loss(self.sums)
 
     def reduce_grads(self) -> None:
         if self.world_size > 1:
@@ -582,9 +609,9 @@ class JointTrainer:
             self.reduce_grads()
             self._launch_adam()
 
-    def _replay(self, view: int, gt: torch.Tensor, do_opt: bool, stats: bool = False) -> None:
-        """Replay (capturing on first use) the CUDA graph of _enqueue_iteration on `view`."""
-        key = (view, gt.data_ptr(), do_opt, self.active_sh_degree, self.cap, self.exact_cull, stats)
+    def _replay(self, key: tuple, slot: "_Slot", enqueue) -> None:
+        """Replay the CUDA graph cached under `key`, capturing enqueue() (an iteration whose forward runs on `slot`'s
+        frame) into it on first use."""
         g = self._graphs.get(key)
         if g is None:
             if len(self._graphs) > 64:
@@ -592,9 +619,9 @@ class JointTrainer:
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                self._enqueue_iteration(view, gt, do_opt, stats)
+                enqueue()
             self._graphs[key] = g
-        self._fwd_count += 1
+        slot.fwd_count += 1
         self._polling = True
         g.replay()
 
@@ -622,45 +649,58 @@ class JointTrainer:
         With G GPUs one call consumes G views (one per rank): `iteration` counts VIEWS, so the learning-rate and
         SH-degree schedules advance per view as in the reference, while Adam's bias correction counts optimizer
         steps.  Nothing in here waits for the GPU except `_settle()`, which waits for an event early in the stream."""
-        c = self.cfg
-        before = self.iteration
-        self.iteration += self.world_size
-        if self.iteration // c.sh_increase_interval > before // c.sh_increase_interval:
-            self.active_sh_degree = min(self.active_sh_degree + 1, c.max_sh_degree)     # oneupSHdegree
         if gt is None:
             gt = self.gt[view]
-        do_opt = self.iteration < c.iterations
-        it = self.iteration
-        stats = self._stats is not None and it < c.densify_until_iter
-        densify_now = stats and it > c.densify_from_iter and it % c.densification_interval == 0
-        reset_now = stats and (it % c.opacity_reset_interval == 0 or
-                               (self.white_background and it == c.densify_from_iter))
-        if densify_now or reset_now:
+        self._run_step(self.world_size, self._single, ("step", view, gt.data_ptr()),
+                       lambda do_opt, n_stats: self._enqueue_iteration(view, gt, do_opt, n_stats > 0))
+
+    def _run_step(self, n: int, slot: "_Slot", head: tuple, enqueue, grad_scale: Optional[float] = None,
+                  skip_ptr=None) -> None:
+        """One optimizer step that consumes n views, whose forward runs on `slot`'s frame.  The schedules come from
+        batch_events and batch_densify_events.  enqueue(do_opt, n_stats) enqueues the iteration with no wait, its
+        backward adding the densification statistics of its first n_stats views; it is launched eagerly or replayed
+        from the graph cached under `head` plus the state a graph bakes in.  An iteration that densifies or resets the
+        opacity runs eagerly without its update, and Adam follows the event with grad_scale and skip_ptr (None:
+        _launch_adam's defaults, read after the event has rebuilt the buffers)."""
+        c = self.cfg
+        ev = batch_events(c, self.iteration, n)
+        de = dict(n_stats=0, densify=False, reset=False, size_threshold=None)
+        if self._stats is not None:
+            de = batch_densify_events(c, self.iteration, n, self.white_background)
+        n_stats = de["n_stats"]
+        self.iteration = ev["iteration"]
+        if ev["sh_up"]:
+            self.active_sh_degree = min(self.active_sh_degree + 1, c.max_sh_degree)     # oneupSHdegree
+        do_opt = ev["do_opt"]
+        if de["densify"] or de["reset"]:
             # train.py:201-211: densify / reset between the backward and the optimizer step, eagerly (the optimizer's
-            # tensor set differs); the replaced tensors take no step in this iteration
-            self._settled(lambda: self._enqueue_iteration(view, gt, False, stats))
+            # tensor set differs); the replaced tensors take no step.  densify_and_prune rebuilds the buffers and the
+            # slots (`slot` stays alive here).
+            self._settled(lambda: enqueue(False, n_stats), batch=slot)
             skip = set()
-            if densify_now:
-                size = c.size_threshold if it > c.opacity_reset_interval else None
-                self.densify_and_prune(c.densify_grad_threshold, c.min_opacity, self.scene_extent, size,
+            if de["densify"]:
+                self.densify_and_prune(c.densify_grad_threshold, c.min_opacity, self.scene_extent, de["size_threshold"],
                                        c.densify_clone_split, self.densify_generator)
-                self.densified_at.append(it)
+                self.densified_at.append(self.iteration)
                 skip.update(name for name, _ in SEGMENTS)
-            if reset_now:
+            if de["reset"]:
                 self.reset_opacity()
-                self.reset_at.append(it)
+                self.reset_at.append(self.iteration)
                 skip.add("opacity")
             if do_opt:
-                self.optimizer_step(skip=[name for name, _ in SEGMENTS if name in skip])
+                skip = [name for name, _ in SEGMENTS if name in skip]
+                self._advance(skip)
+                self._launch_adam(grad_scale, skip, skip_ptr)
         else:
             if do_opt:
-                self._advance()        # once per iteration: a repeat after an overflow takes the same step
-            enqueue = self._replay if self.use_graph and self.cap > 0 else self._enqueue_iteration
-            self._settled(lambda: enqueue(view, gt, do_opt, stats))
-        # crossing a multiple of the interval (with G ranks `iteration` advances by G per step).  The SH-degree, do_opt
-        # and 3D-filter rules of this method are also written out in batch_events (step_batch); keep the two alike.
-        if self.filt is not None and self.iteration // c.mip_filter3d_interval > before // c.mip_filter3d_interval and \
-                self.iteration < c.iterations - 100:
+                self._advance()        # once per step: a repeat after an overflow takes the same step
+            if self.use_graph and slot.frame.cap > 0:
+                run = lambda: self._replay(head + (do_opt, self.active_sh_degree, slot.frame.cap, self.exact_cull,
+                                                   n_stats), slot, lambda: enqueue(do_opt, n_stats))
+            else:
+                run = lambda: enqueue(do_opt, n_stats)
+            self._settled(run, batch=slot)
+        if self.filt is not None and ev["mip"]:
             self.compute_filter_3D()
             self.mip_recomputed_at.append(self.iteration)
 
@@ -708,55 +748,19 @@ class JointTrainer:
                                  f"got {getattr(gts, 'dtype', type(gts))} {tuple(getattr(gts, 'shape', ()))} on "
                                  f"{getattr(gts, 'device', None)}")
             target, rows = gts.contiguous(), list(range(V))
-        c = self.cfg
         b = self._batch_scratch(V)
         # the view ids and target rows reach the (possibly captured) iteration through device memory
         b.sel.copy_(torch.tensor([views, rows], dtype=torch.int64, pin_memory=True), non_blocking=True)
-        de = dict(n_stats=0, densify=False, reset=False, size_threshold=None)
-        if self._stats is not None:
-            de = batch_densify_events(c, self.iteration, V, self.white_background)
-        n_stats = de["n_stats"]
-        ev = batch_events(c, self.iteration, V)
-        self.iteration = ev["iteration"]
-        if ev["sh_up"]:
-            self.active_sh_degree = min(self.active_sh_degree + 1, c.max_sh_degree)     # oneupSHdegree
-        do_opt = ev["do_opt"]
-        if de["densify"] or de["reset"]:
-            # as in step(): densify / reset between the backward and the optimizer step, eagerly; the replaced tensors
-            # take no step.  densify_and_prune rebuilds the buffers and drops the batch scratch (b stays alive here).
-            self._settled(lambda: self._enqueue_batch(b, target, False, n_stats), batch=b)
-            skip = set()
-            if de["densify"]:
-                self.densify_and_prune(c.densify_grad_threshold, c.min_opacity, self.scene_extent, de["size_threshold"],
-                                       c.densify_clone_split, self.densify_generator)
-                self.densified_at.append(self.iteration)
-                skip.update(name for name, _ in SEGMENTS)
-            if de["reset"]:
-                self.reset_opacity()
-                self.reset_at.append(self.iteration)
-                skip.add("opacity")
-            if do_opt:
-                skip = [name for name, _ in SEGMENTS if name in skip]
-                self._advance(skip)
-                self._launch_adam(1.0 / V, skip, skip_ptr=b.frame.word(ST_OVERFLOW).data_ptr())
-        else:
-            if do_opt:
-                self._advance()        # once per step: a repeat after an overflow takes the same step
-            enqueue = self._replay_batch if self.use_graph and b.frame.cap > 0 else self._enqueue_batch
-            self._settled(lambda: enqueue(b, target, do_opt, n_stats), batch=b)
+        self._run_step(V, b, ("batch", V, target.data_ptr()),
+                       lambda do_opt, n_stats: self._enqueue_batch(b, target, do_opt, n_stats),
+                       1.0 / V, b.frame.word(ST_OVERFLOW).data_ptr())
         self._batch_sums = b.sums
-        if self.filt is not None and ev["mip"]:
-            self.compute_filter_3D()
-            self.mip_recomputed_at.append(self.iteration)
 
     def batch_loss_values(self) -> torch.Tensor:
         """loss_value() of each view of the last step_batch call, [V] on the device (views in the call's order)."""
         if self._batch_sums is None:
             raise _lib.GsbError("batch_loss_values: no step_batch call since the trainer was built, resized or restored")
-        s = self._batch_sums
-        n = 3 * self.H * self.W
-        lam = self.cfg.lambda_dssim
-        return (1.0 - lam) * s[:, 0] / n + lam * (1.0 - s[:, 1] / n)
+        return self._loss(self._batch_sums)
 
     # ---- evaluation (train.py:256-290 training_report; DESIGN.md section 4.11) ----------------------------------
     def evaluate(self, views: Optional[Sequence[int]] = None, poses: Optional[torch.Tensor] = None,
@@ -810,8 +814,7 @@ class JointTrainer:
             with torch.no_grad():      # a restored pose table may carry requires_grad from the checkpoint's Parameter
                 pose_rows = self.poses.detach()[torch.tensor(views, dtype=torch.int64, device=dev)].contiguous()
         step = V if max_batch is None else int(max_batch)
-        cam = self.ident.camera(self.active_sh_degree, 16, self.exact_cull)
-        p = self.params
+        cam = self._camera()
         host_status = torch.zeros(ST_WORDS, dtype=torch.int32).pin_memory()
         sums, ovf = [], torch.zeros(1, dtype=torch.int32, device=dev)
         fr = None
@@ -821,8 +824,7 @@ class JointTrainer:
             if fr is None or fr.views != v1 - v0:
                 fr = None
                 fr = Frame(dev, self.P, self.W, self.H, views=v1 - v0)
-            g = gaussians(self.P, *(self.view(p, n) for n in ("xyz", "rotation", "scaling", "opacity", "f_dc",
-                                                               "f_rest")), pr)
+            g = self._gauss(pr)
             fr.preprocess_batch(cam, g, pr, host_status, self.filt)
             torch.cuda.current_stream(dev).synchronize()
             fr.alloc_binning(max(1, read_R(host_status)))
@@ -833,17 +835,22 @@ class JointTrainer:
             raise _lib.GsbError("evaluate: a tile list outgrew the binning buffer sized from the preprocess count")
         return metrics_from_sums(torch.cat(sums), self.H, self.W)
 
-    class _BatchScratch:
-        """step_batch's buffers for V views: the batch Frame with its own pinned status slot (its forwards have their own
-        serial numbers, see _settle), sel [2, V] (view ids, target rows; uploaded per call), the gathered poses and their
-        gradients [V, 7], dL/dimage, loss maps and per-view loss sums."""
+    class _Slot:
+        """Where a forward runs: a Frame, the pinned [2, ST_WORDS] buffer its status words are copied to ([0] after
+        preprocess, [1] after render) and the count of its forwards.  Each frame numbers its forwards in its own status
+        words and copies them to its own pinned buffer, so a serial number is only ever compared with the count of the
+        frame that wrote it (_settle).  V None: step()'s single view.  Otherwise step_batch's buffers for V views:
+        sel [2, V] (view ids, target rows; uploaded per call), the gathered poses and their gradients [V, 7],
+        dL/dimage, loss maps and per-view loss sums."""
 
-        def __init__(self, dev, P, W, H, V):
+        def __init__(self, dev, P, W, H, V=None):
             self.V = V
             self.frame = Frame(dev, P, W, H, views=V)
             self.frame.status.zero_()          # the forward serial number lives in these words
             self.fwd_count = 0
-            self.host_status = torch.zeros(2, ST_WORDS, dtype=torch.int32).pin_memory()   # [0] preprocess, [1] render
+            self.host_status = torch.zeros(2, ST_WORDS, dtype=torch.int32).pin_memory()
+            if V is None:
+                return
             self.sel = torch.zeros(2, V, dtype=torch.int64, device=dev)
             self.rows = torch.zeros(V, dtype=torch.int32, device=dev)
             self.poses = torch.zeros(V, 7, dtype=torch.float32, device=dev)
@@ -852,16 +859,17 @@ class JointTrainer:
             self.maps = torch.empty(3, V, 3, H, W, dtype=torch.float32, device=dev)
             self.sums = torch.zeros(V, 2, dtype=torch.float64, device=dev)
 
-    def _batch_scratch(self, V: int) -> "_BatchScratch":
-        """The scratch for V views; one set is held at a time (a call with another V replaces it, and with it the
-        graphs captured over it)."""
+    def _batch_scratch(self, V: int) -> "_Slot":
+        """The slot for V views; one is held at a time (a call with another V replaces it, and with it the graphs
+        captured over it).  One graph per (V, target buffer, do_opt, active SH degree, capacity, exact_cull, n_stats)
+        serves every choice of views: they are read from sel."""
         if self._batch is None or self._batch.V != V:
             self._batch = None
             self._graphs = {k: g for k, g in self._graphs.items() if k[0] != "batch"}
-            self._batch = self._BatchScratch(self.dev, self.P, self.W, self.H, V)
+            self._batch = self._Slot(self.dev, self.P, self.W, self.H, V)
         return self._batch
 
-    def _enqueue_batch(self, b: "_BatchScratch", target: torch.Tensor, do_opt: bool, n_stats: int = 0) -> None:
+    def _enqueue_batch(self, b: "_Slot", target: torch.Tensor, do_opt: bool, n_stats: int = 0) -> None:
         """One step_batch iteration with no wait, launched eagerly or captured into a graph: gather the pose rows,
         forward, loss, backward summed over the views (and the densification statistics of views 0..n_stats-1),
         scatter dL/dpose into pose_grad, the test hook, and (do_opt) the update, gated on the batch's binning-overflow
@@ -873,19 +881,8 @@ class JointTrainer:
         b.rows.copy_(b.sel[1])
         with torch.no_grad():          # a restored pose table may carry requires_grad from the checkpoint's Parameter
             torch.index_select(self.poses, 0, idx, out=b.poses)
-        cam = self.ident.camera(self.active_sh_degree, 16, self.exact_cull)
-        p = self.params
-        g = gaussians(self.P, *(self.view(p, n) for n in ("xyz", "rotation", "scaling", "opacity", "f_dc", "f_rest")),
-                      b.poses)
-        fr.preprocess_batch(cam, g, b.poses, b.host_status[0], self.filt)
-        if not torch.cuda.is_current_stream_capturing():
-            b.fwd_count += 1
-            self._polling = False
-            self._ev_pre.record()
-            if fr.cap == 0:                           # very first forward: size the buffer from the real count
-                self._ev_pre.synchronize()
-                self._size_binning(read_R(b.host_status[0]), fr)
-        fr.render_batch(cam, b.host_status[1])
+        cam, g = self._camera(), self._gauss(b.poses)
+        self._forward(b, cam, g, b.poses)
         b.sums.zero_()
         check(L.gsb_loss_forward_batch(V, 3, self.H, self.W, fr.color.data_ptr(), target.data_ptr(),
                                        b.rows.data_ptr(), b.sums.data_ptr(), b.maps.data_ptr(), st),
@@ -893,18 +890,10 @@ class JointTrainer:
         check(L.gsb_loss_backward_batch(V, 3, self.H, self.W, fr.color.data_ptr(), target.data_ptr(),
                                         b.rows.data_ptr(), b.maps.data_ptr(), float(self.cfg.lambda_dssim),
                                         b.dL.data_ptr(), st), "gsb_loss_backward_batch")
-        gr = GsbGrads()
-        gd = self.grads
-        gr.dL_dmeans3D = self.view(gd, "xyz").data_ptr()
-        gr.dL_dscales = self.view(gd, "scaling").data_ptr()
-        gr.dL_drotations = self.view(gd, "rotation").data_ptr()
-        gr.dL_dopacities = self.view(gd, "opacity").data_ptr()
-        gr.dL_dsh_dc = self.view(gd, "f_dc").data_ptr()
-        gr.dL_dsh_rest = self.view(gd, "f_rest").data_ptr()
         st = None
         if n_stats > 0:
             st = densify_stats(fr.radii, self._stats[0], self._stats[1], self._stats[2])
-        fr.backward_batch(cam, g, b.poses, b.dL, gr, b.dpose, self.filt, st, n_stats)
+        fr.backward_batch(cam, g, b.poses, b.dL, self._grads(), b.dpose, self.filt, st, n_stats)
         self.pose_grad.zero_()
         with torch.no_grad():
             self.pose_grad.index_copy_(0, idx, b.dpose)
@@ -912,23 +901,6 @@ class JointTrainer:
             self._after_backward()
         if do_opt:
             self._launch_adam(1.0 / V, skip_ptr=fr.word(ST_OVERFLOW).data_ptr())
-
-    def _replay_batch(self, b: "_BatchScratch", target: torch.Tensor, do_opt: bool, n_stats: int = 0) -> None:
-        """Replay (capturing on first use) the CUDA graph of _enqueue_batch: one graph per (V, target buffer, do_opt,
-        active SH degree, capacity, exact_cull, n_stats) serves every choice of views (they are read from b.sel)."""
-        key = ("batch", b.V, target.data_ptr(), do_opt, self.active_sh_degree, b.frame.cap, self.exact_cull, n_stats)
-        g = self._graphs.get(key)
-        if g is None:
-            if len(self._graphs) > 64:
-                self._graphs.clear()
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._enqueue_batch(b, target, do_opt, n_stats)
-            self._graphs[key] = g
-        b.fwd_count += 1
-        self._polling = True
-        g.replay()
 
     # ---- densify / prune / opacity reset on the flat buffers (SURVEY.md section 8 row f4) -----------------------
     # Semantics of scene/gaussian_model.py: prune_points (:359-374) keeps the surviving rows of every
@@ -958,14 +930,12 @@ class JointTrainer:
         if self._stats is not None:
             self._stats = torch.zeros(3, new_P, dtype=torch.float32, device=self.dev) if stats is None else \
                 stats.contiguous()
-        self.frame = Frame(self.dev, new_P, self.W, self.H)   # the next forward sizes its binning buffer
+        self._single = self._Slot(self.dev, new_P, self.W, self.H)   # the next forward sizes its binning buffer
         self._batch = None
         self._batch_sums = None
         self._mip_setup()
         self._keep = None
         self._graphs.clear()
-        self.frame.status.zero_()
-        self._fwd_count = 0
 
     def _set_per_point_lr(self, values: Optional[torch.Tensor]) -> None:
         """The xyz tensor's per-point learning-rate multiplier [P] (None: off), padded with ones over the xyz

@@ -1,5 +1,6 @@
-"""Densify with batched training, host side (no GPU): batch_densify_events against a per-iteration restatement of
-step()'s densify / reset rules, and the batched statistics entry point is exported and declared."""
+"""Densify with batched training, host side (no GPU): batch_densify_events, which step() and step_batch both run,
+against a per-iteration restatement of train.py's densify / reset rules, and the batched statistics entry point is
+exported and declared."""
 import os
 import re
 
@@ -21,7 +22,7 @@ def test_batched_statistics_symbol_exported_and_declared():
 
 
 def _per_iteration(cfg, before, V, white):
-    """step()'s inline rules applied to each iteration j the step covers, then merged: the statistics views, whether
+    """train.py's rules applied to each iteration j the step covers, then merged: the statistics views, whether
     any j densifies or resets, and the size threshold of the last densify point."""
     stats, dens, reset = [], [], False
     for j in range(before + 1, before + V + 1):
@@ -73,7 +74,7 @@ def test_batch_events_equal_the_per_iteration_rules():
 
 
 def test_one_view_is_step():
-    """V = 1 is the rule step() writes out: statistics while iteration < densify_until_iter, the densify and reset
+    """V = 1, step()'s case, is train.py's rule: statistics while iteration < densify_until_iter, the densify and reset
     iterations themselves, and size_threshold past the first reset interval."""
     c = CONFIGS[0]
     assert batch_densify_events(c, 9, 1, False) == dict(n_stats=1, densify=True, reset=False, size_threshold=None)
