@@ -312,6 +312,13 @@ GSB_API int gsb_image_metrics_batch(int32_t V, int32_t C, int32_t H, int32_t W, 
                                     const int32_t* gt_row, int32_t mode, double* out, void* scratch,
                                     size_t scratch_bytes, gsb_stream_t stream);
 
+/* ---- 8-bit frames (render.py:91-93, torchvision.utils.save_image of one [3, H, W] image) ----
+ * img [V, 3, H, W] fp32 -> out [V, H, W, 3] uint8: uint8(clamp(x*255 + 0.5, 0, 255)) per value, each operation rounded
+ * as torch rounds it, truncating (the level GSB_METRIC_PNG8 compares), with the channels interleaved per pixel as PIL
+ * takes an RGB image.  One memory-bound pass, 12 bytes read and 3 written per pixel.  V must not exceed 65535 and
+ * H * W must fit in int32. */
+GSB_API int gsb_frames_u8_batch(int32_t V, int32_t H, int32_t W, const float* img, uint8_t* out, gsb_stream_t stream);
+
 /* Per-point Adam (scene/per_point_adam.py:34-98), n tensors in one launch. */
 typedef struct GsbAdamTensor {
   float* param;

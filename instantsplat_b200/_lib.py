@@ -80,7 +80,8 @@ EXPORTS = ("gsb_geom_bytes", "gsb_binning_bytes", "gsb_image_bytes", "gsb_prepro
            "gsb_geom_bytes_batch", "gsb_binning_bytes_batch", "gsb_image_bytes_batch", "gsb_status_device_batch",
            "gsb_preprocess_batch", "gsb_render_batch", "gsb_backward_pose_batch", "gsb_l1_mask_fwd_bwd_batch",
            "gsb_track_step_batch", "gsb_backward_batch", "gsb_loss_forward_batch", "gsb_loss_backward_batch",
-           "gsb_backward_batch_stats", "gsb_image_metrics_scratch_bytes", "gsb_image_metrics_batch")
+           "gsb_backward_batch_stats", "gsb_image_metrics_scratch_bytes", "gsb_image_metrics_batch",
+           "gsb_frames_u8_batch")
 KERNEL_IDS = ("preprocess", "sort_depth", "scan", "duplicate", "sort_tile", "gather", "blend_fwd", "blend_bwd",
               "preprocess_bwd", "loss_fwd", "loss_bwd", "adam")
 
@@ -166,9 +167,10 @@ def lib() -> ctypes.CDLL:
     L.gsb_image_metrics_scratch_bytes.restype = sz
     L.gsb_image_metrics_scratch_bytes.argtypes = [i32, i32, i32, i32]
     L.gsb_image_metrics_batch.argtypes = [i32, i32, i32, i32, vp, vp, vp, i32, vp, vp, sz, vp]
+    L.gsb_frames_u8_batch.argtypes = [i32, i32, i32, vp, vp, vp]
     for f in ("gsb_preprocess_batch", "gsb_render_batch", "gsb_backward_pose_batch", "gsb_l1_mask_fwd_bwd_batch",
               "gsb_track_step_batch", "gsb_backward_batch", "gsb_loss_forward_batch", "gsb_loss_backward_batch",
-              "gsb_backward_batch_stats", "gsb_image_metrics_batch"):
+              "gsb_backward_batch_stats", "gsb_image_metrics_batch", "gsb_frames_u8_batch"):
         getattr(L, f).restype = ctypes.c_int
     L.gsb_adam_step_gated.argtypes = [i32, ctypes.POINTER(GsbAdamTensor), vp, vp, vp]
     L.gsb_adam_step_gated.restype = ctypes.c_int

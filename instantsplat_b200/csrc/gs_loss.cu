@@ -14,6 +14,7 @@
 //
 // The evaluation metrics (gsb_image_metrics_batch: train.py's training_report, metrics.py) are the same forward on
 // clamped or 8-bit-quantised inputs, with per-CTA partial sums and a fixed-order reduction instead of atomics.
+// gsb_frames_u8_batch writes that 8-bit quantisation out as interleaved RGB frames (render.py's save_image).
 #include <cuda_runtime.h>
 #include <stdio.h>
 
@@ -74,13 +75,16 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
 // uint8(clamp(x * 255 + 0.5, 0, 255)) / 255 in fp32, truncating, so exact ties round up.
 enum { kInRaw = 0, kInClamp = GSB_METRIC_CLAMP, kInPng8 = GSB_METRIC_PNG8 };
 
+// save_image's 8-bit level of x as a float in {0, ..., 255}: x.mul(255).add_(0.5).clamp_(0, 255).to(uint8) with each
+// operation rounded as torch rounds it (no FMA contraction), truncating, so exact ties round up.  NaN gives 0.
+__device__ __forceinline__ float png8_level(float x) {
+  return truncf(fminf(fmaxf(__fadd_rn(__fmul_rn(x, 255.f), 0.5f), 0.f), 255.f));
+}
+
 template <int kIn>
 __device__ __forceinline__ float metric_input(float x) {
   if constexpr (kIn == kInClamp) return fminf(fmaxf(x, 0.f), 1.f);
-  if constexpr (kIn == kInPng8) {
-    const float q = truncf(fminf(fmaxf(__fadd_rn(__fmul_rn(x, 255.f), 0.5f), 0.f), 255.f));
-    return __fdiv_rn(q, 255.f);
-  }
+  if constexpr (kIn == kInPng8) return __fdiv_rn(png8_level(x), 255.f);
   return x;
 }
 
@@ -391,6 +395,42 @@ k_metrics_reduce(int C, int T, const double* __restrict__ partials, double* __re
   }
 }
 
+// save_image's 8-bit frames: img [V, 3, H, W] fp32 -> out [V, H, W, 3] uint8, png8_level of every value with the three
+// channels interleaved per pixel.  Grid (ceil(H W / 1024), V): thread t of view v = blockIdx.y takes the 4 pixels
+// p = 4t .. 4t + 3 of that view.  kVec (H W % 4 == 0, img 16-byte and out 4-byte aligned): one float4 load per channel
+// plane and the 12 interleaved bytes as three uint32 stores; 12 bytes read and 3 written per pixel, nothing else.
+// Otherwise the planes of a view start at misaligned addresses: scalar loads and byte stores, stopping at the view's
+// last pixel (the tail of a group of 4).
+constexpr int kFrameThreads = 256;
+
+__device__ __forceinline__ uint32_t png8_byte(float x) { return __float2uint_rz(png8_level(x)); }
+
+template <bool kVec>
+__global__ void __launch_bounds__(kFrameThreads)
+k_frames_u8(int HW, const float* __restrict__ img, uint8_t* __restrict__ out) {
+  const int p = 4 * (blockIdx.x * kFrameThreads + threadIdx.x);
+  if (p >= HW) return;
+  const size_t pix = (size_t)blockIdx.y * HW + p;            // first pixel of the group in [V, H, W]
+  const float* src = img + (size_t)blockIdx.y * 3 * HW + p;   // its red value
+  if constexpr (kVec) {
+    const float4 r = __ldg(reinterpret_cast<const float4*>(src));
+    const float4 g = __ldg(reinterpret_cast<const float4*>(src + HW));
+    const float4 b = __ldg(reinterpret_cast<const float4*>(src + 2 * (size_t)HW));
+    uint32_t* dst = reinterpret_cast<uint32_t*>(out + 3 * pix);   // little endian: byte k of the group is bits 8k
+    dst[0] = png8_byte(r.x) | png8_byte(g.x) << 8 | png8_byte(b.x) << 16 | png8_byte(r.y) << 24;
+    dst[1] = png8_byte(g.y) | png8_byte(b.y) << 8 | png8_byte(r.z) << 16 | png8_byte(g.z) << 24;
+    dst[2] = png8_byte(b.z) | png8_byte(r.w) << 8 | png8_byte(g.w) << 16 | png8_byte(b.w) << 24;
+  } else {
+    const int n = min(4, HW - p);
+    for (int k = 0; k < n; ++k) {
+      uint8_t* d = out + 3 * (pix + k);
+      d[0] = (uint8_t)png8_byte(__ldg(src + k));
+      d[1] = (uint8_t)png8_byte(__ldg(src + HW + k));
+      d[2] = (uint8_t)png8_byte(__ldg(src + 2 * (size_t)HW + k));
+    }
+  }
+}
+
 int check(cudaError_t e, const char* what) {
   if (e == cudaSuccess) return GSB_OK;
   char buf[256];
@@ -528,4 +568,22 @@ extern "C" GSB_API int gsb_image_metrics_batch(int32_t V, int32_t C, int32_t H, 
   if (rc != GSB_OK) return rc;
   k_metrics_reduce<<<V, kReduceThreads, 0, st>>>(C, (int)(grid.x * grid.y), part, out);
   return check(cudaGetLastError(), "k_metrics_reduce");
+}
+
+extern "C" GSB_API int gsb_frames_u8_batch(int32_t V, int32_t H, int32_t W, const float* img, uint8_t* out,
+                                           gsb_stream_t stream) {
+  if (V <= 0 || V > 65535 || H <= 0 || W <= 0 || (int64_t)H * W > (int64_t)INT32_MAX - 3 || !img || !out) {
+    gsb_set_error("gsb_frames_u8_batch: bad argument");
+    return GSB_ERR_INVALID;
+  }
+  const int HW = H * W;
+  const bool vec = HW % 4 == 0 && reinterpret_cast<uintptr_t>(img) % 16 == 0 && reinterpret_cast<uintptr_t>(out) % 4 == 0;
+  dim3 grid((unsigned)((HW + 4 * kFrameThreads - 1) / (4 * kFrameThreads)), (unsigned)V);
+  cudaStream_t st = (cudaStream_t)stream;
+  gsb_count_launch(1);
+  if (vec)
+    k_frames_u8<true><<<grid, kFrameThreads, 0, st>>>(HW, img, out);
+  else
+    k_frames_u8<false><<<grid, kFrameThreads, 0, st>>>(HW, img, out);
+  return check(cudaGetLastError(), "k_frames_u8");
 }
