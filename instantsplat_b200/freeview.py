@@ -32,7 +32,7 @@ import os
 import sys
 from collections import deque
 from concurrent.futures import ThreadPoolExecutor
-from typing import Iterable, Iterator, Optional, Tuple
+from typing import Iterable, Iterator, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -212,10 +212,12 @@ def _save_png(img: np.ndarray, path: str) -> None:
     Image.fromarray(img).save(path)                       # what save_image does with the uint8 HWC array
 
 
-def write_pngs(frames: Iterable[Tuple[int, np.ndarray]], folder: str, workers: Optional[int] = None) -> int:
-    """Writes every frame of (first_index, uint8 [B, H, W, 3]) chunks to folder/{idx:05d}.png, the file
-    torchvision.utils.save_image writes for that image, encoding on a pool of `workers` threads (None: up to 8; Pillow's
-    encoder releases the GIL).  At most 4 x workers frames wait for the encoder.  Returns the number of files."""
+def write_pngs(frames: Iterable[Tuple[int, np.ndarray]], folder: str, workers: Optional[int] = None,
+               names: Optional[Sequence[str]] = None) -> int:
+    """Writes every frame of (first_index, uint8 [B, H, W, 3]) chunks to folder/{idx:05d}.png (or folder/names[idx]),
+    the file torchvision.utils.save_image writes for that image, encoding on a pool of `workers` threads (None: up to 8;
+    Pillow's encoder releases the GIL).  At most 4 x workers frames wait for the encoder.  Returns the number of
+    files."""
     os.makedirs(folder, exist_ok=True)
     workers = min(8, os.cpu_count() or 1) if workers is None else int(workers)
     if workers < 1:
@@ -224,7 +226,8 @@ def write_pngs(frames: Iterable[Tuple[int, np.ndarray]], folder: str, workers: O
     with ThreadPoolExecutor(max_workers=workers) as pool:
         for first, chunk in frames:
             for i in range(chunk.shape[0]):
-                pending.append(pool.submit(_save_png, chunk[i], os.path.join(folder, f"{first + i:05d}.png")))
+                name = f"{first + i:05d}.png" if names is None else names[first + i]
+                pending.append(pool.submit(_save_png, chunk[i], os.path.join(folder, name)))
                 count += 1
             while len(pending) > 4 * workers:
                 pending.popleft().result()
@@ -272,7 +275,6 @@ def load(source_path: str, model_path: str, n_views: int, iteration: int = -1, w
     pose/ours_<it>/pose_optimized.npy, it).  iteration -1: the largest saved one, for the model and the poses alike
     (render.py looks the poses up under the literal `ours_-1`).  Like render.py, no Mip-Splatting filters: a ply's
     filter_3D is not used (build a PoseTracker with kernel_size and filter_3D and call frames_u8 for that)."""
-    from .scene_io import load_gaussians_ply
     it = max_iteration(model_path) if int(iteration) == -1 else int(iteration)
     ply = os.path.join(model_path, "point_cloud", f"iteration_{it}", "point_cloud.ply")
     npy = os.path.join(model_path, "pose", f"ours_{it}", "pose_optimized.npy")
@@ -280,6 +282,14 @@ def load(source_path: str, model_path: str, n_views: int, iteration: int = -1, w
         if not os.path.isfile(f):
             raise FileNotFoundError(f"{f} not found")
     W, H, fovx, fovy = intrinsics(source_path, n_views)
+    return load_tracker(ply, W, H, fovx, fovy, white_background, device), np.load(npy), it
+
+
+def load_tracker(ply: str, width: int, height: int, fovx: float, fovy: float, white_background: bool = False,
+                 device="cuda") -> PoseTracker:
+    """A PoseTracker over a saved point_cloud.ply as render.py renders it: the SH degree from the file's coefficient
+    count, a black or white background, no Mip-Splatting filters."""
+    from .scene_io import load_gaussians_ply
     g = load_gaussians_ply(ply)
     M = 1 + g["f_rest"].shape[1]
     deg = int(round(M ** 0.5)) - 1
@@ -287,9 +297,8 @@ def load(source_path: str, model_path: str, n_views: int, iteration: int = -1, w
         raise ValueError(f"{ply}: {M} SH coefficients per channel is not a square")
     t = lambda k: torch.from_numpy(np.ascontiguousarray(g[k]))
     bg = torch.ones(3) if white_background else torch.zeros(3)
-    tracker = PoseTracker(t("xyz"), t("rotation"), t("scaling"), t("opacity"), t("f_dc"), t("f_rest"), W, H, fovx,
-                          fovy, bg=bg, sh_degree=deg, device=device)
-    return tracker, np.load(npy), it
+    return PoseTracker(t("xyz"), t("rotation"), t("scaling"), t("opacity"), t("f_dc"), t("f_rest"), width, height, fovx,
+                       fovy, bg=bg, sh_degree=deg, device=device)
 
 
 def main(argv=None) -> int:

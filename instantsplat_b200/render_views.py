@@ -1,0 +1,143 @@
+"""The training- and test-view renders of a trained model: stages 3 and 4 of InstantSplat's scripts/run_eval.sh,
+render.py's render_sets (render.py:189-248) with its branch logic, on the GPU.
+
+  * no --eval (render_set "train", render.py:204-216): the training views of source/sparse_<n>/0 (sorted by
+    image_name) at the poses of pose/ours_<it>/pose_optimized.npy, row i to view i as loadCameras pairs them, turned
+    into render() 7-vectors by freeview.poses_from_w2c.  Writes train/ours_<it>/renders/{idx:05d}.png and
+    gt/{idx:05d}.png.
+  * --eval (render_set_optimize, render.py:99-170): the test views of source/sparse_<n>/1, each starting from
+    get_tensor_from_camera of its own world_view_transform (the same conversion), are tracked for
+    --optim_test_pose_iter iterations in PoseTracker.optimize_batch (render.py's Adam groups, weight decay, cosine
+    schedule and best-candidate rule; each view bit-identical to tracking it alone), then rendered at their best
+    poses.  Writes test/ours_<it>/renders/<image_name>.png and gt/<image_name>.png.
+  * --infer_video without --eval: the fly-through, freeview.main.
+
+Renders are save_image's 8-bit frames (freeview.frames_u8).  A ground-truth file is save_image of the loaded image,
+uint8 -> /255 -> uint8; that round trip is the identity on all 256 levels (checked once, gt_round_trip_is_identity),
+so the gt PNGs are encoded from the decoded bytes.  Every PNG is encoded on freeview.write_pngs' thread pool.
+
+The background is black, or white with --white_background; the SH degree is the ply's.  The model's cfg_args is not
+read: render.py's get_combined_args lets every command-line value that is not None win, and ModelParams is built
+with sentinel=False, so its defaults (white_background False included) always override the saved config there too.
+
+    python -m instantsplat_b200.render_views -s SOURCE -m MODEL --n_views N --iterations IT [--eval] [--infer_video]
+        [--optim_test_pose_iter 500] [--white_background] [--max_batch B] [--workers K]
+"""
+from __future__ import annotations
+
+import argparse
+import os
+import sys
+from typing import Optional
+
+import numpy as np
+import torch
+
+from . import freeview
+from .scene_io import Views, load_views
+from .tracking import PoseTracker
+
+
+def gt_round_trip_is_identity() -> bool:
+    """save_image(PILtoTorch(k)) == k for every 8-bit level k: uint8(clamp(fp32(k / 255) * 255 + 0.5, 0, 255))."""
+    k = torch.arange(256, dtype=torch.uint8)
+    x = k / 255.0
+    return torch.equal(x.mul(255).add_(0.5).clamp_(0, 255).to(torch.uint8), k)
+
+
+def gt_images(views: Views, device) -> torch.Tensor:
+    """The views' images as loadCam hands them to render.py: [V, 3, H, W] fp32 k / 255 on the device."""
+    u8 = torch.from_numpy(np.ascontiguousarray(views.images)).to(device)
+    return (u8 / 255.0).permute(0, 3, 1, 2).contiguous()
+
+
+def tracker_for(model_path: str, it: int, views: Views, white_background: bool = False, device="cuda") -> PoseTracker:
+    ply = os.path.join(model_path, "point_cloud", f"iteration_{it}", "point_cloud.ply")
+    if not os.path.isfile(ply):
+        raise FileNotFoundError(f"{ply} not found")
+    return freeview.load_tracker(ply, views.width, views.height, views.fovx, views.fovy, white_background, device)
+
+
+def _write_gt(views: Views, folder: str, names, workers: Optional[int]) -> None:
+    if not gt_round_trip_is_identity():
+        raise RuntimeError("the 8-bit -> fp32 -> 8-bit round trip is not the identity; gt files cannot be copied")
+    freeview.write_pngs([(0, views.images)], folder, workers, names)
+
+
+def render_train(tracker: PoseTracker, views: Views, w2c_opt, out_dir: str, max_batch: Optional[int] = None,
+                 workers: Optional[int] = None) -> torch.Tensor:
+    """render_set("train"): views at the optimised world-to-camera matrices w2c_opt [V, 4, 4] (pose_optimized.npy,
+    one row per view) -> out_dir/renders/{idx:05d}.png and out_dir/gt/{idx:05d}.png.  Returns the 7-vectors [V, 7]."""
+    w2c_opt = np.asarray(w2c_opt)
+    if w2c_opt.ndim != 3 or w2c_opt.shape[0] != len(views):
+        raise ValueError(f"render_train: {w2c_opt.shape[0] if w2c_opt.ndim == 3 else w2c_opt.shape} optimised poses "
+                         f"for {len(views)} training views; loadCameras pairs them one to one")
+    poses = freeview.poses_from_w2c(w2c_opt)
+    freeview.write_pngs(freeview.frames_u8(tracker, poses, max_batch), os.path.join(out_dir, "renders"), workers)
+    _write_gt(views, os.path.join(out_dir, "gt"), None, workers)
+    return poses
+
+
+def track(tracker: PoseTracker, views: Views, num_iter: int = 500, max_batch: Optional[int] = None) -> torch.Tensor:
+    """render.py:113-161 for every test view: best poses [V, 7] (CPU fp32), from the views' own 7-vectors, tracked in
+    PoseTracker.optimize_batch chunks of max_batch views (None: all at once)."""
+    init = freeview.poses_from_w2c(views.w2c)
+    best, _ = tracker.optimize_batch(init, gt_images(views, tracker.dev), num_iter=num_iter, max_batch=max_batch)
+    return best
+
+
+def render_test(tracker: PoseTracker, views: Views, out_dir: str, num_iter: int = 500, max_batch: Optional[int] = None,
+                workers: Optional[int] = None) -> torch.Tensor:
+    """render_set_optimize: track, then out_dir/renders/<image_name>.png at the best poses and out_dir/gt/<image_name>.png.
+    Returns the best poses [V, 7]."""
+    best = track(tracker, views, num_iter, max_batch)
+    names = [n + ".png" for n in views.names]
+    freeview.write_pngs(freeview.frames_u8(tracker, best, max_batch), os.path.join(out_dir, "renders"), workers, names)
+    _write_gt(views, os.path.join(out_dir, "gt"), names, workers)
+    return best
+
+
+def main(argv=None) -> int:
+    ap = argparse.ArgumentParser(prog="python -m instantsplat_b200.render_views",
+                                 description="render.py: the training views at their optimised poses, or (--eval) "
+                                             "the test views after pose tracking")
+    ap.add_argument("-s", "--source_path", required=True)
+    ap.add_argument("-m", "--model_path", required=True)
+    ap.add_argument("--n_views", type=int, required=True)
+    ap.add_argument("--iterations", type=int, default=-1)
+    ap.add_argument("-r", "--resolution", type=int, default=-1)
+    ap.add_argument("--eval", action="store_true")
+    ap.add_argument("--infer_video", action="store_true")
+    ap.add_argument("--optim_test_pose_iter", type=int, default=500)
+    ap.add_argument("--white_background", action="store_true")
+    ap.add_argument("--max_batch", type=int, default=12,
+                    help="views per batched loop; tracking scratch is about 150 P + 44 H W bytes a view")
+    ap.add_argument("--workers", type=int, default=None, help="PNG encoder threads (default: up to 8)")
+    a = ap.parse_args(argv)
+    if a.max_batch < 1:
+        raise SystemExit("--max_batch must be at least 1")
+    if a.infer_video and not a.eval:
+        fv = ["-s", a.source_path, "-m", a.model_path, "--n_views", str(a.n_views), "--iterations", str(a.iterations),
+              "--max_batch", str(a.max_batch)] + (["--white_background"] if a.white_background else []) \
+            + ([] if a.workers is None else ["--workers", str(a.workers)])
+        return freeview.main(fv)
+    it = freeview.max_iteration(a.model_path) if a.iterations == -1 else a.iterations
+    if a.eval:
+        views = load_views(a.source_path, a.n_views, 1, a.resolution)
+        tracker = tracker_for(a.model_path, it, views, a.white_background)
+        out = os.path.join(a.model_path, "test", f"ours_{it}")
+        render_test(tracker, views, out, a.optim_test_pose_iter, a.max_batch, a.workers)
+    else:
+        npy = os.path.join(a.model_path, "pose", f"ours_{it}", "pose_optimized.npy")
+        if not os.path.isfile(npy):
+            raise FileNotFoundError(f"{npy} not found")
+        views = load_views(a.source_path, a.n_views, 0, a.resolution)
+        tracker = tracker_for(a.model_path, it, views, a.white_background)
+        out = os.path.join(a.model_path, "train", f"ours_{it}")
+        render_train(tracker, views, np.load(npy), out, a.max_batch, a.workers)
+    print(f"{len(views)} views -> {out}")
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

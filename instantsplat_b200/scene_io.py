@@ -68,8 +68,9 @@ def write_colmap_text(folder: str, width: int, height: int, fx: float, fy: float
             f.write(f"{i + 1} {vals} {i + 1} {name}\n\n")
 
 
-def read_colmap_text(folder: str) -> Tuple[Dict[int, dict], Dict[int, dict]]:
-    """Returns (cameras, images) keyed by id; same fields the reference's readers expose."""
+def read_colmap_text(folder: str, models: Tuple[str, ...] = ("PINHOLE",)) -> Tuple[Dict[int, dict], Dict[int, dict]]:
+    """Returns (cameras, images) keyed by id; same fields the reference's readers expose.  models: the camera models
+    accepted (the params are returned as listed: PINHOLE fx fy cx cy, SIMPLE_PINHOLE f cx cy)."""
     cameras, images = {}, {}
     with open(os.path.join(folder, "cameras.txt")) as f:
         for line in f:
@@ -77,8 +78,8 @@ def read_colmap_text(folder: str) -> Tuple[Dict[int, dict], Dict[int, dict]]:
             if not line or line[0] == "#":
                 continue
             e = line.split()
-            if e[1] != "PINHOLE":
-                raise ValueError("only PINHOLE cameras are supported (as in the reference)")
+            if e[1] not in models:
+                raise ValueError(f"only {' / '.join(models)} cameras are supported (as in the reference), got {e[1]}")
             cameras[int(e[0])] = dict(id=int(e[0]), model=e[1], width=int(e[2]), height=int(e[3]),
                                       params=np.array(list(map(float, e[4:]))))
     with open(os.path.join(folder, "images.txt")) as f:
@@ -94,6 +95,175 @@ def read_colmap_text(folder: str) -> Tuple[Dict[int, dict], Dict[int, dict]]:
                                  tvec=np.array(list(map(float, e[5:8]))), camera_id=int(e[8]), name=e[9])
         i += 1                                     # the POINTS2D line
     return cameras, images
+
+
+# ----------------------------------------------------------------------------------------------
+# COLMAP binary images.bin (what read_colmap_gt_pose reads for the pose errors)
+# ----------------------------------------------------------------------------------------------
+def read_colmap_images_bin(path: str) -> Dict[int, dict]:
+    """COLMAP's images.bin keyed by image id, the records of scene/colmap_loader.py's read_extrinsics_binary: id,
+    qvec (w, x, y, z) and tvec as fp64 arrays, camera_id, name, xys [n, 2] fp64 and point3D_ids [n] int64.  Layout
+    (little endian): u64 count, then per image i32 id, 7 f64, i32 camera id, a NUL-terminated name, u64 n and n
+    (f64 x, f64 y, i64 point id)."""
+    import struct
+    images = {}
+    with open(path, "rb") as f:
+        data = f.read()
+    off = 0
+
+    def take(fmt: str):
+        nonlocal off
+        size = struct.calcsize("<" + fmt)
+        if off + size > len(data):
+            raise ValueError(f"{path}: truncated COLMAP images.bin")
+        out = struct.unpack_from("<" + fmt, data, off)
+        off += size
+        return out
+
+    (count,) = take("Q")
+    for _ in range(count):
+        rec = take("idddddddi")
+        end = data.find(b"\x00", off)
+        if end < 0:
+            raise ValueError(f"{path}: truncated COLMAP images.bin (image name)")
+        name = data[off:end].decode("utf-8")
+        off = end + 1
+        (n,) = take("Q")
+        pts = np.frombuffer(data, dtype=np.dtype([("x", "<f8"), ("y", "<f8"), ("id", "<i8")]), count=n, offset=off) \
+            if n else np.zeros(0, dtype=[("x", "<f8"), ("y", "<f8"), ("id", "<i8")])
+        off += 24 * n
+        if off > len(data):
+            raise ValueError(f"{path}: truncated COLMAP images.bin (points)")
+        images[rec[0]] = dict(id=rec[0], qvec=np.array(rec[1:5]), tvec=np.array(rec[5:8]), camera_id=rec[8], name=name,
+                              xys=np.stack([pts["x"], pts["y"]], axis=1).astype(np.float64),
+                              point3D_ids=pts["id"].astype(np.int64))
+    return images
+
+
+def write_colmap_images_bin(path: str, poses: np.ndarray, image_names: List[str], image_ids: List[int] = None,
+                            camera_ids: List[int] = None, points2d: List[np.ndarray] = None) -> None:
+    """The inverse of read_colmap_images_bin: one record per pose row [qw,qx,qy,qz,tx,ty,tz] (world-to-camera, written
+    as given).  image_ids / camera_ids default to 1..n; points2d: per image an [n, 3] array of (x, y, point id)."""
+    import struct
+    n = len(image_names)
+    ids = list(range(1, n + 1)) if image_ids is None else list(image_ids)
+    cids = list(range(1, n + 1)) if camera_ids is None else list(camera_ids)
+    os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
+    with open(path, "wb") as f:
+        f.write(struct.pack("<Q", n))
+        for k in range(n):
+            p = np.asarray(poses[k], np.float64)
+            f.write(struct.pack("<idddddddi", ids[k], *p[:7].tolist(), cids[k]))
+            f.write(image_names[k].encode("utf-8") + b"\x00")
+            pts = np.zeros((0, 3)) if points2d is None else np.asarray(points2d[k]).reshape(-1, 3)
+            f.write(struct.pack("<Q", pts.shape[0]))
+            for x, y, pid in pts:
+                f.write(struct.pack("<ddq", float(x), float(y), int(pid)))
+
+
+def read_colmap_gt_pose(source_path: str) -> np.ndarray:
+    """utils/sfm_utils.py read_colmap_gt_pose: source/sparse/0/images.bin sorted by image name, each record as
+    [qvec2rotmat(q)^T | t] in np.eye(4): [N, 4, 4] fp64 (the matrix metrics.py aligns; its rotation block is the
+    transposed world-to-camera rotation, as in the reference)."""
+    path = os.path.join(source_path, "sparse", "0", "images.bin")
+    if not os.path.isfile(path):
+        raise FileNotFoundError(f"{path} not found")
+    recs = sorted(read_colmap_images_bin(path).values(), key=lambda r: r["name"])
+    out = []
+    for r in recs:
+        pose = np.eye(4, 4)
+        pose[:3, :3] = np.transpose(qvec2rotmat(r["qvec"]))
+        pose[:3, 3] = np.array(r["tvec"])
+        out.append(pose)
+    return np.array(out)
+
+
+def split_train_test(items, n_views: int):
+    """utils/sfm_utils.py split_train_test (llffhold is unused there): 12 test items at np.linspace(1, N - 2, 12)
+    (int), the rest thinned to n_views training items at np.linspace(0, n_rest - 1, n_views) (int).  Returns
+    (train, test) lists."""
+    test_idx = np.linspace(1, len(items) - 2, num=12, dtype=int)
+    train_idx = [i for i in range(len(items)) if i not in test_idx]
+    sparse_idx = np.linspace(0, len(train_idx) - 1, num=n_views, dtype=int)
+    train_idx = [train_idx[i] for i in sparse_idx]
+    return [items[i] for i in train_idx], [items[i] for i in test_idx]
+
+
+# ----------------------------------------------------------------------------------------------
+# the cameras render.py renders: readColmapSceneInfo + loadCam
+# ----------------------------------------------------------------------------------------------
+class Views:
+    """The cameras of one sparse_<n>/<k> folder, sorted by image_name: names [N] (image_name, the file name without
+    its extension), w2c [N, 4, 4] fp64 world-to-camera matrices [qvec2rotmat(q) | t], images [N, H, W, 3] uint8 (the
+    decoded files), width / height (the images'), fovx / fovy (focal2fov of the intrinsics)."""
+
+    def __init__(self, names, w2c, images, width, height, fovx, fovy):
+        self.names, self.w2c, self.images = list(names), w2c, images
+        self.width, self.height, self.fovx, self.fovy = width, height, fovx, fovy
+
+    def __len__(self) -> int:
+        return len(self.names)
+
+
+def loaded_size(width: int, height: int, resolution: int) -> Tuple[int, int]:
+    """The size loadCam (utils/camera_utils.py) resizes a width x height image to at `-r resolution` and resolution
+    scale 1."""
+    if resolution in (1, 2, 4, 8):
+        return round(width / (1.0 * resolution)), round(height / (1.0 * resolution))
+    if resolution == -1:
+        global_down = width / 1600 if width > 1600 else 1
+    else:
+        global_down = width / resolution
+    scale = float(global_down) * 1.0
+    return int(width / scale), int(height / scale)
+
+
+def load_views(source_path: str, n_views: int, split: int = 0, resolution: int = 1) -> Views:
+    """render.py's cameras: readColmapSceneInfo (scene/dataset_readers.py:315-369) reads source/sparse_<n_views>/<split>
+    ({0: the training views, 1: the test views of --eval}), cameras.txt (PINHOLE or SIMPLE_PINHOLE) and images.txt,
+    opens source/images/<basename of the name> and sorts the views by image_name; loadCam resizes each image to
+    loaded_size(resolution) and divides by 255.
+
+    Refused, with the reason: a resolution at which loadCam would resample an image (only sizes PIL's resize copies
+    are kept), an image that is not 8-bit RGB (RGBA included: Camera's alpha mask is not implemented), and views
+    whose image size or field of view differ (one PoseTracker renders them all)."""
+    import math
+    from PIL import Image
+    folder = os.path.join(source_path, f"sparse_{n_views}", str(split))
+    for f in ("cameras.txt", "images.txt"):
+        if not os.path.isfile(os.path.join(folder, f)):
+            raise FileNotFoundError(f"{os.path.join(folder, f)} not found")
+    cams, imgs = read_colmap_text(folder, ("PINHOLE", "SIMPLE_PINHOLE"))
+    if not imgs:
+        raise ValueError(f"{folder}/images.txt lists no image")
+    focal2fov = lambda f, pixels: 2 * math.atan(pixels / (2 * f))
+    recs = []
+    for extr in imgs.values():
+        intr = cams[extr["camera_id"]]
+        path = os.path.join(source_path, "images", os.path.basename(extr["name"]))
+        name = os.path.basename(path).split(".")[0]
+        with Image.open(path) as im:
+            if im.mode != "RGB":
+                raise ValueError(f"{path}: mode {im.mode}; only 8-bit RGB images are supported (an alpha channel "
+                                 "would be Camera's gt_alpha_mask, which is not implemented)")
+            W, H = im.size
+            if loaded_size(W, H, resolution) != (W, H):
+                raise ValueError(f"{path}: -r {resolution} resizes {W}x{H} to {loaded_size(W, H, resolution)}; "
+                                 "resampled images are not supported (use -r 1, or -r -1 up to 1600 pixels wide)")
+            pixels = np.array(im)
+        fx = float(intr["params"][0])
+        fy = fx if intr["model"] == "SIMPLE_PINHOLE" else float(intr["params"][1])
+        w2c = np.eye(4)
+        w2c[:3, :3] = qvec2rotmat(extr["qvec"])
+        w2c[:3, 3] = extr["tvec"]
+        recs.append((name, w2c, pixels, (W, H, focal2fov(fx, intr["width"]), focal2fov(fy, intr["height"]))))
+    recs.sort(key=lambda r: r[0])
+    keys = {r[3] for r in recs}
+    if len(keys) != 1:
+        raise ValueError(f"{folder}: the cameras' intrinsics differ ({len(keys)} distinct image sizes and fields of "
+                         "view); the views are rendered with one camera")
+    W, H, fovx, fovy = keys.pop()
+    return Views([r[0] for r in recs], np.stack([r[1] for r in recs]), np.stack([r[2] for r in recs]), W, H, fovx, fovy)
 
 
 # ----------------------------------------------------------------------------------------------
