@@ -135,7 +135,8 @@ class GaussianModel:
         f_rest = torch.zeros(n, M - 1, 3, device=dev)
         dist2 = torch.clamp_min(distCUDA2(xyz), 0.0000001)
         if scale_gaussian is not None:
-            dist2 = torch.min(torch.as_tensor(scale_gaussian).float().to(dev) ** 2, dist2)
+            # squared in its own dtype, then rounded to fp32, as the reference does (torch.from_numpy(sg ** 2).float())
+            dist2 = torch.min((torch.as_tensor(scale_gaussian) ** 2).float().to(dev), dist2)
         scales = torch.log(torch.sqrt(dist2))[..., None].repeat(1, 3)
         rots = torch.zeros(n, 4, device=dev)
         rots[:, 0] = 1

@@ -195,11 +195,14 @@ def split_train_test(items, n_views: int):
 class Views:
     """The cameras of one sparse_<n>/<k> folder, sorted by image_name: names [N] (image_name, the file name without
     its extension), w2c [N, 4, 4] fp64 world-to-camera matrices [qvec2rotmat(q) | t], images [N, H, W, 3] uint8 (the
-    decoded files), width / height (the images'), fovx / fovy (focal2fov of the intrinsics)."""
+    decoded files), width / height (the images'), fovx / fovy (focal2fov of the intrinsics), camera_ids [N] (each
+    view's COLMAP camera id, intr.id: what readColmapCameras stores as the CameraInfo uid and train.py's save_pose
+    looks up as colmap_id; None when not known)."""
 
-    def __init__(self, names, w2c, images, width, height, fovx, fovy):
+    def __init__(self, names, w2c, images, width, height, fovx, fovy, camera_ids=None):
         self.names, self.w2c, self.images = list(names), w2c, images
         self.width, self.height, self.fovx, self.fovy = width, height, fovx, fovy
+        self.camera_ids = None if camera_ids is None else [int(c) for c in camera_ids]
 
     def __len__(self) -> int:
         return len(self.names)
@@ -218,11 +221,11 @@ def loaded_size(width: int, height: int, resolution: int) -> Tuple[int, int]:
     return int(width / scale), int(height / scale)
 
 
-def load_views(source_path: str, n_views: int, split: int = 0, resolution: int = 1) -> Views:
+def load_views(source_path: str, n_views: int, split: int = 0, resolution: int = 1, images: str = "images") -> Views:
     """render.py's cameras: readColmapSceneInfo (scene/dataset_readers.py:315-369) reads source/sparse_<n_views>/<split>
     ({0: the training views, 1: the test views of --eval}), cameras.txt (PINHOLE or SIMPLE_PINHOLE) and images.txt,
-    opens source/images/<basename of the name> and sorts the views by image_name; loadCam resizes each image to
-    loaded_size(resolution) and divides by 255.
+    opens source/<images>/<basename of the name> (`images`: train.py's -i, the folder name) and sorts the views by
+    image_name; loadCam resizes each image to loaded_size(resolution) and divides by 255.
 
     Refused, with the reason: a resolution at which loadCam would resample an image (only sizes PIL's resize copies
     are kept), an image that is not 8-bit RGB (RGBA included: Camera's alpha mask is not implemented), and views
@@ -240,7 +243,7 @@ def load_views(source_path: str, n_views: int, split: int = 0, resolution: int =
     recs = []
     for extr in imgs.values():
         intr = cams[extr["camera_id"]]
-        path = os.path.join(source_path, "images", os.path.basename(extr["name"]))
+        path = os.path.join(source_path, images, os.path.basename(extr["name"]))
         name = os.path.basename(path).split(".")[0]
         with Image.open(path) as im:
             if im.mode != "RGB":
@@ -256,14 +259,15 @@ def load_views(source_path: str, n_views: int, split: int = 0, resolution: int =
         w2c = np.eye(4)
         w2c[:3, :3] = qvec2rotmat(extr["qvec"])
         w2c[:3, 3] = extr["tvec"]
-        recs.append((name, w2c, pixels, (W, H, focal2fov(fx, intr["width"]), focal2fov(fy, intr["height"]))))
+        recs.append((name, w2c, pixels, (W, H, focal2fov(fx, intr["width"]), focal2fov(fy, intr["height"])), intr["id"]))
     recs.sort(key=lambda r: r[0])
     keys = {r[3] for r in recs}
     if len(keys) != 1:
         raise ValueError(f"{folder}: the cameras' intrinsics differ ({len(keys)} distinct image sizes and fields of "
                          "view); the views are rendered with one camera")
     W, H, fovx, fovy = keys.pop()
-    return Views([r[0] for r in recs], np.stack([r[1] for r in recs]), np.stack([r[2] for r in recs]), W, H, fovx, fovy)
+    return Views([r[0] for r in recs], np.stack([r[1] for r in recs]), np.stack([r[2] for r in recs]), W, H, fovx, fovy,
+                 [r[4] for r in recs])
 
 
 # ----------------------------------------------------------------------------------------------
