@@ -319,6 +319,36 @@ GSB_API int gsb_image_metrics_batch(int32_t V, int32_t C, int32_t H, int32_t W, 
  * H * W must fit in int32. */
 GSB_API int gsb_frames_u8_batch(int32_t V, int32_t H, int32_t W, const float* img, uint8_t* out, gsb_stream_t stream);
 
+/* ---- LPIPS, VGG16 v0.1 (metrics.py:69 lpips(render, gt, net_type='vgg'); lpipsPyTorch/modules/lpips.py,
+ * networks.py BaseNet / VGG16, utils.py normalize_activation).  DESIGN.md 4.15.  fp32 FFMA, NHWC activations, every
+ * sum in one fixed order: an image's values are bit-identical from run to run and whatever else is in the batch.
+ *
+ * gsb_lpips_prepare       ->  BaseNet.z_score: x, y [V, 3, H, W] -> out [2V, H, W, 3], images 0..V-1 from x and
+ *                             V..2V-1 from y, (v - mean) / std in fp32.
+ * gsb_lpips_conv3x3_relu  ->  one Conv2d(Cin, Cout, 3, padding=1) + ReLU of vgg16().features: in [N, H, W, Cin] ->
+ *                             out [N, H, W, Cout].  w_packed [Cin, 3, 3, Cout] (weight.permute(1, 2, 3, 0)), bias
+ *                             [Cout].  Cin is 3 or a multiple of 8, Cout a multiple of 64; w_packed, out (and in when
+ *                             Cin > 3) 16-byte aligned.
+ * gsb_lpips_maxpool2      ->  MaxPool2d(2, 2), floor mode: in [N, H, W, C] -> out [N, H / 2, W / 2, C]; C a multiple
+ *                             of 4, both 16-byte aligned.
+ * gsb_lpips_head          ->  normalize_activation of both feature maps, (fx - fy)^2, the lin layer's 1x1 conv and
+ *                             the sum over H x W: feats [2V, H, W, C] (x's V images, then y's), lin_w [C]; writes
+ *                             out[v * 5 + layer] (fp64), the sum over pixels (the mean is out / (H W)).  partials: at
+ *                             least V * GSB_LPIPS_HEAD_PARTS doubles; C a multiple of 32.
+ * gsb_lpips_scratch_bytes ->  what one call of a V-pair batch at H x W needs: two activation buffers of
+ *                             2V * H * W * 64 floats each (the largest activation, relu1_x) followed by the head's
+ *                             V * GSB_LPIPS_HEAD_PARTS doubles. */
+#define GSB_LPIPS_HEAD_PARTS 128
+GSB_API size_t gsb_lpips_scratch_bytes(int32_t V, int32_t H, int32_t W);
+GSB_API int gsb_lpips_prepare(int32_t V, int32_t H, int32_t W, const float* x, const float* y, float* out,
+                              gsb_stream_t stream);
+GSB_API int gsb_lpips_conv3x3_relu(int32_t N, int32_t H, int32_t W, int32_t Cin, int32_t Cout, const float* in,
+                                   const float* w_packed, const float* bias, float* out, gsb_stream_t stream);
+GSB_API int gsb_lpips_maxpool2(int32_t N, int32_t H, int32_t W, int32_t C, const float* in, float* out,
+                               gsb_stream_t stream);
+GSB_API int gsb_lpips_head(int32_t V, int32_t H, int32_t W, int32_t C, const float* feats, const float* lin_w,
+                           int32_t layer, double* out, double* partials, gsb_stream_t stream);
+
 /* Per-point Adam (scene/per_point_adam.py:34-98), n tensors in one launch. */
 typedef struct GsbAdamTensor {
   float* param;

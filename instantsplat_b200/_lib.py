@@ -81,7 +81,8 @@ EXPORTS = ("gsb_geom_bytes", "gsb_binning_bytes", "gsb_image_bytes", "gsb_prepro
            "gsb_preprocess_batch", "gsb_render_batch", "gsb_backward_pose_batch", "gsb_l1_mask_fwd_bwd_batch",
            "gsb_track_step_batch", "gsb_backward_batch", "gsb_loss_forward_batch", "gsb_loss_backward_batch",
            "gsb_backward_batch_stats", "gsb_image_metrics_scratch_bytes", "gsb_image_metrics_batch",
-           "gsb_frames_u8_batch")
+           "gsb_frames_u8_batch", "gsb_lpips_scratch_bytes", "gsb_lpips_prepare", "gsb_lpips_conv3x3_relu",
+           "gsb_lpips_maxpool2", "gsb_lpips_head")
 KERNEL_IDS = ("preprocess", "sort_depth", "scan", "duplicate", "sort_tile", "gather", "blend_fwd", "blend_bwd",
               "preprocess_bwd", "loss_fwd", "loss_bwd", "adam")
 
@@ -168,9 +169,16 @@ def lib() -> ctypes.CDLL:
     L.gsb_image_metrics_scratch_bytes.argtypes = [i32, i32, i32, i32]
     L.gsb_image_metrics_batch.argtypes = [i32, i32, i32, i32, vp, vp, vp, i32, vp, vp, sz, vp]
     L.gsb_frames_u8_batch.argtypes = [i32, i32, i32, vp, vp, vp]
+    L.gsb_lpips_scratch_bytes.restype = sz
+    L.gsb_lpips_scratch_bytes.argtypes = [i32, i32, i32]
+    L.gsb_lpips_prepare.argtypes = [i32, i32, i32, vp, vp, vp, vp]
+    L.gsb_lpips_conv3x3_relu.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp]
+    L.gsb_lpips_maxpool2.argtypes = [i32, i32, i32, i32, vp, vp, vp]
+    L.gsb_lpips_head.argtypes = [i32, i32, i32, i32, vp, vp, i32, vp, vp, vp]
     for f in ("gsb_preprocess_batch", "gsb_render_batch", "gsb_backward_pose_batch", "gsb_l1_mask_fwd_bwd_batch",
               "gsb_track_step_batch", "gsb_backward_batch", "gsb_loss_forward_batch", "gsb_loss_backward_batch",
-              "gsb_backward_batch_stats", "gsb_image_metrics_batch", "gsb_frames_u8_batch"):
+              "gsb_backward_batch_stats", "gsb_image_metrics_batch", "gsb_frames_u8_batch", "gsb_lpips_prepare",
+              "gsb_lpips_conv3x3_relu", "gsb_lpips_maxpool2", "gsb_lpips_head"):
         getattr(L, f).restype = ctypes.c_int
     L.gsb_adam_step_gated.argtypes = [i32, ctypes.POINTER(GsbAdamTensor), vp, vp, vp]
     L.gsb_adam_step_gated.restype = ctypes.c_int

@@ -5,8 +5,10 @@ model directory and per test/<method>.
     pairing, in sorted order here), decoded by PIL to k / 255 (to_tensor) and measured in one batched
     evaluation.image_metrics call (mode "png8", the identity on k / 255): PSNR of the whole image's MSE and the
     loss's SSIM, per view in fp64.  Written as metrics.txt lines in the reference's format, results.json (the means)
-    and per_view.json (per file name), with the reference's keys and nesting.  LPIPS is not computed (it needs
-    pretrained VGG weights): its key is left out and the run says so.
+    and per_view.json (per file name), with the reference's keys and nesting.  LPIPS (VGG) needs pretrained weights:
+    with --lpips_weights DIR (a directory holding torch hub's vgg16-397923af.pth and vgg.pth, such as
+    $TORCH_HOME/hub/checkpoints) it is computed on the GPU by lpips.LpipsVGG, built once per run, and written where
+    the reference writes it; without it its key is left out and the run says so.
   * Poses: source/sparse/0/images.bin (read_colmap_gt_pose), thinned to the training views by split_train_test,
     against pose/<method>/pose_optimized.npy: align_pose (scale and centre the translations, orthogonal Procrustes),
     then align_ate_c2b_use_a2b (a sim3 Umeyama fit in fp32), then compute_ATE and compute_rpe.  RPE_t is reported x
@@ -16,7 +18,7 @@ model directory and per test/<method>.
 A model directory without test/ is reported and skipped; a method without sparse/0/images.bin or pose_optimized.npy
 keeps its image numbers and skips the pose part, with a message.
 
-    python -m instantsplat_b200.metrics -s SOURCE -m MODEL [MODEL ...] --n_views N
+    python -m instantsplat_b200.metrics -s SOURCE -m MODEL [MODEL ...] --n_views N [--lpips_weights DIR]
 """
 from __future__ import annotations
 
@@ -29,6 +31,7 @@ from typing import Dict, List, Tuple
 import numpy as np
 import torch
 
+from . import lpips as LP
 from .scene_io import read_colmap_gt_pose, split_train_test
 
 
@@ -170,21 +173,37 @@ def image_numbers(renders: np.ndarray, gts: np.ndarray, device="cuda") -> Dict[s
     return {"PSNR": m["psnr"].cpu(), "SSIM": m["ssim"].cpu()}
 
 
-def evaluate_method(scene_dir: str, method: str, source_path: str, n_views: int, device="cuda"):
+def lpips_numbers(renders: np.ndarray, gts: np.ndarray, net, device="cuda") -> torch.Tensor:
+    """LPIPS per view of uint8 [V, H, W, 3] images read as to_tensor reads them (k / 255), by lpips.LpipsVGG `net`:
+    an fp64 CPU tensor [V]."""
+    f = lambda u8: (torch.from_numpy(np.ascontiguousarray(u8)).to(device) / 255.0).permute(0, 3, 1, 2).contiguous()
+    return net(f(renders), f(gts))[0].cpu()
+
+
+def evaluate_method(scene_dir: str, method: str, source_path: str, n_views: int, device="cuda", lpips_net=None):
     """One test/<method> of one model directory: writes test/<method>/metrics.txt and (when the pose inputs exist)
-    pose/<method>/pose_eval.txt.  Returns (full, per_view) entries for results.json and per_view.json."""
+    pose/<method>/pose_eval.txt.  Returns (full, per_view) entries for results.json and per_view.json.  LPIPS is
+    measured with lpips_net (an lpips.LpipsVGG) when it is given."""
     method_dir = os.path.join(scene_dir, "test", method)
     renders, gts, names = read_pairs(method_dir)
     m = image_numbers(renders, gts, device)
     psnr, ssim = m["PSNR"].tolist(), m["SSIM"].tolist()
+    lp = lpips_numbers(renders, gts, lpips_net, device) if lpips_net is not None else None
     with open(os.path.join(method_dir, "metrics.txt"), "w") as f:
         for idx, name in enumerate(names):
-            f.write(f"image name{name}, image idx: {idx}, PSNR: {psnr[idx]:.2f}, SSIM: {ssim[idx]:.4f}\n")
+            tail = "" if lp is None else f", LPIPS: {lp[idx].item():.4f}"
+            f.write(f"image name{name}, image idx: {idx}, PSNR: {psnr[idx]:.2f}, SSIM: {ssim[idx]:.4f}{tail}\n")
     full = {"SSIM": float(m["SSIM"].mean()), "PSNR": float(m["PSNR"].mean())}
     per_view = {"SSIM": dict(zip(names, ssim)), "PSNR": dict(zip(names, psnr))}
+    if lp is not None:
+        full["LPIPS"] = float(lp.mean())
+        per_view["LPIPS"] = dict(zip(names, lp.tolist()))
     print(f"  SSIM : {full['SSIM']:>12.7f}")
     print(f"  PSNR : {full['PSNR']:>12.7f}")
-    print("  LPIPS: not computed (it needs pretrained VGG weights)")
+    if lp is None:
+        print("  LPIPS: not computed (it needs pretrained VGG weights)")
+    else:
+        print(f"  LPIPS: {full['LPIPS']:>12.7f}")
     pose_dir = os.path.join(scene_dir, "pose", method)
     npy = os.path.join(pose_dir, "pose_optimized.npy")
     try:
@@ -205,7 +224,7 @@ def evaluate_method(scene_dir: str, method: str, source_path: str, n_views: int,
     return full, per_view
 
 
-def evaluate(scene_dirs, source_path: str, n_views: int, device="cuda") -> int:
+def evaluate(scene_dirs, source_path: str, n_views: int, device="cuda", lpips_net=None) -> int:
     """metrics.py's evaluate over model directories: <scene>/results.json and <scene>/per_view.json for each.
     Returns the number of model directories that could not be evaluated (each is reported with its reason)."""
     failed = 0
@@ -220,7 +239,8 @@ def evaluate(scene_dirs, source_path: str, n_views: int, device="cuda") -> int:
                 if not os.path.isdir(os.path.join(test_dir, method)):
                     continue
                 print("Method:", method)
-                full[method], per_view[method] = evaluate_method(scene_dir, method, source_path, n_views, device)
+                full[method], per_view[method] = evaluate_method(scene_dir, method, source_path, n_views, device,
+                                                                  lpips_net)
         except (OSError, ValueError) as e:
             print(f"Unable to compute metrics for model {scene_dir}: {e}")
             failed += 1
@@ -234,12 +254,21 @@ def evaluate(scene_dirs, source_path: str, n_views: int, device="cuda") -> int:
 
 def main(argv=None) -> int:
     ap = argparse.ArgumentParser(prog="python -m instantsplat_b200.metrics",
-                                 description="metrics.py: PSNR / SSIM of the test renders and the pose errors")
+                                 description="metrics.py: PSNR / SSIM (and LPIPS) of the test renders and the pose errors")
     ap.add_argument("-s", "--source_path", required=True)
     ap.add_argument("-m", "--model_paths", required=True, nargs="+")
     ap.add_argument("--n_views", type=int, required=True)
+    ap.add_argument("--lpips_weights", metavar="DIR", default=None,
+                    help=f"directory holding {LP.VGG_FILE} and {LP.LIN_FILE} (torch hub's checkpoints directory): "
+                         "also report LPIPS (VGG)")
     a = ap.parse_args(argv)
-    return 1 if evaluate(a.model_paths, a.source_path, a.n_views) else 0
+    net = None
+    if a.lpips_weights is not None:
+        try:
+            net = LP.LpipsVGG.from_dir(a.lpips_weights, "cuda")
+        except (OSError, ValueError) as e:
+            ap.error(str(e))
+    return 1 if evaluate(a.model_paths, a.source_path, a.n_views, lpips_net=net) else 0
 
 
 if __name__ == "__main__":
