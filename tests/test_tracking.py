@@ -72,7 +72,8 @@ def test_masked_l1_kernel_matches_reference_formula():
     from instantsplat_b200 import _lib
     L = _lib.lib()
     g = torch.Generator().manual_seed(0)
-    for shape in ((3, 37, 53), (3, 64, 64)):
+    # n < 4 runs only the scalar tail (no group of four), n = 5 one group and a tail
+    for shape in ((3, 37, 53), (3, 64, 64), (1, 1, 1), (1, 1, 2), (3, 1, 1), (1, 1, 5)):
         img = torch.rand(*shape, generator=g) - 0.3       # some non-positive entries -> masked out
         gt = torch.rand(*shape, generator=g)
         a = img.clone().requires_grad_(True)
