@@ -248,7 +248,8 @@ __device__ __forceinline__ void stage_out(float* __restrict__ dst, const float* 
 //   cam | xyz[3N] | scale[3N] | quat[4N] | opacity[N] | sh[49N]
 // Every array is copied CONTIGUOUSLY (128-bit global loads -> 128-bit shared stores, conflict-free);
 // each thread then walks its own row with an odd word stride (3, 45; the quaternion is one LDS.128), so
-// the strided accesses are conflict-free too.  Split SH layout: dc at sh[3t], rest at sh[3N + 45t].
+// the strided accesses are conflict-free too.  Split SH layout: dc at sh[3t], rest at sh[3N + 3(M-1)t] (stride 45 at
+// M = 16 and 9 at M = 4; the 24 of M = 9 is even, so its rest rows see 8-way bank conflicts).
 // Packed [P,M,3] layout (generic B2 boundary): rows padded to kRowPad = 49 words.
 constexpr int kSmXyz = 0, kSmSc = 3 * kPT, kSmQ = 6 * kPT, kSmOp = 10 * kPT, kSmSh = 11 * kPT;
 constexpr int kSmFloats = 11 * kPT + kRowPad * kPT;
@@ -312,12 +313,16 @@ __device__ __forceinline__ void load_block_inputs(const InPtrs& in, int first, i
 // issues one bulk copy per input array (cp.async.bulk.shared.global, SASS UBLKCP); nothing passes through registers or
 // allocates L1 lines (with register staging, the 180 KB a resident set of CTAs keeps in flight is bounded by the L1
 // carve-out, so giving shared memory the whole unified storage does not help).
-__device__ __forceinline__ bool block_inputs_bulk_ok(const InPtrs& in, int nv, bool use_sh, int M) {
-  return in.vec_ok != 0 && nv == kPT && in.scales && in.rots && (!use_sh || (!in.sh_packed && M == 16));
+// Any coefficient count M of the split layout qualifies: the CTA's rest slice is 3 (M - 1) kPT floats, a multiple of 16
+// bytes in size and offset (rest_bytes).
+__device__ __forceinline__ uint32_t rest_bytes(int M) { return (uint32_t)(3 * (M - 1) * kPT * 4); }
+__device__ __forceinline__ bool block_inputs_bulk_ok(const InPtrs& in, int nv, bool use_sh) {
+  return in.vec_ok != 0 && nv == kPT && in.scales && in.rots && (!use_sh || !in.sh_packed);
 }
-__device__ __forceinline__ void bulk_load_block_inputs(const InPtrs& in, int first, bool use_sh, int D, float* sm,
+__device__ __forceinline__ void bulk_load_block_inputs(const InPtrs& in, int first, bool use_sh, int D, int M, float* sm,
                                                        uint64_t* bar) {
-  constexpr uint32_t B3 = 3 * kPT * 4, B4 = 4 * kPT * 4, B1 = kPT * 4, BR = 45 * kPT * 4;
+  constexpr uint32_t B3 = 3 * kPT * 4, B4 = 4 * kPT * 4, B1 = kPT * 4;
+  const uint32_t BR = rest_bytes(M);
   const bool rest = use_sh && D > 0;
   mbar_expect_tx(bar, 2 * B3 + B4 + B1 + (use_sh ? B3 : 0u) + (rest ? BR : 0u));
   bulk_g2s(sm + kSmXyz, in.means + (size_t)3 * first, B3, bar);
@@ -325,13 +330,13 @@ __device__ __forceinline__ void bulk_load_block_inputs(const InPtrs& in, int fir
   bulk_g2s(sm + kSmQ, in.rots + (size_t)4 * first, B4, bar);
   bulk_g2s(sm + kSmOp, in.opac + first, B1, bar);
   if (use_sh) bulk_g2s(sm + kSmSh, in.sh_dc + (size_t)3 * first, B3, bar);
-  if (rest) bulk_g2s(sm + kSmSh + 3 * kPT, in.sh_rest + (size_t)45 * first, BR, bar);
+  if (rest) bulk_g2s(sm + kSmSh + 3 * kPT, in.sh_rest + (size_t)3 * (M - 1) * first, BR, bar);
 }
 // all threads call; returns when the CTA's inputs are in shared memory
 __device__ __forceinline__ void stage_block_inputs(const InPtrs& in, int first, int nv, bool use_sh, int D, int M, float* sm,
                                                    uint64_t* bar) {
-  if (block_inputs_bulk_ok(in, nv, use_sh, M)) {
-    if (threadIdx.x == 0) bulk_load_block_inputs(in, first, use_sh, D, sm, bar);
+  if (block_inputs_bulk_ok(in, nv, use_sh)) {
+    if (threadIdx.x == 0) bulk_load_block_inputs(in, first, use_sh, D, M, sm, bar);
     mbar_wait(bar, 0u);
   } else {
     load_block_inputs(in, first, nv, use_sh, D, M, sm);
@@ -490,19 +495,19 @@ __device__ __forceinline__ bool store_block_grads(const InPtrs& in, const OutPtr
                                                   int first, int nv, int M, bool use_sh, bool vec) {
   // Full CTA, aligned, split SH layout: every gradient array of the CTA leaves as one bulk store (shared -> global)
   // issued by one thread; the generic path below covers ragged / unaligned / packed cases.
-  const bool bulk_out = vec && nv == kPT && !in.sh_packed && M == 16;
+  const bool bulk_out = vec && nv == kPT && !in.sh_packed;
   if (bulk_out) tma_store_fence();
   __syncthreads();
   if (bulk_out) {
     if (threadIdx.x == 0) {
-      constexpr uint32_t B3 = 3 * kPT * 4, B4 = 4 * kPT * 4, B1 = kPT * 4, BR = 45 * kPT * 4;
+      constexpr uint32_t B3 = 3 * kPT * 4, B4 = 4 * kPT * 4, B1 = kPT * 4;
       if (out.dmeans) bulk_s2g(out.dmeans + (size_t)3 * first, sm + kSmXyz, B3);
       if (out.dscales) bulk_s2g(out.dscales + (size_t)3 * first, sm + kSmSc, B3);
       if (out.drots) bulk_s2g(out.drots + (size_t)4 * first, sm + kSmQ, B4);
       if (out.dopac) bulk_s2g(out.dopac + first, sm + kSmOp, B1);
       if (use_sh && out.dsh_dc) {
         bulk_s2g(out.dsh_dc + (size_t)3 * first, sh, B3);
-        if (out.dsh_rest) bulk_s2g(out.dsh_rest + (size_t)45 * first, sh + 3 * kPT, BR);
+        if (M > 1 && out.dsh_rest) bulk_s2g(out.dsh_rest + (size_t)3 * (M - 1) * first, sh + 3 * kPT, rest_bytes(M));
       }
       bulk_commit();
     }
@@ -809,19 +814,20 @@ k_preprocess_bwd(InPtrs in, GeomView gv, const int pose_only_layout, OutPtrs out
   }
   // Full CTA, aligned, split SH layout: every gradient array of the CTA leaves as one bulk store (shared -> global)
   // issued by one thread; the generic path below covers ragged / unaligned / packed cases.
-  const bool bulk_out = vec && nv == kPT && !in.sh_packed && M == 16;
+  const bool bulk_out = vec && nv == kPT && !in.sh_packed;
   if (bulk_out) tma_store_fence();
   __syncthreads();
   if (bulk_out) {
     if (threadIdx.x == 0) {
-      constexpr uint32_t B3 = 3 * kPT * 4, B4 = 4 * kPT * 4, B1 = kPT * 4, BR = 45 * kPT * 4;
+      constexpr uint32_t B3 = 3 * kPT * 4, B4 = 4 * kPT * 4, B1 = kPT * 4;
       if (out.dmeans) bulk_s2g(out.dmeans + (size_t)3 * first, sm + kSmXyz, B3);
       if (out.dscales) bulk_s2g(out.dscales + (size_t)3 * first, sm + kSmSc, B3);
       if (out.drots) bulk_s2g(out.drots + (size_t)4 * first, sm + kSmQ, B4);
       if (out.dopac) bulk_s2g(out.dopac + first, sm + kSmOp, B1);
       if (use_sh && out.dsh_dc) {
         bulk_s2g(out.dsh_dc + (size_t)3 * first, sm + kSmSh, B3);
-        if (out.dsh_rest) bulk_s2g(out.dsh_rest + (size_t)45 * first, sm + kSmSh + 3 * kPT, BR);
+        if (M > 1 && out.dsh_rest)
+          bulk_s2g(out.dsh_rest + (size_t)3 * (M - 1) * first, sm + kSmSh + 3 * kPT, rest_bytes(M));
       }
       bulk_commit();
     }

@@ -96,6 +96,8 @@ class PerPointAdam(Optimizer):
                     st["exp_avg"] = torch.zeros_like(p)
                     st["exp_avg_sq"] = torch.zeros_like(p)
                 st["step"] += 1
+                if p.numel() == 0:                           # SH degree 0's f_rest: counts its step, nothing to launch
+                    continue
                 t = st["step"]
                 # old-style bias correction folded into the step size, evaluated on the host in double
                 step_size = group["lr"] * ((1 - b2 ** t) ** 0.5 / (1 - b1 ** t))

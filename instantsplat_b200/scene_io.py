@@ -8,8 +8,8 @@ What the reference's training stage reads and writes, so a scene produced here c
   utils/sfm_utils.py:202-315;
 * `points3D.ply`: x,y,z f4 | nx,ny,nz f4 | red,green,blue u1 (scene/dataset_readers.py:315-369);
 * `confidence_dsp.npy` [P,1] (train.py:63-96);
-* the trained model `point_cloud.ply`: x,y,z,nx,ny,nz,f_dc_0..2,f_rest_0..44,opacity,scale_0..2,rot_0..3, all f4,
-  SH stored channel-major (scene/gaussian_model.py:247-278), optionally followed by Mip-Splatting's `filter_3D` f4;
+* the trained model `point_cloud.ply`: x,y,z,nx,ny,nz,f_dc_0..2,f_rest_0..44,opacity,scale_0..2,rot_0..3, all f4
+  (f_rest_0..3(M-1)-1 at SH degree D, M = (D+1)^2: none at degree 0), SH stored channel-major (scene/gaussian_model.py:247-278), optionally followed by Mip-Splatting's `filter_3D` f4;
 * `pose_optimized.npy` [n,4,4] world-to-camera matrices ordered by COLMAP image id
   (train.py:46-60).
 
@@ -362,7 +362,9 @@ def load_gaussians_ply(path: str) -> Dict[str, np.ndarray]:
     P = d.shape[0]
     col = lambda prefix: np.stack([d[n] for n in sorted((n for n in d.dtype.names if n.startswith(prefix)),
                                                         key=lambda s: int(s.split("_")[-1]))], axis=1)
-    rest = col("f_rest_")
+    # SH degree 0 stores no f_rest_* property: f_rest is then [P, 0, 3]
+    has_rest = any(n.startswith("f_rest_") for n in d.dtype.names)
+    rest = col("f_rest_") if has_rest else np.zeros((P, 0), np.float32)
     out = dict(xyz=np.stack([d["x"], d["y"], d["z"]], axis=1),
                f_dc=col("f_dc_").reshape(P, 3, 1).transpose(0, 2, 1).copy(),
                f_rest=rest.reshape(P, 3, rest.shape[1] // 3).transpose(0, 2, 1).copy(),

@@ -37,6 +37,8 @@ from .frame import densify_stats
 from .per_point_adam import launch_adam
 from .scenes import Scene
 
+# The six per-Gaussian tensors and their floats per Gaussian at SH degree 3 (15 f_rest rows).  A trainer's own widths
+# follow its scene's f_rest (segment_widths, JointTrainer.widths); the names and their order are the same at every degree.
 SEGMENTS = (("xyz", 3), ("f_dc", 3), ("f_rest", 45), ("opacity", 1), ("scaling", 3), ("rotation", 4))
 ADAM_BETAS, ADAM_EPS = (0.9, 0.999), 1e-15       # training_setup_pp's PerPointAdam (scene/gaussian_model.py:221)
 
@@ -173,11 +175,35 @@ def L_sig_words():
     return (_lib.lib().gsb_peer_signal_bytes() + 3) // 4
 
 
-def _layout(P: int):
-    """Where the SEGMENTS tensors of P Gaussians lie in the flat buffers: {name: (begin, end)}, each segment padded to a
-    multiple of 64 floats (256 bytes), and the buffers' length."""
+def sh_rest_rows(f_rest: torch.Tensor, P: int) -> int:
+    """The f_rest rows per Gaussian, M - 1 = (D+1)^2 - 1 for SH degree D (0, 3, 8 or 15), of an f_rest tensor
+    [P, M-1, 3] (or [P, 3(M-1)]); GsbError with the reason for any other shape."""
+    shape = tuple(f_rest.shape)
+    if len(shape) == 3 and shape[0] == P and shape[2] == 3:
+        rows = shape[1]
+    elif len(shape) == 2 and shape[0] == P and shape[1] % 3 == 0:
+        rows = shape[1] // 3
+    else:
+        raise _lib.GsbError(f"f_rest has shape {shape}; expected [P, M-1, 3] with P = {P}")
+    d = int(round((rows + 1) ** 0.5)) - 1
+    if rows not in (0, 3, 8, 15):
+        raise _lib.GsbError(f"f_rest has {rows} rows per Gaussian; SH degree D stores (D+1)^2 - 1 of them, so one of "
+                            "0, 3, 8 or 15 (degrees 0 to 3)" + (" (degree 4 and above are not supported)"
+                                                                 if (d + 1) ** 2 == rows + 1 else ""))
+    return rows
+
+
+def segment_widths(rest_rows: int):
+    """(name, floats per Gaussian) of the six per-Gaussian tensors of a model with `rest_rows` f_rest rows: SEGMENTS
+    with f_rest at 3 * rest_rows (empty at degree 0)."""
+    return tuple((name, 3 * rest_rows if name == "f_rest" else k) for name, k in SEGMENTS)
+
+
+def flat_layout(P: int, widths=SEGMENTS):
+    """Where the per-Gaussian tensors (name, width) of P Gaussians lie in the flat buffers: {name: (begin, end)}, each
+    segment padded to a multiple of 64 floats (256 bytes; an empty f_rest takes no space), and the buffers' length."""
     segments, total = {}, 0
-    for name, k in SEGMENTS:
+    for name, k in widths:
         segments[name] = (total, total + (P * k + 63) // 64 * 64)
         total = segments[name][1]
     return segments, total
@@ -204,8 +230,17 @@ class JointTrainer:
         self.fovx, self.fovy = float(scene.fovx), float(scene.fovy)
         self.sh_degree = scene.sh_degree
         self.n_views = scene.n_views
+        # ---- the SH layout: the stored degree follows the scene's f_rest; cfg.max_sh_degree may not exceed it
+        rows = sh_rest_rows(scene.params["f_rest"], P)
+        self.stored_sh_degree = int(round((rows + 1) ** 0.5)) - 1
+        self.sh_coeffs = rows + 1
+        if self.cfg.max_sh_degree > self.stored_sh_degree:
+            raise _lib.GsbError(f"OptimConfig.max_sh_degree {self.cfg.max_sh_degree} exceeds the scene's stored SH "
+                                f"degree {self.stored_sh_degree} (f_rest has {rows} rows per Gaussian): the trainer "
+                                "would raise the active degree past the coefficients it holds")
+        self.widths = segment_widths(rows)
         # ---- flat buffers
-        self.segments, self.total = _layout(P)
+        self.segments, self.total = flat_layout(P, self.widths)
         total = self.total
         if self._fused:
             # peer-visible parameter / gradient buffers (CUDA IPC) and shard-sized Adam moments
@@ -226,7 +261,7 @@ class JointTrainer:
             self.grads = torch.zeros(total, dtype=torch.float32, device=self.dev)
             self.exp_avg = torch.zeros(total, dtype=torch.float32, device=self.dev)
             self.exp_avg_sq = torch.zeros(total, dtype=torch.float32, device=self.dev)
-        for name, k in SEGMENTS:
+        for name, k in self.widths:
             self.view(self.params, name).copy_(scene.params[name].reshape(P, k).to(self.dev))
         self.poses = scene.poses.to(self.dev).float().contiguous()              # [n_views,7]
         if self.exchange == "fused_p2p_nccl":
@@ -277,7 +312,7 @@ class JointTrainer:
         self._keep = None
         # per-tensor Adam step counts are opt_step minus the optimizer steps that skipped the tensor (the densify and
         # opacity-reset iterations replace tensors, which then have no gradient in the reference)
-        self._lag = {name: 0 for name, _ in SEGMENTS}
+        self._lag = {name: 0 for name, _ in self.widths}
         self._stats = None
         if c.densify:
             self._stats = torch.zeros(3, P, dtype=torch.float32, device=self.dev)
@@ -290,7 +325,7 @@ class JointTrainer:
 
     # ------------------------------------------------------------------------------------------
     def view(self, flat: torch.Tensor, name: str) -> torch.Tensor:
-        k = dict(SEGMENTS)[name]
+        k = dict(self.widths)[name]
         o = self.segments[name][0]
         return flat[o:o + self.P * k].view(self.P, k)
 
@@ -332,7 +367,7 @@ class JointTrainer:
         return None if self._stats is None else self._stats[2]
 
     def step_count(self, name: str) -> int:
-        """Adam step count of one tensor ("pose" or a SEGMENTS name)."""
+        """Adam step count of one tensor ("pose" or a per-Gaussian tensor's name)."""
         return self.opt_step - self._lag.get(name, 0)
 
     def _mip_setup(self) -> None:
@@ -352,11 +387,15 @@ class JointTrainer:
     def _gauss(self, poses: torch.Tensor) -> GsbGaussians:
         """The Gaussians at a pose row [7] (or, for the batched entry points, rows [V, 7])."""
         p = self.params
-        return gaussians(self.P, *(self.view(p, n) for n in ("xyz", "rotation", "scaling", "opacity", "f_dc", "f_rest")),
-                         poses)
+        return gaussians(self.P, *(self.view(p, n) for n in ("xyz", "rotation", "scaling", "opacity", "f_dc")),
+                         self.view(p, "f_rest") if self.sh_coeffs > 1 else None, poses)
 
     def _camera(self):
-        return self.ident.camera(self.active_sh_degree, 16, self.exact_cull)
+        return self.ident.camera(self.active_sh_degree, self.sh_coeffs, self.exact_cull)
+
+    def _nonempty(self):
+        """The (name, width) of the per-Gaussian tensors the kernels update: all six, but f_rest only above degree 0."""
+        return [(name, k) for name, k in self.widths if k > 0]
 
     # ------------------------------------------------------------------------------------------
     def _size_binning(self, R: int, slot: Optional["_Slot"] = None) -> None:
@@ -463,7 +502,7 @@ class JointTrainer:
         gr.dL_drotations = self.view(gd, "rotation").data_ptr()
         gr.dL_dopacities = self.view(gd, "opacity").data_ptr()
         gr.dL_dsh_dc = self.view(gd, "f_dc").data_ptr()
-        gr.dL_dsh_rest = self.view(gd, "f_rest").data_ptr()
+        gr.dL_dsh_rest = self.view(gd, "f_rest").data_ptr() if self.sh_coeffs > 1 else None
         return gr
 
     def _loss(self, sums: torch.Tensor) -> torch.Tensor:
@@ -482,8 +521,9 @@ class JointTrainer:
             allreduce_sum_((self.grads, self._pg_buf), self.pg)
 
     def _stepped(self, skip=()) -> List[str]:
-        """The tensors an optimizer update steps, in launch order: entry i of the update reads _step_dev[i]."""
-        names = [name for name, _ in SEGMENTS if name not in skip]
+        """The tensors an optimizer update steps, in launch order: entry i of the update reads _step_dev[i].  An empty
+        f_rest (degree 0) is not launched; its step count still advances with the others (_lag)."""
+        names = [name for name, _ in self._nonempty() if name not in skip]
         return names + ["pose"] if self.cfg.optim_pose else names
 
     def _advance(self, skip=()) -> None:
@@ -500,14 +540,14 @@ class JointTrainer:
         self._step_dev[:len(names)].copy_(host, non_blocking=True)
 
     def _adam_entry(self, name: str, grad_scale: float) -> dict:
-        """launch_adam's entry of one tensor ("pose" or a SEGMENTS name); its step size is in _step_dev."""
+        """launch_adam's entry of one tensor ("pose" or a per-Gaussian tensor's name); its step size is in _step_dev."""
         if name == "pose":
             t = dict(param=self.poses, grad=self.pose_grad, exp_avg=self.pose_m, exp_avg_sq=self.pose_v, row_len=7,
                      per_point_lr=None)
         else:
             t = dict(param=self.view(self.params, name), grad=self.view(self.grads, name),
                      exp_avg=self.view(self.exp_avg, name), exp_avg_sq=self.view(self.exp_avg_sq, name),
-                     row_len=dict(SEGMENTS)[name], per_point_lr=self.per_point_lr if name == "xyz" else None)
+                     row_len=dict(self.widths)[name], per_point_lr=self.per_point_lr if name == "xyz" else None)
         return dict(t, beta1=ADAM_BETAS[0], beta2=ADAM_BETAS[1], eps=ADAM_EPS, weight_decay=0.0, grad_scale=grad_scale)
 
     def optimizer_step(self, grad_scale: Optional[float] = None, skip=()) -> None:
@@ -542,12 +582,13 @@ class JointTrainer:
         L = _lib.lib()
         st = _lib.stream_ptr()
         # 1. whole-tensor gates on the local gradients, OR-ed across ranks
-        arr = (GsbAdamTensor * len(SEGMENTS))()
-        for a, (name, k) in zip(arr, SEGMENTS):
+        segs = self._nonempty()
+        arr = (GsbAdamTensor * len(segs))()
+        for a, (name, k) in zip(arr, segs):
             g = self.view(self.grads, name)
             a.param = a.exp_avg = a.exp_avg_sq = a.grad = g.data_ptr()
             a.numel, a.row_len, a.grad_scale = g.numel(), k, 1.0
-        check(L.gsb_adam_gate(len(SEGMENTS), arr, self.flags.data_ptr(), st), "gsb_adam_gate")
+        check(L.gsb_adam_gate(len(segs), arr, self.flags.data_ptr(), st), "gsb_adam_gate")
         if self.exchange == "fused_p2p":
             # gate flags, the binning-overflow word and the pose-gradient table are summed over the ranks by ONE tiny
             # kernel through peer memory; its flag barrier is also "every rank's gradients are written".  Epoch 0 = the
@@ -567,7 +608,7 @@ class JointTrainer:
         # skipped: the number of Gaussians is fixed with peer-memory buffers)
         lo, hi = self.shard
         pieces = []
-        for fi, (name, k) in enumerate(SEGMENTS):
+        for fi, (name, k) in enumerate(segs):
             s0, s1 = self.segments[name]
             b, e = max(lo, s0), min(hi, s1)
             if e > b:
@@ -586,7 +627,7 @@ class JointTrainer:
         # 3. pose table: replicated Adam on the all-reduced pose gradients
         if self.cfg.optim_pose:
             launch_adam([self._adam_entry("pose", 1.0 / self.world_size)], self._pose_flags, skip_ptr=self._ovf.data_ptr(),
-                        step_sizes_dev=self._step_dev[len(SEGMENTS):])
+                        step_sizes_dev=self._step_dev[len(segs):])
         # 4. nobody may start the next forward before every rank's parameter stores have landed
         if self.exchange == "fused_p2p":
             check(L.gsb_peer_barrier(self.world_size, self.rank, self._peer_sig.ptr_array(), 0, 1, st),
@@ -682,13 +723,13 @@ class JointTrainer:
                 self.densify_and_prune(c.densify_grad_threshold, c.min_opacity, self.scene_extent, de["size_threshold"],
                                        c.densify_clone_split, self.densify_generator)
                 self.densified_at.append(self.iteration)
-                skip.update(name for name, _ in SEGMENTS)
+                skip.update(name for name, _ in self.widths)
             if de["reset"]:
                 self.reset_opacity()
                 self.reset_at.append(self.iteration)
                 skip.add("opacity")
             if do_opt:
-                skip = [name for name, _ in SEGMENTS if name in skip]
+                skip = [name for name, _ in self.widths if name in skip]
                 self._advance(skip)
                 self._launch_adam(grad_scale, skip, skip_ptr)
         else:
@@ -914,15 +955,15 @@ class JointTrainer:
             raise _lib.GsbError("changing the number of Gaussians is not supported with peer-memory buffers "
                                 "(exchange='fused_p2p'); use exchange='allreduce'")
         new = {name: rows(name, self.view(self.params, name), self.view(self.exp_avg, name),
-                          self.view(self.exp_avg_sq, name)) for name, _ in SEGMENTS}
+                          self.view(self.exp_avg_sq, name)) for name, _ in self.widths}
         self.P = new_P
-        self.segments, total = _layout(new_P)
+        self.segments, total = flat_layout(new_P, self.widths)
         self.total = total
         self.params = torch.zeros(total, dtype=torch.float32, device=self.dev)
         self.grads = torch.zeros(total, dtype=torch.float32, device=self.dev)
         self.exp_avg = torch.zeros(total, dtype=torch.float32, device=self.dev)
         self.exp_avg_sq = torch.zeros(total, dtype=torch.float32, device=self.dev)
-        for name, k in SEGMENTS:
+        for name, k in self.widths:
             p_, m_, v_ = new[name]
             self.view(self.params, name).copy_(p_.reshape(new_P, k))
             self.view(self.exp_avg, name).copy_(m_.reshape(new_P, k))
@@ -962,7 +1003,7 @@ class JointTrainer:
         ext = dict(xyz=new_xyz, f_dc=new_features_dc, f_rest=new_features_rest, opacity=new_opacities,
                    scaling=new_scaling, rotation=new_rotation)
         n_new = int(new_xyz.shape[0])
-        k_of = dict(SEGMENTS)
+        k_of = dict(self.widths)
         ppl = None
         if self.per_point_lr is not None:
             add = torch.ones(n_new, device=self.dev) if new_per_point_lr is None else \
@@ -1004,7 +1045,7 @@ class JointTrainer:
 
     # ---- save points (train.py:103-105, :220-227; DESIGN.md section 4.9) ---------------------------------------
     def _shapes(self):
-        m1 = dict(SEGMENTS)["f_rest"] // 3
+        m1 = self.sh_coeffs - 1
         return dict(xyz=(self.P, 3), f_dc=(self.P, 1, 3), f_rest=(self.P, m1, 3), opacity=(self.P, 1),
                     scaling=(self.P, 3), rotation=(self.P, 4))
 
@@ -1021,10 +1062,10 @@ class JointTrainer:
         if self.world_size > 1:
             raise _lib.GsbError("checkpoints need world_size == 1: the fused exchange shards the Adam moments")
         shapes = self._shapes()
-        prm = {name: nn.Parameter(self.view(self.params, name).reshape(shapes[name]).clone()) for name, _ in SEGMENTS}
+        prm = {name: nn.Parameter(self.view(self.params, name).reshape(shapes[name]).clone()) for name, _ in self.widths}
         pose = nn.Parameter(self.poses.clone())
         groups, state = [], {}
-        for i, ((name, _), lr) in enumerate(zip(SEGMENTS + (("pose", 7),), self._group_lrs())):
+        for i, ((name, _), lr) in enumerate(zip(self.widths + (("pose", 7),), self._group_lrs())):
             ppl = None
             if name == "xyz" and self.per_point_lr is not None:
                 ppl = self.per_point_lr[:self.P].reshape(self.P, 1).clone()
@@ -1101,8 +1142,14 @@ class JointTrainer:
         shapes = self._shapes()
         m1 = shapes["f_rest"][1]
         if tuple(t["f_rest"].shape[1:]) != (m1, 3):
+            rows = t["f_rest"].shape[1]
+            d = int(round((rows + 1) ** 0.5)) - 1
+            held = f"SH degree {d}" if (d + 1) ** 2 == rows + 1 else f"{rows} SH rows"
             raise _lib.GsbError(f"checkpoint: f_rest is {tuple(t['f_rest'].shape)}, the trainer's SH layout needs "
-                                f"[P,{m1},3]")
+                                f"[P,{m1},3]" + ("" if self.stored_sh_degree == 3 else
+                                                 f" (the checkpoint holds {held}, the trainer's scene SH degree "
+                                                 f"{self.stored_sh_degree}; build the trainer on a scene of the "
+                                                 "checkpoint's degree)"))
         if not 0 <= t["active_sh_degree"] <= self.cfg.max_sh_degree:
             raise _lib.GsbError(f"checkpoint: active_sh_degree {t['active_sh_degree']} is out of range")
         if extra is not None:
@@ -1115,15 +1162,15 @@ class JointTrainer:
                                     ", ".join(f"{k} {fr.get(k)} != {mine[k]}" for k in bad))
         steps = t["steps"]
         if extra is not None:
-            opt_step, lag = int(extra["opt_step"]), {name: int(extra["lag"][name]) for name, _ in SEGMENTS}
-            want = {name: opt_step - lag[name] for name, _ in SEGMENTS if opt_step - lag[name] > 0}
+            opt_step, lag = int(extra["opt_step"]), {name: int(extra["lag"][name]) for name, _ in self.widths}
+            want = {name: opt_step - lag[name] for name, _ in self.widths if opt_step - lag[name] > 0}
             if "pose" in steps:
                 want["pose"] = opt_step
             if steps != want:
                 raise _lib.GsbError(f"checkpoint: step counts {steps} disagree with opt_step {opt_step} and the lags")
         else:
-            opt_step = steps.get("pose", 0) or max(steps.get(name, 0) for name, _ in SEGMENTS)
-            lag = {name: opt_step - steps.get(name, 0) for name, _ in SEGMENTS}
+            opt_step = steps.get("pose", 0) or max(steps.get(name, 0) for name, _ in self.widths)
+            lag = {name: opt_step - steps.get(name, 0) for name, _ in self.widths}
         dev = self.dev
         self.poses.copy_(t["pose"].to(dev))
         for buf, key in ((self.pose_m, "m"), (self.pose_v, "v")):
@@ -1135,7 +1182,7 @@ class JointTrainer:
                                  t["max_radii2D"].reshape(P))).to(dev).float()
 
         def rows(name, p, m, v):
-            k = dict(SEGMENTS)[name]
+            k = dict(self.widths)[name]
             new = t[name].detach().to(dev).float().reshape(P, k)
             mv = t["moments"].get(name)
             if mv is None:
@@ -1195,7 +1242,8 @@ class JointTrainer:
         """SURVEY.md section 8(d) per-kernel algorithmic HBM bytes for the last step (fp32)."""
         P, R, HW = self.P, self.last_R, self.W * self.H
         T = ((self.W + 15) // 16) * ((self.H + 15) // 16)
-        K = (self.sh_degree + 1) ** 2
+        K = (min(self.sh_degree, self.stored_sh_degree) + 1) ** 2
+        F = sum(k for _, k in self.widths)          # floats per Gaussian in each flat buffer: 14 / 23 / 38 / 59 at D = 0..3
         V = P
         return dict(
             preprocess_fwd=P * (12 + 12 + 16 + 4) + V * 12 * K + V * (8 + 4 + 16 + 12 + 4) + P * 4,
@@ -1203,7 +1251,7 @@ class JointTrainer:
             blend_bwd=R * 40 + HW * 20 + T * 8 + V * 36,
             preprocess_bwd=P * 44 + V * (12 * K + 36) + P * 44 + V * 12 * K,
             loss=HW * 36,
-            adam=59 * P * 28 + P * 4,
+            adam=F * P * 28 + P * 4,
         )
 
 
