@@ -277,6 +277,19 @@ GSB_API int gsb_backward_batch_stats(const GsbCamera* cam, const GsbGaussians* g
                                      int32_t n_stats, const GsbDensifyStats* stats, const float* poses7, void* geom,
                                      void* binning, int64_t R, void* image, const float* dL_dout,
                                      const GsbGrads* grads, float* dpose7, gsb_stream_t stream);
+/* Per-view backgrounds (JointTrainer's random background): gsb_render_batch and gsb_backward_batch_stats with view v
+ * blended over bg[3 v .. 3 v + 2] of a device [V, 3] fp32 table instead of cam->bg (which is then not read by the
+ * blend).  Each view's image and gradients are bit-identical to those of the shared-background call with cam->bg
+ * holding that view's row.  The backward must get the table its forward used.  Only blend version 2 (the default)
+ * takes a table; with gsb_set_option("blend_version", 1) both return GSB_ERR_INVALID. */
+GSB_API int gsb_render_batch_bg(const GsbCamera* cam, int32_t P, int32_t V, const float* bg, void* geom, void* binning,
+                                size_t binning_bytes, int64_t R, void* image, float* out_color, uint32_t* status_host,
+                                gsb_stream_t stream);
+GSB_API int gsb_backward_batch_stats_bg(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, int32_t V,
+                                        const float* bg, int32_t n_stats, const GsbDensifyStats* stats,
+                                        const float* poses7, void* geom, void* binning, int64_t R, void* image,
+                                        const float* dL_dout, const GsbGrads* grads, float* dpose7,
+                                        gsb_stream_t stream);
 /* gsb_loss_forward / gsb_loss_backward on V images img [V, C, H, W]: view v's target is the [C, H, W] block
  * gt + gt_row[v] * C*H*W (gt_row: device int32 [V], so that one captured launch serves any choice of targets).
  * sums [V, 2] (double, caller zeroes), maps [3, V, C, H, W]; dL_dimg [V, C, H, W], each view scaled by 1/N with

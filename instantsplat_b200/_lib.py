@@ -82,7 +82,7 @@ EXPORTS = ("gsb_geom_bytes", "gsb_binning_bytes", "gsb_image_bytes", "gsb_prepro
            "gsb_track_step_batch", "gsb_backward_batch", "gsb_loss_forward_batch", "gsb_loss_backward_batch",
            "gsb_backward_batch_stats", "gsb_image_metrics_scratch_bytes", "gsb_image_metrics_batch",
            "gsb_frames_u8_batch", "gsb_lpips_scratch_bytes", "gsb_lpips_prepare", "gsb_lpips_conv3x3_relu",
-           "gsb_lpips_maxpool2", "gsb_lpips_head")
+           "gsb_lpips_maxpool2", "gsb_lpips_head", "gsb_render_batch_bg", "gsb_backward_batch_stats_bg")
 KERNEL_IDS = ("preprocess", "sort_depth", "scan", "duplicate", "sort_tile", "gather", "blend_fwd", "blend_bwd",
               "preprocess_bwd", "loss_fwd", "loss_bwd", "adam")
 
@@ -163,6 +163,10 @@ def lib() -> ctypes.CDLL:
     L.gsb_backward_batch_stats.argtypes = [ctypes.POINTER(GsbCamera), ctypes.POINTER(GsbGaussians),
                                            ctypes.POINTER(GsbFilter), i32, i32, ctypes.POINTER(GsbDensifyStats), vp, vp,
                                            vp, i64, vp, vp, ctypes.POINTER(GsbGrads), vp, vp]
+    L.gsb_render_batch_bg.argtypes = [ctypes.POINTER(GsbCamera), i32, i32, vp, vp, vp, sz, i64, vp, vp, vp, vp]
+    L.gsb_backward_batch_stats_bg.argtypes = [ctypes.POINTER(GsbCamera), ctypes.POINTER(GsbGaussians),
+                                              ctypes.POINTER(GsbFilter), i32, vp, i32, ctypes.POINTER(GsbDensifyStats),
+                                              vp, vp, vp, i64, vp, vp, ctypes.POINTER(GsbGrads), vp, vp]
     L.gsb_loss_forward_batch.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
     L.gsb_loss_backward_batch.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, ctypes.c_float, vp, vp]
     L.gsb_image_metrics_scratch_bytes.restype = sz
@@ -178,7 +182,8 @@ def lib() -> ctypes.CDLL:
     for f in ("gsb_preprocess_batch", "gsb_render_batch", "gsb_backward_pose_batch", "gsb_l1_mask_fwd_bwd_batch",
               "gsb_track_step_batch", "gsb_backward_batch", "gsb_loss_forward_batch", "gsb_loss_backward_batch",
               "gsb_backward_batch_stats", "gsb_image_metrics_batch", "gsb_frames_u8_batch", "gsb_lpips_prepare",
-              "gsb_lpips_conv3x3_relu", "gsb_lpips_maxpool2", "gsb_lpips_head"):
+              "gsb_lpips_conv3x3_relu", "gsb_lpips_maxpool2", "gsb_lpips_head", "gsb_render_batch_bg",
+              "gsb_backward_batch_stats_bg"):
         getattr(L, f).restype = ctypes.c_int
     L.gsb_adam_step_gated.argtypes = [i32, ctypes.POINTER(GsbAdamTensor), vp, vp, vp]
     L.gsb_adam_step_gated.restype = ctypes.c_int

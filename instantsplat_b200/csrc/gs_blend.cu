@@ -458,7 +458,7 @@ __device__ __forceinline__ float2 f2s(float a) { return make_float2(a, a); }
 template <bool BULK, bool STATS = false>
 __global__ void __launch_bounds__(kThreads2, GSB_FWD_MINB)
 k_blend_fwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids, const float4* __restrict__ rec,
-             const float* __restrict__ bg, int W, int H, int gx,
+             const float* __restrict__ bg, int bg_stride, int W, int H, int gx,
              float* __restrict__ out_color, float* __restrict__ final_T, uint32_t* __restrict__ n_contrib,
              unsigned long long* __restrict__ stats = nullptr) {
   unsigned int st_iter = 0, st_valid = 0;
@@ -557,6 +557,7 @@ k_blend_fwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids,
     if (lane == 0) { atomicAdd(stats + 0, (unsigned long long)st_iter); atomicAdd(stats + 1, (unsigned long long)st_valid); }
   }
   const size_t hw = (size_t)W * H;
+  bg += (size_t)blockIdx.y * bg_stride;            // view v's background: a [V, 3] table (3) or one shared (0)
   const float b0 = bg[0], b1 = bg[1], b2 = bg[2];
   if (inA) {
     size_t pix = (size_t)pyA * W + px;
@@ -624,7 +625,7 @@ __device__ __forceinline__ void batch_flush(const float (*rows)[kBatchRow], int 
 template <bool BULK, bool STATS = false, bool POSE_ONLY = false, bool BATCH = true>
 __global__ void __launch_bounds__(kThreads2, BATCH ? GSB_BWD_MINB : kBwdMinBFly)
 k_blend_bwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids, const float4* __restrict__ rec,
-             const float* __restrict__ bg, int W, int H, int gx,
+             const float* __restrict__ bg, int bg_stride, int W, int H, int gx,
              const float* __restrict__ final_T, const uint32_t* __restrict__ n_contrib,
              const float* __restrict__ dL_dpix, unsigned long long* __restrict__ dacc,
              const uint32_t* __restrict__ dscale, unsigned long long* __restrict__ stats = nullptr) {
@@ -659,6 +660,7 @@ k_blend_bwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids,
   float2 dLr = f2(0.f, 0.f), dLg = f2(0.f, 0.f), dLb = f2(0.f, 0.f);
   if (inA) { dLr.x = dL_dpix[pixA]; dLg.x = dL_dpix[hw + pixA]; dLb.x = dL_dpix[2 * hw + pixA]; }
   if (inB) { dLr.y = dL_dpix[pixB]; dLg.y = dL_dpix[hw + pixB]; dLb.y = dL_dpix[2 * hw + pixB]; }
+  bg += (size_t)blockIdx.y * bg_stride;            // the forward's background of this view
   const float b0 = bg[0], b1 = bg[1], b2 = bg[2];
   const float2 tf_bg = mul2(T_final, f2(b0 * dLr.x + b1 * dLg.x + b2 * dLb.x, b0 * dLr.y + b1 * dLg.y + b2 * dLb.y));
   int wmaxA = lcA, wmaxB = lcB;
@@ -797,17 +799,19 @@ k_blend_bwd2(const uint2* __restrict__ ranges, const uint32_t* __restrict__ ids,
 
 }  // namespace
 
-int gsb_launch_blend_fwd(const GeomView& gv, const BinView& bv, const ImgView& iv, const float* bg, int W, int H, int V,
-                         float* out_color, cudaStream_t st) {
+int gsb_launch_blend_fwd(const GeomView& gv, const BinView& bv, const ImgView& iv, const float* bg, int bg_stride,
+                         int W, int H, int V, float* out_color, cudaStream_t st) {
   const int gx = (W + kBlock - 1) / kBlock;
   const dim3 grid(gx * ((H + kBlock - 1) / kBlock), V);
-  ProfScope ps(GSB_K_BLEND_FWD, st);
   const int ver = gsb_option_blend_version(), bulk = gsb_option_stage_bulk();
+  GSB_REQUIRE(bg_stride == 0 || bg_stride == 3, "background stride must be 0 (shared) or 3 (one row per view)");
+  GSB_REQUIRE(bg_stride == 0 || ver == 2, "blend version 1 takes one shared background, not a per-view table");
+  ProfScope ps(GSB_K_BLEND_FWD, st);
   if (ver == 2 && bulk)
-    k_blend_fwd2<true><<<grid, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, out_color,
+    k_blend_fwd2<true><<<grid, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, bg_stride, W, H, gx, out_color,
                                                    iv.final_T, iv.n_contrib);
   else if (ver == 2)
-    k_blend_fwd2<false><<<grid, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, out_color,
+    k_blend_fwd2<false><<<grid, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, bg_stride, W, H, gx, out_color,
                                                     iv.final_T, iv.n_contrib);
   else
     k_blend_fwd<<<grid, kThreads, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, out_color, iv.final_T,
@@ -816,10 +820,13 @@ int gsb_launch_blend_fwd(const GeomView& gv, const BinView& bv, const ImgView& i
   return GSB_OK;
 }
 
-int gsb_launch_blend_bwd(const GeomView& gv, const BinView& bv, const ImgView& iv, const float* bg, int W, int H, int V,
-                         const float* dL_dout, bool pose_only, cudaStream_t st) {
+int gsb_launch_blend_bwd(const GeomView& gv, const BinView& bv, const ImgView& iv, const float* bg, int bg_stride,
+                         int W, int H, int V, const float* dL_dout, bool pose_only, cudaStream_t st) {
   const int gx = (W + kBlock - 1) / kBlock;
   const dim3 grid(gx * ((H + kBlock - 1) / kBlock), V);
+  GSB_REQUIRE(bg_stride == 0 || bg_stride == 3, "background stride must be 0 (shared) or 3 (one row per view)");
+  GSB_REQUIRE(bg_stride == 0 || gsb_option_blend_version() == 2,
+              "blend version 1 takes one shared background, not a per-view table");
   ProfScope ps(GSB_K_BLEND_BWD, st, 2);
   const size_t n = (size_t)3 * W * H;
   const size_t nb = (n + kThreads - 1) / kThreads, max_blocks = 4 * (size_t)gsb_sm_count();
@@ -828,8 +835,8 @@ int gsb_launch_blend_bwd(const GeomView& gv, const BinView& bv, const ImgView& i
   const bool batch = gsb_option_blend_bwd_batch();
   unsigned long long* dacc = gv.dacc;
   auto v2 = [&](auto kernel) {
-    kernel<<<grid, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, W, H, gx, iv.final_T, iv.n_contrib, dL_dout, dacc,
-                                       gv.dscale, nullptr);
+    kernel<<<grid, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, bg, bg_stride, W, H, gx, iv.final_T, iv.n_contrib,
+                                       dL_dout, dacc, gv.dscale, nullptr);
   };
   if (pose_only)
     batch ? v2(k_blend_bwd2<true, false, true, true>) : v2(k_blend_bwd2<true, false, true, false>);
@@ -860,10 +867,10 @@ extern "C" GSB_API int gsb_blend_stats(const GsbCamera* cam, int32_t P, void* ge
   BinView bv = bin_view(binning, R, W, H);
   ImgView iv = img_view(image, W, H);
   GSB_CUDA(cudaMemsetAsync(stats, 0, 8 * sizeof(unsigned long long), st));
-  k_blend_fwd2<true, true><<<gx * gy, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, cam->bg, W, H, gx, out_color,
+  k_blend_fwd2<true, true><<<gx * gy, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, cam->bg, 0, W, H, gx, out_color,
                                                           iv.final_T, iv.n_contrib, stats);
   if (dL_dout)
-    k_blend_bwd2<true, true><<<gx * gy, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, cam->bg, W, H, gx, iv.final_T,
+    k_blend_bwd2<true, true><<<gx * gy, kThreads2, 0, st>>>(bv.ranges, bv.ids, gv.rec, cam->bg, 0, W, H, gx, iv.final_T,
                                                             iv.n_contrib, dL_dout, gv.dacc, gv.dscale, stats);
   GSB_CUDA(cudaGetLastError());
   return GSB_OK;

@@ -211,11 +211,11 @@ int gsb_launch_big_rects(int P, int V, const gsb::GeomView& gv, unsigned long lo
 // scatter + per-tile (depth, id) sort + slab gather + ranges; cap = instance capacity of the binning buffer
 int gsb_launch_binning(int P, int V, const gsb::GeomView& gv, const gsb::BinView& bv, int W, int H, int exact_cull,
                        uint32_t cap, cudaStream_t st);
-// out_color [V, 3, H, W]
-int gsb_launch_blend_fwd(const gsb::GeomView& gv, const gsb::BinView& bv, const gsb::ImgView& iv, const float* bg, int W, int H,
-                         int V, float* out_color, cudaStream_t st);
+// out_color [V, 3, H, W]; view v's background is bg + v * bg_stride (0: one shared [3], 3: a [V, 3] table; v2 only)
+int gsb_launch_blend_fwd(const gsb::GeomView& gv, const gsb::BinView& bv, const gsb::ImgView& iv, const float* bg,
+                         int bg_stride, int W, int H, int V, float* out_color, cudaStream_t st);
 // pose_only: 8-value accumulator layout (dacc[5] = dL/db, no dL/dopacity), see k_blend_bwd2
 // computes max |dL_dout| into gv.dscale (zeroed by the caller, as is gv.dacc), then the blend backward into gv.dacc
-// dL_dout [V, 3, H, W]; one M per view (gv.dscale[v])
-int gsb_launch_blend_bwd(const gsb::GeomView& gv, const gsb::BinView& bv, const gsb::ImgView& iv, const float* bg, int W, int H,
-                         int V, const float* dL_dout, bool pose_only, cudaStream_t st);
+// dL_dout [V, 3, H, W]; one M per view (gv.dscale[v]); bg, bg_stride as in gsb_launch_blend_fwd
+int gsb_launch_blend_bwd(const gsb::GeomView& gv, const gsb::BinView& bv, const gsb::ImgView& iv, const float* bg,
+                         int bg_stride, int W, int H, int V, const float* dL_dout, bool pose_only, cudaStream_t st);

@@ -1055,8 +1055,10 @@ extern "C" GSB_API int gsb_preprocess(const GsbCamera* cam, const GsbGaussians* 
   return gsb_preprocess_ex(cam, g, nullptr, geom, geom_bytes, radii, status_host, stream);
 }
 
+// bg_table: [V, 3] backgrounds, view v's at bg_table + 3 v (NULL: cam->bg for every view)
 static int render_views(const GsbCamera* cam, int32_t P, int V, void* geom, void* binning, size_t binning_bytes,
-                        int64_t R, void* image, float* out_color, uint32_t* status_host, cudaStream_t st) {
+                        int64_t R, void* image, float* out_color, uint32_t* status_host, cudaStream_t st,
+                        const float* bg_table = nullptr) {
   GSB_REQUIRE(cam && geom && binning && image && out_color, "null buffer");
   GSB_REQUIRE(R >= 0 && R < (int64_t)0x7fffffff, "R out of range");
   GSB_REQUIRE(V >= 1 && V <= 65535 && P >= 0 && (long long)V * P < 0x7fffffffLL, "bad V / P");
@@ -1067,7 +1069,7 @@ static int render_views(const GsbCamera* cam, int32_t P, int V, void* geom, void
   ImgView iv = img_view(image, W, H, V);
   int rc = gsb_launch_binning(P, V, gv, bv, W, H, cam->exact_cull, (uint32_t)R, st);
   if (rc) return rc;
-  rc = gsb_launch_blend_fwd(gv, bv, iv, cam->bg, W, H, V, out_color, st);
+  rc = gsb_launch_blend_fwd(gv, bv, iv, bg_table ? bg_table : cam->bg, bg_table ? 3 : 0, W, H, V, out_color, st);
   if (rc) return rc;
   if (status_host) GSB_CUDA(cudaMemcpyAsync(status_host, gv.status, 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   GSB_CUDA(cudaGetLastError());
@@ -1085,9 +1087,18 @@ extern "C" GSB_API int gsb_render_batch(const GsbCamera* cam, int32_t P, int32_t
   return render_views(cam, P, V, geom, binning, binning_bytes, R, image, out_color, status_host, (cudaStream_t)stream);
 }
 
+extern "C" GSB_API int gsb_render_batch_bg(const GsbCamera* cam, int32_t P, int32_t V, const float* bg, void* geom,
+                                           void* binning, size_t binning_bytes, int64_t R, void* image,
+                                           float* out_color, uint32_t* status_host, gsb_stream_t stream) {
+  GSB_REQUIRE(bg, "gsb_render_batch_bg: null background table");
+  return render_views(cam, P, V, geom, binning, binning_bytes, R, image, out_color, status_host, (cudaStream_t)stream,
+                      bg);
+}
+
 static int backward_views(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, const GsbDensifyStats* stats,
                           int V, void* geom, void* binning, int64_t R, void* image, const float* dL_dout,
-                          const GsbGrads* grads, cudaStream_t st, bool sum_views = false, int n_stats = 1);
+                          const GsbGrads* grads, cudaStream_t st, bool sum_views = false, int n_stats = 1,
+                          const float* bg_table = nullptr);
 
 extern "C" GSB_API int gsb_backward_stats(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt,
                                           const GsbDensifyStats* stats, void* geom, void* binning, int64_t R, void* image,
@@ -1107,11 +1118,10 @@ extern "C" GSB_API int gsb_backward_pose_batch(const GsbCamera* cam, const GsbGa
   return backward_views(cam, &gb, filt, nullptr, V, geom, binning, R, image, dL_dout, &gr, (cudaStream_t)stream);
 }
 
-extern "C" GSB_API int gsb_backward_batch_stats(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt,
-                                                int32_t V, int32_t n_stats, const GsbDensifyStats* stats,
-                                                const float* poses7, void* geom, void* binning, int64_t R, void* image,
-                                                const float* dL_dout, const GsbGrads* grads, float* dpose7,
-                                                gsb_stream_t stream) {
+static int backward_batch(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, int32_t V, int32_t n_stats,
+                          const GsbDensifyStats* stats, const float* bg_table, const float* poses7, void* geom,
+                          void* binning, int64_t R, void* image, const float* dL_dout, const GsbGrads* grads,
+                          float* dpose7, gsb_stream_t stream) {
   GSB_REQUIRE(n_stats >= 0 && n_stats <= V, "gsb_backward_batch_stats: n_stats must be in 0..V");
   GSB_REQUIRE(stats || n_stats == 0, "gsb_backward_batch_stats: n_stats > 0 needs statistics");
   GSB_REQUIRE(g && poses7 && grads && dpose7, "gsb_backward_batch: null gaussians / poses / grads / dpose");
@@ -1122,7 +1132,26 @@ extern "C" GSB_API int gsb_backward_batch_stats(const GsbCamera* cam, const GsbG
   GsbGrads gr = *grads;
   gr.dL_dpose = dpose7;
   return backward_views(cam, &gb, filt, stats, V, geom, binning, R, image, dL_dout, &gr, (cudaStream_t)stream, true,
-                        n_stats);
+                        n_stats, bg_table);
+}
+
+extern "C" GSB_API int gsb_backward_batch_stats(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt,
+                                                int32_t V, int32_t n_stats, const GsbDensifyStats* stats,
+                                                const float* poses7, void* geom, void* binning, int64_t R, void* image,
+                                                const float* dL_dout, const GsbGrads* grads, float* dpose7,
+                                                gsb_stream_t stream) {
+  return backward_batch(cam, g, filt, V, n_stats, stats, nullptr, poses7, geom, binning, R, image, dL_dout, grads, dpose7,
+                        stream);
+}
+
+extern "C" GSB_API int gsb_backward_batch_stats_bg(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt,
+                                                   int32_t V, const float* bg, int32_t n_stats,
+                                                   const GsbDensifyStats* stats, const float* poses7, void* geom,
+                                                   void* binning, int64_t R, void* image, const float* dL_dout,
+                                                   const GsbGrads* grads, float* dpose7, gsb_stream_t stream) {
+  GSB_REQUIRE(bg, "gsb_backward_batch_stats_bg: null background table");
+  return backward_batch(cam, g, filt, V, n_stats, stats, bg, poses7, geom, binning, R, image, dL_dout, grads, dpose7,
+                        stream);
 }
 
 extern "C" GSB_API int gsb_backward_batch(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, int32_t V,
@@ -1140,7 +1169,7 @@ extern "C" GSB_API int gsb_backward_batch(const GsbCamera* cam, const GsbGaussia
 // single view counts its statistics when stats is given.
 static int backward_views(const GsbCamera* cam, const GsbGaussians* g, const GsbFilter* filt, const GsbDensifyStats* stats,
                           int V, void* geom, void* binning, int64_t R, void* image, const float* dL_dout,
-                          const GsbGrads* grads, cudaStream_t st, bool sum_views, int n_stats) {
+                          const GsbGrads* grads, cudaStream_t st, bool sum_views, int n_stats, const float* bg_table) {
   int rc = batch_args(V, cam, g);
   if (rc) return rc;
   InPtrs in;
@@ -1172,7 +1201,8 @@ static int backward_views(const GsbCamera* cam, const GsbGaussians* g, const Gsb
                          !grads->dL_drotations && !grads->dL_dopacities && !grads->dL_dsh_dc && !grads->dL_dsh_rest &&
                          !grads->dL_dcolors && !grads->dL_dcov3D && gsb_option_blend_version() == 2 &&
                          gsb_option_stage_bulk() == 1;
-  rc = gsb_launch_blend_bwd(gv, bv, iv, cam->bg, W, H, V, dL_dout, pose_only, st);
+  rc = gsb_launch_blend_bwd(gv, bv, iv, bg_table ? bg_table : cam->bg, bg_table ? 3 : 0, W, H, V, dL_dout, pose_only,
+                            st);
   if (rc) return rc;
   OutPtrs out;
   out.dmeans = grads->dL_dmeans3D; out.dmeans2D = grads->dL_dmeans2D; out.dscales = grads->dL_dscales;

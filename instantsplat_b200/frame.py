@@ -119,6 +119,14 @@ def _f(filt):
     return None if filt is None else ctypes.byref(filt)
 
 
+def _bg_table(bg, views) -> None:
+    """Refuse a per-view background table that is not a contiguous fp32 [views, 3] CUDA tensor."""
+    if not (isinstance(bg, torch.Tensor) and bg.is_cuda and bg.dtype == torch.float32 and bg.is_contiguous() and
+            tuple(bg.shape) == (views, 3)):
+        raise _lib.GsbError(f"background table: expected a contiguous float32 [{views}, 3] CUDA tensor, got "
+                            f"{getattr(bg, 'dtype', type(bg))} {tuple(getattr(bg, 'shape', ()))}")
+
+
 class Frame:
     """Scratch of forwards at one (device, P, W, H): the geometry buffer (which holds the status words), radii, the
     image buffer, the rendered colour [3, H, W], and a binning buffer of `cap` instances (0: none yet).
@@ -196,11 +204,20 @@ class Frame:
                                               self.radii.data_ptr(), _p(host_status), _lib.stream_ptr()),
               "gsb_preprocess_batch")
 
-    def render_batch(self, cam, host_status=None) -> None:
-        check(_lib.lib().gsb_render_batch(ctypes.byref(cam), self.P, self.views, self.geom.data_ptr(),
-                                          self.binning.data_ptr(), self.binning.numel(), self.cap,
-                                          self.image.data_ptr(), self.color.data_ptr(), _p(host_status),
-                                          _lib.stream_ptr()), "gsb_render_batch")
+    def render_batch(self, cam, host_status=None, bg=None) -> None:
+        """bg: contiguous fp32 [views, 3] device tensor, view v blended over row v (gsb_render_batch_bg); None: cam's
+        background for every view."""
+        if bg is None:
+            check(_lib.lib().gsb_render_batch(ctypes.byref(cam), self.P, self.views, self.geom.data_ptr(),
+                                              self.binning.data_ptr(), self.binning.numel(), self.cap,
+                                              self.image.data_ptr(), self.color.data_ptr(), _p(host_status),
+                                              _lib.stream_ptr()), "gsb_render_batch")
+            return
+        _bg_table(bg, self.views)
+        check(_lib.lib().gsb_render_batch_bg(ctypes.byref(cam), self.P, self.views, bg.data_ptr(), self.geom.data_ptr(),
+                                             self.binning.data_ptr(), self.binning.numel(), self.cap,
+                                             self.image.data_ptr(), self.color.data_ptr(), _p(host_status),
+                                             _lib.stream_ptr()), "gsb_render_batch_bg")
 
     def backward_pose_batch(self, cam, g, poses7, dL_dimage, dpose7, filt=None) -> None:
         """dL_dimage [views, 3, H, W] -> dpose7 [views, 7] (pose gradients only)."""
@@ -209,11 +226,21 @@ class Frame:
                                                  self.cap, self.image.data_ptr(), dL_dimage.data_ptr(),
                                                  dpose7.data_ptr(), _lib.stream_ptr()), "gsb_backward_pose_batch")
 
-    def backward_batch(self, cam, g, poses7, dL_dimage, grads, dpose7, filt=None, stats=None, n_stats=0) -> None:
+    def backward_batch(self, cam, g, poses7, dL_dimage, grads, dpose7, filt=None, stats=None, n_stats=0,
+                       bg=None) -> None:
         """dL_dimage [views, 3, H, W] -> every per-Gaussian gradient of `grads` summed over the views in view order
         (bit-identical to single-view backwards added in that order), and dpose7 [views, 7].  stats: densify_stats(...)
         over this frame's [views, P] radii, or None; the same launch accumulates the statistics of views 0..n_stats-1,
-        bit-identical to single-view backwards with statistics made in view order."""
+        bit-identical to single-view backwards with statistics made in view order.  bg: the [views, 3] table the
+        forward was rendered over (render_batch), or None."""
+        if bg is not None:
+            _bg_table(bg, self.views)
+            check(_lib.lib().gsb_backward_batch_stats_bg(
+                ctypes.byref(cam), ctypes.byref(g), _f(filt), self.views, bg.data_ptr(), int(n_stats),
+                None if stats is None else ctypes.byref(stats), poses7.data_ptr(), self.geom.data_ptr(),
+                self.binning.data_ptr(), self.cap, self.image.data_ptr(), dL_dimage.data_ptr(), ctypes.byref(grads),
+                dpose7.data_ptr(), _lib.stream_ptr()), "gsb_backward_batch_stats_bg")
+            return
         check(_lib.lib().gsb_backward_batch_stats(ctypes.byref(cam), ctypes.byref(g), _f(filt), self.views, int(n_stats),
                                                   None if stats is None else ctypes.byref(stats), poses7.data_ptr(),
                                                   self.geom.data_ptr(), self.binning.data_ptr(), self.cap,

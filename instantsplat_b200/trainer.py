@@ -101,6 +101,11 @@ class OptimConfig:
     # events of the iterations a batch covers fired once at its end.  Off: step_batch refuses densify=True, so that a
     # run configured for train.py's per-iteration schedule does not move its events by switching to step_batch.
     densify_batches = False
+    # train.py's random background (DESIGN.md section 4.17), one GPU only: every iteration's forward and backward blend
+    # over a fresh colour, torch.rand((3), device="cuda") from a CUDA generator seeded with background_seed (safe_state's
+    # torch.manual_seed(0)).  render(), evaluate() and PoseTracker keep the scene's background.
+    random_background = False
+    background_seed = 0
 
 
 def lr_schedules(args, spatial_lr_scale):
@@ -217,6 +222,9 @@ class JointTrainer:
         if self.cfg.densify and world_size > 1:
             raise _lib.GsbError("densify=True needs world_size == 1: every rank would accumulate different "
                                 "densification statistics")
+        if self.cfg.random_background and world_size > 1:
+            raise _lib.GsbError("random_background=True needs world_size == 1: the ranks' views of one step would need "
+                                "consecutive colours of one shared sequence, which several GPUs do not draw")
         self.dev = torch.device(device)
         self.world_size, self.rank, self.pg = world_size, rank, process_group
         if exchange not in ("allreduce", "fused_p2p", "fused_p2p_nccl"):
@@ -320,6 +328,10 @@ class JointTrainer:
             self.densify_generator = torch.Generator(device=self.dev).manual_seed(int(c.densify_seed))
             self.white_background = bool((scene.bg == 1).all())
         self.densified_at, self.reset_at = [], []
+        # one generator for the run's background colours, drawn from outside any graph into the slots' fixed rows
+        self.background_generator = None
+        if c.random_background:
+            self.background_generator = torch.Generator(device=self.dev).manual_seed(int(c.background_seed))
         self._batch = None            # step_batch's slot for the view count of its last call (_batch_scratch)
         self._batch_sums = None       # per-view loss sums of the last step_batch (batch_loss_values)
 
@@ -390,8 +402,24 @@ class JointTrainer:
         return gaussians(self.P, *(self.view(p, n) for n in ("xyz", "rotation", "scaling", "opacity", "f_dc")),
                          self.view(p, "f_rest") if self.sh_coeffs > 1 else None, poses)
 
-    def _camera(self):
-        return self.ident.camera(self.active_sh_degree, self.sh_coeffs, self.exact_cull)
+    def _camera(self, bg: Optional[torch.Tensor] = None):
+        """The frame's camera at the active SH degree; bg: a [3] device tensor to blend over instead of the scene's."""
+        cam = self.ident.camera(self.active_sh_degree, self.sh_coeffs, self.exact_cull)
+        if bg is not None:
+            cam.bg = bg.data_ptr()
+        return cam
+
+    def _train_bg(self, slot: "_Slot") -> Optional[torch.Tensor]:
+        """The background a training forward on `slot` blends over: its drawn colours with random_background (step():
+        [3], step_batch: [V, 3]), else None (the scene's)."""
+        return slot.bg if self.background_generator is not None else None
+
+    def _draw_backgrounds(self, slot: "_Slot") -> None:
+        """train.py:164's bg = torch.rand((3), device="cuda") once for each iteration a step covers, into `slot`'s rows
+        (row k: iteration before + k + 1), on the current stream and outside any graph, so a graph reads the new colours
+        at the same address.  One torch draw of 3 per row: a single draw of [V, 3] would not give train.py's sequence."""
+        for row in slot.bg.view(-1, 3):
+            row.uniform_(0.0, 1.0, generator=self.background_generator)
 
     def _nonempty(self):
         """The (name, width) of the per-Gaussian tensors the kernels update: all six, but f_rest only above degree 0."""
@@ -402,10 +430,11 @@ class JointTrainer:
         """A binning buffer for R instances plus headroom, in `slot`'s frame (None: step()'s)."""
         (slot or self._single).frame.alloc_binning(capacity(R, self.headroom))
 
-    def _forward(self, slot: "_Slot", cam, g: GsbGaussians, poses: Optional[torch.Tensor] = None) -> None:
-        """Enqueue a forward of `slot`'s frame (poses: the [V, 7] rows of a batch slot) without ever waiting for the
-        GPU: the instance count R stays on the device; the host only provides a capacity (sized from the counts seen
-        so far, +50 %) and reads R back lazily."""
+    def _forward(self, slot: "_Slot", cam, g: GsbGaussians, poses: Optional[torch.Tensor] = None,
+                 bg: Optional[torch.Tensor] = None) -> None:
+        """Enqueue a forward of `slot`'s frame (poses: the [V, 7] rows of a batch slot; bg: its [V, 3] background
+        table, None: cam's background) without ever waiting for the GPU: the instance count R stays on the device; the
+        host only provides a capacity (sized from the counts seen so far, +50 %) and reads R back lazily."""
         fr, hs = slot.frame, slot.host_status
         if slot.V is None:
             fr.preprocess(cam, g, hs[0], self.filt)
@@ -418,10 +447,13 @@ class JointTrainer:
             if fr.cap == 0:                           # very first forward: size the buffer from the real count
                 self._ev_pre.synchronize()
                 self._size_binning(read_R(hs[0]), slot)
-        (fr.render if slot.V is None else fr.render_batch)(cam, hs[1])
+        if slot.V is None:
+            fr.render(cam, hs[1])
+        else:
+            fr.render_batch(cam, hs[1], bg)
 
-    def _launch_forward(self, view: int) -> None:
-        cam, g = self._camera(), self._gauss(self.poses[view])
+    def _launch_forward(self, view: int, bg: Optional[torch.Tensor] = None) -> None:
+        cam, g = self._camera(bg), self._gauss(self.poses[view])
         self._forward(self._single, cam, g)
         self._keep = (cam, g)
 
@@ -638,7 +670,7 @@ class JointTrainer:
     def _enqueue_iteration(self, view: int, gt: torch.Tensor, do_opt: bool, stats: bool = False) -> None:
         """One iteration on `view` with no wait, launched eagerly or captured into a graph: forward, loss + backward,
         the test hook, and (do_opt) the exchange and update with the step sizes _advance uploaded."""
-        self._launch_forward(view)
+        self._launch_forward(view, self._train_bg(self._single))
         self.loss_and_backward(view, gt, stats)
         if self._after_backward is not None:
             self._after_backward()
@@ -689,7 +721,8 @@ class JointTrainer:
         1000 iterations, render, loss, backward, optimizer step (skipped on the very last iteration, :209-211).
         With G GPUs one call consumes G views (one per rank): `iteration` counts VIEWS, so the learning-rate and
         SH-degree schedules advance per view as in the reference, while Adam's bias correction counts optimizer
-        steps.  Nothing in here waits for the GPU except `_settle()`, which waits for an event early in the stream."""
+        steps.  Nothing in here waits for the GPU except `_settle()`, which waits for an event early in the stream.
+        With cfg.random_background the iteration renders over its own colour (train.py:164), drawn once per call."""
         if gt is None:
             gt = self.gt[view]
         self._run_step(self.world_size, self._single, ("step", view, gt.data_ptr()),
@@ -710,6 +743,8 @@ class JointTrainer:
             de = batch_densify_events(c, self.iteration, n, self.white_background)
         n_stats = de["n_stats"]
         self.iteration = ev["iteration"]
+        if self.background_generator is not None:
+            self._draw_backgrounds(slot)   # once per step: a repeat after an overflow and an eager event reuse them
         if ev["sh_up"]:
             self.active_sh_degree = min(self.active_sh_degree + 1, c.max_sh_degree)     # oneupSHdegree
         do_opt = ev["do_opt"]
@@ -754,6 +789,8 @@ class JointTrainer:
         the order of `views`, each view's dL/dpose lands in its row of pose_grad (the other rows are zero); one Adam
         step with grad_scale = 1/V over the six tensors and the whole pose table (skipped at the last iteration).
         step_batch([v]) equals step(v) bit for bit.  The per-view losses stay on the device (batch_loss_values()).
+        With cfg.random_background, views[k] renders over the colour of iteration `iteration + k + 1` (the V colours
+        step() would draw over the same V iterations).
 
         With OptimConfig.densify, cfg.densify_batches must be set: each view whose iteration is below densify_until_iter
         adds its own statistics (batch_densify_events), and the densify / opacity-reset events of the iterations the
@@ -880,7 +917,8 @@ class JointTrainer:
         """Where a forward runs: a Frame, the pinned [2, ST_WORDS] buffer its status words are copied to ([0] after
         preprocess, [1] after render) and the count of its forwards.  Each frame numbers its forwards in its own status
         words and copies them to its own pinned buffer, so a serial number is only ever compared with the count of the
-        frame that wrote it (_settle).  V None: step()'s single view.  Otherwise step_batch's buffers for V views:
+        frame that wrote it (_settle); bg: the colours random_background draws for the slot's forward ([3], or [V, 3]
+        for a batch).  V None: step()'s single view.  Otherwise step_batch's buffers for V views:
         sel [2, V] (view ids, target rows; uploaded per call), the gathered poses and their gradients [V, 7],
         dL/dimage, loss maps and per-view loss sums."""
 
@@ -890,6 +928,7 @@ class JointTrainer:
             self.frame.status.zero_()          # the forward serial number lives in these words
             self.fwd_count = 0
             self.host_status = torch.zeros(2, ST_WORDS, dtype=torch.int32).pin_memory()
+            self.bg = torch.empty(3 if V is None else (V, 3), dtype=torch.float32, device=dev)
             if V is None:
                 return
             self.sel = torch.zeros(2, V, dtype=torch.int64, device=dev)
@@ -922,8 +961,8 @@ class JointTrainer:
         b.rows.copy_(b.sel[1])
         with torch.no_grad():          # a restored pose table may carry requires_grad from the checkpoint's Parameter
             torch.index_select(self.poses, 0, idx, out=b.poses)
-        cam, g = self._camera(), self._gauss(b.poses)
-        self._forward(b, cam, g, b.poses)
+        cam, g, bg = self._camera(), self._gauss(b.poses), self._train_bg(b)
+        self._forward(b, cam, g, b.poses, bg)
         b.sums.zero_()
         check(L.gsb_loss_forward_batch(V, 3, self.H, self.W, fr.color.data_ptr(), target.data_ptr(),
                                        b.rows.data_ptr(), b.sums.data_ptr(), b.maps.data_ptr(), st),
@@ -934,7 +973,7 @@ class JointTrainer:
         st = None
         if n_stats > 0:
             st = densify_stats(fr.radii, self._stats[0], self._stats[1], self._stats[2])
-        fr.backward_batch(cam, g, b.poses, b.dL, self._grads(), b.dpose, self.filt, st, n_stats)
+        fr.backward_batch(cam, g, b.poses, b.dL, self._grads(), b.dpose, self.filt, st, n_stats, bg)
         self.pose_grad.zero_()
         with torch.no_grad():
             self.pose_grad.index_copy_(0, idx, b.dpose)
@@ -1090,6 +1129,8 @@ class JointTrainer:
             cfg={k: getattr(c, k) for k in dir(OptimConfig) if not k.startswith("_")},
             frame=dict(W=self.W, H=self.H, fovx=self.fovx, fovy=self.fovy,
                        bg=[float(b) for b in self.ident.bg.tolist()], n_views=self.n_views, sh_degree=self.sh_degree))
+        if self.background_generator is not None:
+            extra["background_generator"] = self.background_generator.get_state()
         sd = {"state": state, "param_groups": groups, CHECKPOINT_KEY: extra}
         if self._stats is not None:
             accum, denom, radii = self.xyz_gradient_accum.clone(), self.denom.clone(), self.max_radii2D.clone()
@@ -1211,6 +1252,12 @@ class JointTrainer:
                 self.densify_generator.set_state(gen.cpu())
             else:
                 self.densify_generator.manual_seed(int(self.cfg.densify_seed))
+        if self.background_generator is not None:
+            gen = None if extra is None else extra.get("background_generator")
+            if gen is not None:
+                self.background_generator.set_state(gen.cpu())
+            else:
+                self.background_generator.manual_seed(int(self.cfg.background_seed))
 
     def save_ply(self, path: str) -> None:
         """scene.save: point_cloud.ply of the current Gaussians (with the filter_3D property when Mip is on)."""
@@ -1262,6 +1309,8 @@ CHECKPOINT_KEY = "joint_trainer"
 _GROUP_NAMES = tuple(name for name, _ in SEGMENTS) + ("pose",)
 _EXTRA_KEYS = ("iteration", "opt_step", "lag", "densify_generator", "scene_extent", "filter_3D", "mip_recomputed_at",
                "densified_at", "reset_at", "cfg", "frame")
+# ... and, from a run with random_background, "background_generator": the state of the colours' generator.  Optional: a
+# file without it (any other run's) continues the colours from background_seed.
 
 
 def read_checkpoint(path: str, device=None):
@@ -1337,5 +1386,8 @@ def _parse_capture(model_args, first_iter) -> dict:
             bad(f"first_iter {first_iter} differs from the saved iteration {extra['iteration']}")
         if extra["filter_3D"] is not None and extra["filter_3D"].numel() != P:
             bad("filter_3D must have one value per Gaussian")
+        bg_gen = extra.get("background_generator")
+        if bg_gen is not None and not (torch.is_tensor(bg_gen) and bg_gen.dtype == torch.uint8):
+            bad("background_generator must be a generator state (a uint8 tensor)")
     t.update(P=P, steps=steps, moments=moments, extra=extra, per_point_lr=None if ppl is None else ppl.reshape(P))
     return t
