@@ -290,14 +290,20 @@ def load_tracker(ply: str, width: int, height: int, fovx: float, fovy: float, wh
     """A PoseTracker over a saved point_cloud.ply as render.py renders it: the SH degree from the file's coefficient
     count, a black or white background, no Mip-Splatting filters."""
     from .scene_io import load_gaussians_ply
-    g = load_gaussians_ply(ply)
+    g = {k: torch.from_numpy(np.ascontiguousarray(a)) for k, a in load_gaussians_ply(ply).items()}
+    return tracker_from_gaussians(g, width, height, fovx, fovy, white_background, device, ply)
+
+
+def tracker_from_gaussians(g, width: int, height: int, fovx: float, fovy: float, white_background: bool = False,
+                           device="cuda", where: str = "the model") -> PoseTracker:
+    """load_tracker without the file: g holds load_gaussians_ply's tensors (JointTrainer.ply_tensors gives them from a
+    trainer).  Tensors already on the device, fp32 and contiguous are shared with the tracker, not copied."""
     M = 1 + g["f_rest"].shape[1]
     deg = int(round(M ** 0.5)) - 1
     if (deg + 1) ** 2 != M:
-        raise ValueError(f"{ply}: {M} SH coefficients per channel is not a square")
-    t = lambda k: torch.from_numpy(np.ascontiguousarray(g[k]))
+        raise ValueError(f"{where}: {M} SH coefficients per channel is not a square")
     bg = torch.ones(3) if white_background else torch.zeros(3)
-    return PoseTracker(t("xyz"), t("rotation"), t("scaling"), t("opacity"), t("f_dc"), t("f_rest"), width, height, fovx,
+    return PoseTracker(g["xyz"], g["rotation"], g["scaling"], g["opacity"], g["f_dc"], g["f_rest"], width, height, fovx,
                        fovy, bg=bg, sh_degree=deg, device=device)
 
 
@@ -316,12 +322,20 @@ def main(argv=None) -> int:
     if a.n_views < 2:
         raise SystemExit("--n_views must be at least 2: the fly-through joins consecutive key poses")
     tracker, keys, it = load(a.source_path, a.model_path, a.n_views, a.iterations, a.white_background)
-    path = interpolated_w2c(keys, a.n_views)
-    np.save(os.path.join(a.model_path, "pose", f"ours_{it}", "pose_interpolated.npy"), path)
-    folder = os.path.join(a.model_path, "interp", f"ours_{it}", "renders")
-    n = write_pngs(frames_u8(tracker, poses_from_w2c(path), a.max_batch), folder, a.workers)
+    n, folder = fly_through(tracker, keys, it, a.model_path, a.n_views, a.max_batch, a.workers)
     print(f"{n} frames -> {folder}")
     return 0
+
+
+def fly_through(tracker: PoseTracker, keys, it: int, model_path: str, n_views: int, max_batch: Optional[int] = None,
+                workers: Optional[int] = None, write=write_pngs) -> Tuple[int, str]:
+    """What main does after loading: pose/ours_<it>/pose_interpolated.npy from the key poses keys [n, 4, 4]
+    (pose_optimized.npy's rows), then the frames through write (write_pngs' signature) to interp/ours_<it>/renders.
+    Returns (frames, folder)."""
+    path = interpolated_w2c(keys, n_views)
+    np.save(os.path.join(model_path, "pose", f"ours_{it}", "pose_interpolated.npy"), path)
+    folder = os.path.join(model_path, "interp", f"ours_{it}", "renders")
+    return write(frames_u8(tracker, poses_from_w2c(path), max_batch), folder, workers), folder
 
 
 if __name__ == "__main__":

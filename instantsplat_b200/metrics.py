@@ -180,12 +180,14 @@ def lpips_numbers(renders: np.ndarray, gts: np.ndarray, net, device="cuda") -> t
     return net(f(renders), f(gts))[0].cpu()
 
 
-def evaluate_method(scene_dir: str, method: str, source_path: str, n_views: int, device="cuda", lpips_net=None):
+def evaluate_method(scene_dir: str, method: str, source_path: str, n_views: int, device="cuda", lpips_net=None,
+                    pairs=None):
     """One test/<method> of one model directory: writes test/<method>/metrics.txt and (when the pose inputs exist)
     pose/<method>/pose_eval.txt.  Returns (full, per_view) entries for results.json and per_view.json.  LPIPS is
-    measured with lpips_net (an lpips.LpipsVGG) when it is given."""
+    measured with lpips_net (an lpips.LpipsVGG) when it is given.  pairs: what read_pairs would return for the method,
+    held in memory (renders and gts uint8 [V, H, W, 3] in sorted file-name order, the names); None reads the files."""
     method_dir = os.path.join(scene_dir, "test", method)
-    renders, gts, names = read_pairs(method_dir)
+    renders, gts, names = read_pairs(method_dir) if pairs is None else pairs
     m = image_numbers(renders, gts, device)
     psnr, ssim = m["PSNR"].tolist(), m["SSIM"].tolist()
     lp = lpips_numbers(renders, gts, lpips_net, device) if lpips_net is not None else None
@@ -224,9 +226,11 @@ def evaluate_method(scene_dir: str, method: str, source_path: str, n_views: int,
     return full, per_view
 
 
-def evaluate(scene_dirs, source_path: str, n_views: int, device="cuda", lpips_net=None) -> int:
+def evaluate(scene_dirs, source_path: str, n_views: int, device="cuda", lpips_net=None, held=None) -> int:
     """metrics.py's evaluate over model directories: <scene>/results.json and <scene>/per_view.json for each.
-    Returns the number of model directories that could not be evaluated (each is reported with its reason)."""
+    Returns the number of model directories that could not be evaluated (each is reported with its reason).
+    held: {method: pairs} (evaluate_method's pairs) for methods whose images are in memory; the rest are read."""
+    held = held or {}
     failed = 0
     for scene_dir in scene_dirs:
         print("Scene:", scene_dir)
@@ -240,7 +244,7 @@ def evaluate(scene_dirs, source_path: str, n_views: int, device="cuda", lpips_ne
                     continue
                 print("Method:", method)
                 full[method], per_view[method] = evaluate_method(scene_dir, method, source_path, n_views, device,
-                                                                  lpips_net)
+                                                                  lpips_net, held.get(method))
         except (OSError, ValueError) as e:
             print(f"Unable to compute metrics for model {scene_dir}: {e}")
             failed += 1
@@ -252,7 +256,8 @@ def evaluate(scene_dirs, source_path: str, n_views: int, device="cuda", lpips_ne
     return failed
 
 
-def main(argv=None) -> int:
+def parser() -> argparse.ArgumentParser:
+    """metrics.py's command line as this stage reads it."""
     ap = argparse.ArgumentParser(prog="python -m instantsplat_b200.metrics",
                                  description="metrics.py: PSNR / SSIM (and LPIPS) of the test renders and the pose errors")
     ap.add_argument("-s", "--source_path", required=True)
@@ -261,6 +266,11 @@ def main(argv=None) -> int:
     ap.add_argument("--lpips_weights", metavar="DIR", default=None,
                     help=f"directory holding {LP.VGG_FILE} and {LP.LIN_FILE} (torch hub's checkpoints directory): "
                          "also report LPIPS (VGG)")
+    return ap
+
+
+def main(argv=None) -> int:
+    ap = parser()
     a = ap.parse_args(argv)
     net = None
     if a.lpips_weights is not None:

@@ -58,23 +58,24 @@ def tracker_for(model_path: str, it: int, views: Views, white_background: bool =
     return freeview.load_tracker(ply, views.width, views.height, views.fovx, views.fovy, white_background, device)
 
 
-def _write_gt(views: Views, folder: str, names, workers: Optional[int]) -> None:
+def _write_gt(views: Views, folder: str, names, workers: Optional[int], write=freeview.write_pngs) -> None:
     if not gt_round_trip_is_identity():
         raise RuntimeError("the 8-bit -> fp32 -> 8-bit round trip is not the identity; gt files cannot be copied")
-    freeview.write_pngs([(0, views.images)], folder, workers, names)
+    write([(0, views.images)], folder, workers, names)
 
 
 def render_train(tracker: PoseTracker, views: Views, w2c_opt, out_dir: str, max_batch: Optional[int] = None,
-                 workers: Optional[int] = None) -> torch.Tensor:
+                 workers: Optional[int] = None, write=freeview.write_pngs) -> torch.Tensor:
     """render_set("train"): views at the optimised world-to-camera matrices w2c_opt [V, 4, 4] (pose_optimized.npy,
-    one row per view) -> out_dir/renders/{idx:05d}.png and out_dir/gt/{idx:05d}.png.  Returns the 7-vectors [V, 7]."""
+    one row per view) -> out_dir/renders/{idx:05d}.png and out_dir/gt/{idx:05d}.png, each folder's frames handed to
+    write (freeview.write_pngs' signature).  Returns the 7-vectors [V, 7]."""
     w2c_opt = np.asarray(w2c_opt)
     if w2c_opt.ndim != 3 or w2c_opt.shape[0] != len(views):
         raise ValueError(f"render_train: {w2c_opt.shape[0] if w2c_opt.ndim == 3 else w2c_opt.shape} optimised poses "
                          f"for {len(views)} training views; loadCameras pairs them one to one")
     poses = freeview.poses_from_w2c(w2c_opt)
-    freeview.write_pngs(freeview.frames_u8(tracker, poses, max_batch), os.path.join(out_dir, "renders"), workers)
-    _write_gt(views, os.path.join(out_dir, "gt"), None, workers)
+    write(freeview.frames_u8(tracker, poses, max_batch), os.path.join(out_dir, "renders"), workers)
+    _write_gt(views, os.path.join(out_dir, "gt"), None, workers, write)
     return poses
 
 
@@ -87,17 +88,18 @@ def track(tracker: PoseTracker, views: Views, num_iter: int = 500, max_batch: Op
 
 
 def render_test(tracker: PoseTracker, views: Views, out_dir: str, num_iter: int = 500, max_batch: Optional[int] = None,
-                workers: Optional[int] = None) -> torch.Tensor:
-    """render_set_optimize: track, then out_dir/renders/<image_name>.png at the best poses and out_dir/gt/<image_name>.png.
-    Returns the best poses [V, 7]."""
+                workers: Optional[int] = None, write=freeview.write_pngs) -> torch.Tensor:
+    """render_set_optimize: track, then out_dir/renders/<image_name>.png at the best poses and out_dir/gt/<image_name>.png,
+    through write as in render_train.  Returns the best poses [V, 7]."""
     best = track(tracker, views, num_iter, max_batch)
     names = [n + ".png" for n in views.names]
-    freeview.write_pngs(freeview.frames_u8(tracker, best, max_batch), os.path.join(out_dir, "renders"), workers, names)
-    _write_gt(views, os.path.join(out_dir, "gt"), names, workers)
+    write(freeview.frames_u8(tracker, best, max_batch), os.path.join(out_dir, "renders"), workers, names)
+    _write_gt(views, os.path.join(out_dir, "gt"), names, workers, write)
     return best
 
 
-def main(argv=None) -> int:
+def parser() -> argparse.ArgumentParser:
+    """render.py's command line as this stage reads it."""
     ap = argparse.ArgumentParser(prog="python -m instantsplat_b200.render_views",
                                  description="render.py: the training views at their optimised poses, or (--eval) "
                                              "the test views after pose tracking")
@@ -113,7 +115,11 @@ def main(argv=None) -> int:
     ap.add_argument("--max_batch", type=int, default=12,
                     help="views per batched loop; tracking scratch is about 150 P + 44 H W bytes a view")
     ap.add_argument("--workers", type=int, default=None, help="PNG encoder threads (default: up to 8)")
-    a = ap.parse_args(argv)
+    return ap
+
+
+def main(argv=None) -> int:
+    a = parser().parse_args(argv)
     if a.max_batch < 1:
         raise SystemExit("--max_batch must be at least 1")
     if a.infer_video and not a.eval:

@@ -374,11 +374,17 @@ def load_gaussians_ply(path: str) -> Dict[str, np.ndarray]:
     return out
 
 
-def save_pose_npy(path: str, poses7: np.ndarray, colmap_ids: List[int] = None) -> np.ndarray:
-    """train.py:46-60: [n,7] quaternion poses -> [n,4,4] w2c matrices, row i = the camera with COLMAP id i+1."""
+def pose_matrices(poses7: np.ndarray, colmap_ids: List[int] = None) -> np.ndarray:
+    """train.py:46-60 without the file: [n,7] quaternion poses -> [n,4,4] fp32 w2c matrices, row i = the camera with
+    COLMAP id i+1."""
     n = poses7.shape[0]
     ids = list(range(1, n + 1)) if colmap_ids is None else list(colmap_ids)
-    mats = np.stack([pose7_to_matrix(poses7[ids.index(i + 1)]) for i in range(n)]).astype(np.float32)
+    return np.stack([pose7_to_matrix(poses7[ids.index(i + 1)]) for i in range(n)]).astype(np.float32)
+
+
+def save_pose_npy(path: str, poses7: np.ndarray, colmap_ids: List[int] = None) -> np.ndarray:
+    """train.py:46-60: [n,7] quaternion poses -> [n,4,4] w2c matrices, row i = the camera with COLMAP id i+1."""
+    mats = pose_matrices(poses7, colmap_ids)
     os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
     np.save(path, mats)
     return mats

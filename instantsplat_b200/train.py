@@ -316,13 +316,15 @@ class RunResult:
     """trainer: the JointTrainer at the end; rows: the pose row of each iteration run; first_iter: the iteration the
     run started after; losses [len(rows)] fp64 (CPU): each iteration's loss; phases: wall seconds per phase (load:
     PNG decode, PLY and confidence read; init: the Gaussians and targets on the GPU; trainer: trainer construction or
-    restore; loop: the iterations without their saves; saves: ply, pose and checkpoint files); colmap_ids."""
+    restore; loop: the iterations without their saves; saves: ply, pose and checkpoint files); colmap_ids; host: the
+    HostScene the run trained on (its views are the decoded training images)."""
     trainer: "object"
     rows: List[int]
     first_iter: int
     losses: torch.Tensor
     phases: Dict[str, float]
     colmap_ids: List[int]
+    host: HostScene
 
 
 def run(args: argparse.Namespace, device="cuda", log=print) -> RunResult:
@@ -422,7 +424,7 @@ def run(args: argparse.Namespace, device="cuda", log=print) -> RunResult:
     phases["loop"] = time.perf_counter() - t_loop - save_s
     phases["saves"] = save_s
     say("\nTraining complete.")
-    return RunResult(tr, rows, first_iter, tr._loss(ring[:n]).cpu(), phases, ids)
+    return RunResult(tr, rows, first_iter, tr._loss(ring[:n]).cpu(), phases, ids, host)
 
 
 def _device_scene(host: HostScene, sh_degree: int, white_background: bool, dev) -> TrainingScene:

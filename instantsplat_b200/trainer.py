@@ -1266,6 +1266,18 @@ class JointTrainer:
         save_gaussians_ply(path, v("xyz"), v("f_dc"), v("f_rest"), v("opacity"), v("scaling"), v("rotation"),
                            None if self.filter_3D is None else self.filter_3D.cpu().numpy())
 
+    def ply_tensors(self) -> Dict[str, torch.Tensor]:
+        """The Gaussians save_ply writes, as scene_io.load_gaussians_ply reads them back, without the file: device
+        copies (not views of the flat buffers) xyz [P,3], f_dc [P,1,3], f_rest [P,M-1,3] at the stored SH degree,
+        opacity [P,1], scaling [P,3], rotation [P,4]; and filter_3D [P,1] when Mip is on."""
+        P, w = self.P, dict(self.widths)
+        v = lambda name, *shape: self.view(self.params, name).reshape(P, *shape).clone()
+        out = dict(xyz=v("xyz", 3), f_dc=v("f_dc", 1, 3), f_rest=v("f_rest", w["f_rest"] // 3, 3),
+                   opacity=v("opacity", 1), scaling=v("scaling", 3), rotation=v("rotation", 4))
+        if self.filter_3D is not None:
+            out["filter_3D"] = self.filter_3D.reshape(P, 1).clone()
+        return out
+
     def save_poses(self, path: str, colmap_ids: Optional[List[int]] = None):
         """train.py save_pose: the pose table as [n_views,4,4] world-to-camera matrices in COLMAP id order."""
         from .scene_io import save_pose_npy
