@@ -375,7 +375,7 @@ typedef struct GsbAdamTensor {
   double step_size;          /* lr * sqrt(1-b2^t) / (1-b1^t), computed on the host in double */
   double beta1, beta2, eps, weight_decay;
 } GsbAdamTensor;
-/* flags: [n] uint32 scratch (device); gate g.norm()>0 per tensor is evaluated on the device. */
+/* flags: [n] uint32 scratch (device); gate g.norm()>0 per tensor is evaluated on the device (see gsb_adam_gate). */
 GSB_API int gsb_adam_step(int32_t n, const GsbAdamTensor* tensors_host, uint32_t* flags, gsb_stream_t stream);
 /* Same, but the whole update is skipped on the device when *skip_if_nonzero != 0 (device pointer, may be NULL):
  * pass gsb_status_device(geom, P) + 1 so that a binning overflow leaves the parameters untouched and the
@@ -383,8 +383,12 @@ GSB_API int gsb_adam_step(int32_t n, const GsbAdamTensor* tensors_host, uint32_t
 GSB_API int gsb_adam_step_gated(int32_t n, const GsbAdamTensor* tensors_host, uint32_t* flags,
                                 const uint32_t* skip_if_nonzero, gsb_stream_t stream);
 
-/* flags[k] = (tensor k's scaled gradient has a non-zero element); the gate half of gsb_adam_step, exposed so
- * the multi-GPU path can all-reduce the flags before the fused exchange kernel. */
+/* flags[k] = GSB_ADAM_FLAG_NONZERO if tensor k's scaled gradient has a non-zero element, | GSB_ADAM_FLAG_NAN if it has
+ * a NaN; the gate half of gsb_adam_step, exposed so the multi-GPU path can all-reduce the flags before the fused
+ * exchange kernel.  The moments are updated when 1 <= flag < GSB_ADAM_FLAG_NAN: the reference's gate grad.norm() > 0
+ * is false for a NaN anywhere in the tensor.  Flags summed over at most 8 ranks keep that meaning. */
+#define GSB_ADAM_FLAG_NONZERO 1u
+#define GSB_ADAM_FLAG_NAN 256u
 GSB_API int gsb_adam_gate(int32_t n, const GsbAdamTensor* tensors_host, uint32_t* flags, gsb_stream_t stream);
 
 /* ---- multi-GPU: fused reduce-scatter -> per-point Adam -> all-gather over NVLink peer memory ----------

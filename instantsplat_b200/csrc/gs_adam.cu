@@ -3,12 +3,13 @@
 //
 // Semantics are those of scene/per_point_adam.py:34-98:
 //   * whole-tensor gate  mask = grad.norm() > 0  (:66-67): moments are updated only when the
-//     gradient tensor is not identically zero; evaluated on the device by k_adam_gate
+//     gradient tensor is not identically zero and holds no NaN (a NaN makes the norm NaN, the gate false);
+//     evaluated on the device by k_adam_gate
 //   * old-style bias correction folded into step_size = lr*sqrt(1-b2^t)/(1-b1^t) (:76-81),
 //     denom = sqrt(v) + eps (eps NOT divided by sqrt(bc2))
 //   * optional per-row learning-rate multiplier per_point_lr [rows,1,..] (:84-95)
 //   * the parameter is updated even when the gate is false (stale momentum)
-// HBM traffic per element: read p,g,m,v + write p,m,v = 28 B (the roofline of this kernel).
+// HBM traffic per element: read p,g,m,v + write p,m,v = 28 B (the roofline of k_adam), plus the gate's read of g.
 #include <cuda_runtime.h>
 #include <stdio.h>
 
@@ -18,6 +19,7 @@ void gsb_set_error(const char* s);
 void gsb_count_launch(int n);
 int gsb_prof_begin(int id, cudaStream_t st);
 void gsb_prof_end(int slot, cudaStream_t st);
+int gsb_sm_count();
 
 namespace {
 
@@ -41,39 +43,58 @@ __device__ __forceinline__ int find_tensor(const AdamArgs& a, unsigned int b) {
   return k;
 }
 
-// flags[k] = 1 when tensor k's (scaled, decayed) gradient has any element with g*g > 0.
-// Grid = n_tensors x kGateSlots CTAs: CTA (k, j) scans chunks j, j+kGateSlots, ... of tensor k and re-reads
-// the flag before every chunk after its first, so in the usual case (some gradient is non-zero) each CTA
-// touches one chunk and the whole gate costs a few microseconds; an all-zero tensor is scanned completely.
-constexpr int kGateSlots = 84;
-__global__ void __launch_bounds__(kAT) k_adam_gate(AdamArgs a, unsigned int* flags) {
-  const int k = blockIdx.x / kGateSlots;
-  const unsigned int slot = blockIdx.x - k * kGateSlots;
-  const AdamT& t = a.t[k];
-  __shared__ unsigned int s_set;
-  for (unsigned int vb = slot; vb < t.nblocks; vb += kGateSlots) {
-    if (vb != slot) {
-      __syncthreads();
-      if (threadIdx.x == 0) s_set = *((volatile unsigned int*)(flags + k));
-      __syncthreads();
-      if (s_set) return;
-    }
-    const long long base = (long long)vb * kPerBlock;
-    bool any = false;
+// flags[k] |= GSB_ADAM_FLAG_NONZERO when tensor k's (scaled, decayed) gradient has an element with g*g > 0, and
+// |= GSB_ADAM_FLAG_NAN when it has a NaN element (the reference's grad.norm() > 0 is then false: the moments freeze).
+// A non-zero element does not settle the gate, so every chunk is read unless the CTA has already seen a NaN in that
+// tensor: a grid-stride loop over the chunks of all tensors (k_adam's numbering), the bits gathered per CTA in
+// shared memory and OR-ed into flags once per (CTA, tensor).  Reads 4 B per element (8 with weight decay), as
+// 128-bit loads where the chunk is whole and aligned.
+__device__ __forceinline__ unsigned int gate_bits(const AdamT& t, float g, float p) {
+  g *= t.gscale;
+  if (t.wd != 0.f) g += t.wd * p;
+  return g * g > 0.f ? GSB_ADAM_FLAG_NONZERO : (g != g ? GSB_ADAM_FLAG_NAN : 0u);
+}
+
+__global__ void __launch_bounds__(kAT) k_adam_gate(AdamArgs a, unsigned int nb, unsigned int* flags) {
+  __shared__ unsigned int s_bits[GSB_ADAM_MAX_TENSORS];
+  if (threadIdx.x < GSB_ADAM_MAX_TENSORS) s_bits[threadIdx.x] = 0u;
+  __syncthreads();
+  for (unsigned int b = blockIdx.x; b < nb; b += gridDim.x) {
+    const int k = find_tensor(a, b);
+    const AdamT& t = a.t[k];
+    if (__shfl_sync(0xffffffffu, s_bits[k], 0) & GSB_ADAM_FLAG_NAN) continue;     // warp-uniform skip
+    const long long base = (long long)(b - t.first_block) * kPerBlock;
+    unsigned int bits = 0u;
+    const bool wd = t.wd != 0.f;
+    if ((((uintptr_t)t.g | (wd ? (uintptr_t)t.p : 0)) & 15) == 0 && base + kPerBlock <= t.numel) {
 #pragma unroll
-    for (int u = 0; u < kPerThread; ++u) {
-      const long long e = base + (long long)u * kAT + threadIdx.x;
-      if (e < t.numel) {
-        float g = t.g[e] * t.gscale;
-        if (t.wd != 0.f) g += t.wd * t.p[e];
-        any |= (g * g > 0.f);
+      for (int u = 0; u < kPerThread / 4; ++u) {
+        const long long e = base + ((long long)u * kAT + threadIdx.x) * 4;
+        const float4 g = __ldg(reinterpret_cast<const float4*>(t.g + e));
+        const float4 p = wd ? __ldg(reinterpret_cast<const float4*>(t.p + e)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        bits |= gate_bits(t, g.x, p.x) | gate_bits(t, g.y, p.y) | gate_bits(t, g.z, p.z) | gate_bits(t, g.w, p.w);
+      }
+    } else {
+#pragma unroll
+      for (int u = 0; u < kPerThread; ++u) {
+        const long long e = base + (long long)u * kAT + threadIdx.x;
+        if (e < t.numel) bits |= gate_bits(t, t.g[e], wd ? t.p[e] : 0.f);
       }
     }
-    if (__syncthreads_or(any)) {
-      if (threadIdx.x == 0) atomicOr(flags + k, 1u);
-      return;
-    }
+    bits = __reduce_or_sync(0xffffffffu, bits);
+    if ((threadIdx.x & 31) == 0 && (bits & ~s_bits[k])) atomicOr(s_bits + k, bits);
   }
+  __syncthreads();
+  if (threadIdx.x < a.n && s_bits[threadIdx.x]) atomicOr(flags + threadIdx.x, s_bits[threadIdx.x]);
+}
+
+__device__ __forceinline__ bool adam_gate_open(unsigned int flag) {
+  return flag >= GSB_ADAM_FLAG_NONZERO && flag < GSB_ADAM_FLAG_NAN;
+}
+
+unsigned int gate_grid(unsigned int nb) {     // every chunk is read: fill the GPU, at most one CTA per chunk
+  const unsigned int full = 8u * (unsigned int)gsb_sm_count();
+  return nb < full ? nb : full;
 }
 
 __device__ __forceinline__ void adam_elem(const AdamT& t, float step, bool gate, float lr_mul, float& p, float g,
@@ -94,7 +115,7 @@ __global__ void __launch_bounds__(kAT) k_adam(AdamArgs a, const unsigned int* __
   if (skip && *skip) return;     // e.g. the forward's overflow word: the caller redoes the step with larger buffers
   const int k = find_tensor(a, blockIdx.x);
   const AdamT& t = a.t[k];
-  const bool gate = flags[k] != 0;
+  const bool gate = adam_gate_open(flags[k]);
   // step size = lr * sqrt(1-b2^t)/(1-b1^t): a launch argument, or (CUDA-graph replay: arguments are frozen) read from
   // a device array the host refreshes before every replay
   const float step = a.step_dev ? a.step_dev[k] : t.step;
@@ -183,7 +204,7 @@ extern "C" GSB_API int gsb_adam_gate(int32_t n, const GsbAdamTensor* ts, uint32_
   cudaError_t e = cudaMemsetAsync(flags, 0, sizeof(uint32_t) * n, st);
   if (e == cudaSuccess && nb > 0) {
     gsb_count_launch(1);
-    k_adam_gate<<<n * kGateSlots, kAT, 0, st>>>(a, flags);
+    k_adam_gate<<<gate_grid(nb), kAT, 0, st>>>(a, nb, flags);
     e = cudaGetLastError();
   }
   return finish(e, "gsb_adam_gate");
@@ -207,7 +228,7 @@ extern "C" GSB_API int gsb_adam_step_ex(int32_t n, const GsbAdamTensor* ts, uint
   if (e == cudaSuccess && nb > 0) {
     gsb_count_launch(2);
     int slot = gsb_prof_begin(GSB_K_ADAM, st);
-    k_adam_gate<<<n * kGateSlots, kAT, 0, st>>>(a, flags);
+    k_adam_gate<<<gate_grid(nb), kAT, 0, st>>>(a, nb, flags);
     k_adam<<<nb, kAT, 0, st>>>(a, flags, skip_if_nonzero);
     gsb_prof_end(slot, st);
     e = cudaGetLastError();

@@ -5,7 +5,7 @@
 // its flat gradient buffer.  Rank r owns the r-th contiguous shard of the flat index space.  ONE
 // kernel per rank then, for each 128-bit group of its shard:
 //     g   = sum over ranks of peer_grads[rank][i]          (P2P loads over NVLink, fixed order)
-//     m,v = Adam moment update (local, shard-sized)         (scene/per_point_adam.py:66-73)
+//     m,v = Adam moment update (local, shard-sized)         (scene/per_point_adam.py:66-73; gate: gsb_adam_gate)
 //     p   = p - step * lr_i * m / (sqrt(v) + eps)           (:76-98)
 //     peer_params[rank][i] = p   for every rank             (P2P stores over NVLink)
 // i.e. the reduce-scatter, the optimizer and the all-gather of the "NCCL all-reduce + Adam"
@@ -85,7 +85,9 @@ __global__ void __launch_bounds__(kFT) k_fused_rs_adam_ag(FusedArgs a, const uns
   for (int i = 1; i < kMaxPieces; ++i)
     if (i < a.n_pieces && blockIdx.x >= a.pc[i].first_block) k = i;
   const Piece& t = a.pc[k];
-  const bool gate = flags[t.flag_index] != 0;
+  // the per-rank gate flags summed over the ranks: some rank saw a non-zero element and none saw a NaN (gsb200.h)
+  const unsigned int flag = flags[t.flag_index];
+  const bool gate = flag >= GSB_ADAM_FLAG_NONZERO && flag < GSB_ADAM_FLAG_NAN;
   const float step = a.step_dev ? a.step_dev[t.flag_index] : t.step;
   const long long base = t.begin + (long long)(blockIdx.x - t.first_block) * kElemsPerBlock;
 #pragma unroll
