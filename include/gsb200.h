@@ -332,6 +332,21 @@ GSB_API int gsb_image_metrics_batch(int32_t V, int32_t C, int32_t H, int32_t W, 
  * H * W must fit in int32. */
 GSB_API int gsb_frames_u8_batch(int32_t V, int32_t H, int32_t W, const float* img, uint8_t* out, gsb_stream_t stream);
 
+/* ---- PNG encoding of 8-bit RGB frames (save_image's files, re-compressed; DESIGN.md 4.19) ----
+ * rgb [V, H, W, 3] uint8 (gsb_frames_u8_batch's layout) -> out [V, gsb_png_bound(H, W)] uint8: frame v's zlib stream
+ * (the concatenated IDAT data of its PNG) at out + v * gsb_png_bound(H, W), its length in sizes[v] (device int64).
+ * The scanlines are filtered as Pillow filters them (of None, Sub, Up and Paeth, the least sum of |int8|, the first on
+ * a tie), so the stream inflates to Pillow's filtered bytes; the deflate itself differs from zlib's, so the files are
+ * not byte-identical to Pillow's.  A frame's bytes depend on its pixels only: not on V, its place in the batch, the
+ * stream or the timing.
+ * gsb_png_bound: the largest stream a frame needs (every 32 KiB segment stored, plus the zlib framing); 0 for a bad
+ * size.  gsb_png_scratch_bytes: the scratch one call needs.  H, W >= 1, H (3W + 1) below 2^31 - 4096, V <= 65535;
+ * scratch 16-byte and sizes 8-byte aligned; else GSB_ERR_INVALID. */
+GSB_API size_t gsb_png_bound(int32_t H, int32_t W);
+GSB_API size_t gsb_png_scratch_bytes(int32_t V, int32_t H, int32_t W);
+GSB_API int gsb_png_encode_batch(int32_t V, int32_t H, int32_t W, const uint8_t* rgb, void* scratch,
+                                 size_t scratch_bytes, uint8_t* out, int64_t* sizes, gsb_stream_t stream);
+
 /* ---- LPIPS, VGG16 v0.1 (metrics.py:69 lpips(render, gt, net_type='vgg'); lpipsPyTorch/modules/lpips.py,
  * networks.py BaseNet / VGG16, utils.py normalize_activation).  DESIGN.md 4.15.  fp32 FFMA, NHWC activations, every
  * sum in one fixed order: an image's values are bit-identical from run to run and whatever else is in the batch.

@@ -24,6 +24,7 @@ else: frames_u8(tracker, poses_from_w2c(np.load(".../pose_optimized.npy"))) and 
 Not done: the mp4 (images_to_video needs imageio / ffmpeg), the pose plots (matplotlib) and save_time.
 
     python -m instantsplat_b200.freeview -s SOURCE -m MODEL --n_views N --iterations IT [--white_background]
+        [--png_encoder pil|gpu]
 """
 from __future__ import annotations
 
@@ -37,7 +38,7 @@ from typing import Iterable, Iterator, Optional, Sequence, Tuple
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, png
 from ._lib import check
 from .frame import ST_OVERFLOW
 from .tracking import PoseTracker
@@ -236,6 +237,17 @@ def write_pngs(frames: Iterable[Tuple[int, np.ndarray]], folder: str, workers: O
     return count
 
 
+def add_png_encoder_arg(ap: argparse.ArgumentParser) -> None:
+    ap.add_argument("--png_encoder", choices=("pil", "gpu"), default="pil",
+                    help="pil: save_image's files, byte for byte; gpu: encoded on the GPU (png.py), other bytes that "
+                         "decode to the same pixels")
+
+
+def png_writer(encoder: str):
+    """write_pngs for --png_encoder pil, png.write_pngs for gpu."""
+    return png.write_pngs if encoder == "gpu" else write_pngs
+
+
 # ---- the command line: stage 3 of run_infer.sh ---------------------------------------------------------------
 def max_iteration(model_path: str) -> int:
     """searchForMaxIteration (utils/system_utils.py:26-28) over model_path/point_cloud."""
@@ -318,11 +330,13 @@ def main(argv=None) -> int:
     ap.add_argument("--max_batch", type=int, default=4,
                     help="frames per batched forward; scratch grows by about 150 P + 60 H W bytes a frame")
     ap.add_argument("--workers", type=int, default=None, help="PNG encoder threads (default: up to 8)")
+    add_png_encoder_arg(ap)
     a = ap.parse_args(argv)
     if a.n_views < 2:
         raise SystemExit("--n_views must be at least 2: the fly-through joins consecutive key poses")
     tracker, keys, it = load(a.source_path, a.model_path, a.n_views, a.iterations, a.white_background)
-    n, folder = fly_through(tracker, keys, it, a.model_path, a.n_views, a.max_batch, a.workers)
+    n, folder = fly_through(tracker, keys, it, a.model_path, a.n_views, a.max_batch, a.workers,
+                            png_writer(a.png_encoder))
     print(f"{n} frames -> {folder}")
     return 0
 

@@ -2,9 +2,9 @@
 on one GPU (DESIGN.md section 4.18).
 
     python -m instantsplat_b200.pipeline eval  --data_root ROOT --output_dir OUT --datasets D.. --scenes S..
-        --n_views N.. --iterations IT.. [--lpips_weights DIR] [--workers K]
+        --n_views N.. --iterations IT.. [--lpips_weights DIR] [--workers K] [--png_encoder pil|gpu]
     python -m instantsplat_b200.pipeline infer --data_root ROOT --output_dir OUT --datasets D.. --scenes S..
-        --n_views N.. --iterations IT.. [--workers K]
+        --n_views N.. --iterations IT.. [--workers K] [--png_encoder pil|gpu]
 
 Tasks run in the scripts' loop order (dataset, scene, n_views, iterations), one after another.  The source is
 ROOT/D/S/24_views for eval and ROOT/D/S for infer; the model is OUT/D/S/<N>_views.  Each stage is the stage module's
@@ -20,8 +20,9 @@ memory instead:
   * infer: freeview.fly_through.
 
 Every PNG goes to one process-wide encoder pool (PngWriter) that the GPU stages do not wait for, up to a bound on the
-frames queued.  Every task is checked before anything is written (refusals).  The scripts' nvidia-smi GPU picker and
-init_geo (stage 1) are not part of this.
+frames queued; with --png_encoder gpu the frames are encoded on the GPU and the pool only writes the files.  Every
+task is checked before anything is written (refusals).  The scripts' nvidia-smi GPU picker and init_geo (stage 1) are
+not part of this.
 """
 from __future__ import annotations
 
@@ -38,7 +39,7 @@ from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from . import freeview, metrics, render_views, train
+from . import freeview, metrics, png, render_views, train
 from .scene_io import load_views, pose_matrices
 
 # stage -> (log file, the script's start line, its completion line)
@@ -135,12 +136,16 @@ class PngWriter:
     """One pool of `workers` PNG encoder threads for a whole run (None: up to 8).  write queues frames and returns
     without waiting for their encodes; at most 4 x workers frames wait, so the host memory they hold stays bounded,
     and write blocks while the queue is full.  A failed write raises WriteError, naming the file, from the first call
-    that finds it done (write, wait or close)."""
+    that finds it done (write, wait or close).  encoder "gpu": write encodes each chunk on the GPU (png.encode_host,
+    on the current stream) and queues only the file writes."""
 
-    def __init__(self, workers: Optional[int] = None):
+    def __init__(self, workers: Optional[int] = None, encoder: str = "pil"):
         self.workers = min(8, os.cpu_count() or 1) if workers is None else int(workers)
         if self.workers < 1:
             raise ValueError("PngWriter: workers must be >= 1")
+        if encoder not in ("pil", "gpu"):
+            raise ValueError(f"PngWriter: encoder must be 'pil' or 'gpu', got {encoder!r}")
+        self.encoder = encoder
         self.cap = 4 * self.workers
         self._pool = ThreadPoolExecutor(max_workers=self.workers)
         self._pending = deque()                     # (future, path) in submission order
@@ -152,11 +157,13 @@ class PngWriter:
         os.makedirs(folder, exist_ok=True)
         count = 0
         for first, chunk in frames:
+            files = png.encode_host(chunk) if self.encoder == "gpu" else None
             for i in range(chunk.shape[0]):
                 while len(self._pending) >= self.cap:
                     self._finish(*self._pending.popleft())
                 path = os.path.join(folder, f"{first + i:05d}.png" if names is None else names[first + i])
-                self._pending.append((self._pool.submit(freeview._save_png, chunk[i], path), path))
+                job = (freeview._save_png, chunk[i]) if files is None else (png.write_file, files[i])
+                self._pending.append((self._pool.submit(*job, path), path))
                 count += 1
             while self._pending and self._pending[0][0].done():
                 self._finish(*self._pending.popleft())
@@ -272,10 +279,11 @@ def run_task(t: Task, pool: PngWriter, lpips_net=None, lpips_weights: Optional[s
 
 
 def run_tasks(ts: Sequence[Task], workers: Optional[int] = None, lpips_net=None, lpips_weights: Optional[str] = None,
-              device="cuda") -> Tuple[int, List[Dict[str, float]]]:
-    """Every task in order on one encoder pool, then every write waited for.  Returns (model directories metrics
-    could not evaluate, per-task stage times).  Raises WriteError when a PNG could not be written."""
-    pool = PngWriter(workers)
+              device="cuda", png_encoder: str = "pil") -> Tuple[int, List[Dict[str, float]]]:
+    """Every task in order on one encoder pool (PngWriter with png_encoder), then every write waited for.  Returns
+    (model directories metrics could not evaluate, per-task stage times).  Raises WriteError when a PNG could not be
+    written."""
+    pool = PngWriter(workers, png_encoder)
     failed, times = 0, []
     try:
         for k, t in enumerate(ts, 1):
@@ -307,6 +315,7 @@ def parser() -> argparse.ArgumentParser:
             p.add_argument("--lpips_weights", metavar="DIR", default=None, help="as metrics --lpips_weights")
         p.add_argument("--workers", type=int, default=None, help="PNG encoder threads for the whole run (default: up "
                                                                   "to 8)")
+        freeview.add_png_encoder_arg(p)
     return ap
 
 
@@ -328,7 +337,7 @@ def main(argv=None) -> int:
         except (OSError, ValueError) as e:
             ap.error(str(e))
     try:
-        failed, _ = run_tasks(ts, a.workers, net, weights)
+        failed, _ = run_tasks(ts, a.workers, net, weights, png_encoder=a.png_encoder)
     except WriteError as e:
         raise SystemExit(f"instantsplat_b200.pipeline: {e}")
     print("=" * 55)

@@ -14,14 +14,15 @@ render.py's render_sets (render.py:189-248) with its branch logic, on the GPU.
 
 Renders are save_image's 8-bit frames (freeview.frames_u8).  A ground-truth file is save_image of the loaded image,
 uint8 -> /255 -> uint8; that round trip is the identity on all 256 levels (checked once, gt_round_trip_is_identity),
-so the gt PNGs are encoded from the decoded bytes.  Every PNG is encoded on freeview.write_pngs' thread pool.
+so the gt PNGs are encoded from the decoded bytes.  Every PNG is encoded on freeview.write_pngs' thread pool, or on the
+GPU by png.write_pngs with --png_encoder gpu.
 
 The background is black, or white with --white_background; the SH degree is the ply's.  The model's cfg_args is not
 read: render.py's get_combined_args lets every command-line value that is not None win, and ModelParams is built
 with sentinel=False, so its defaults (white_background False included) always override the saved config there too.
 
     python -m instantsplat_b200.render_views -s SOURCE -m MODEL --n_views N --iterations IT [--eval] [--infer_video]
-        [--optim_test_pose_iter 500] [--white_background] [--max_batch B] [--workers K]
+        [--optim_test_pose_iter 500] [--white_background] [--max_batch B] [--workers K] [--png_encoder pil|gpu]
 """
 from __future__ import annotations
 
@@ -115,6 +116,7 @@ def parser() -> argparse.ArgumentParser:
     ap.add_argument("--max_batch", type=int, default=12,
                     help="views per batched loop; tracking scratch is about 150 P + 44 H W bytes a view")
     ap.add_argument("--workers", type=int, default=None, help="PNG encoder threads (default: up to 8)")
+    freeview.add_png_encoder_arg(ap)
     return ap
 
 
@@ -125,14 +127,15 @@ def main(argv=None) -> int:
     if a.infer_video and not a.eval:
         fv = ["-s", a.source_path, "-m", a.model_path, "--n_views", str(a.n_views), "--iterations", str(a.iterations),
               "--max_batch", str(a.max_batch)] + (["--white_background"] if a.white_background else []) \
-            + ([] if a.workers is None else ["--workers", str(a.workers)])
+            + ([] if a.workers is None else ["--workers", str(a.workers)]) + ["--png_encoder", a.png_encoder]
         return freeview.main(fv)
+    write = freeview.png_writer(a.png_encoder)
     it = freeview.max_iteration(a.model_path) if a.iterations == -1 else a.iterations
     if a.eval:
         views = load_views(a.source_path, a.n_views, 1, a.resolution)
         tracker = tracker_for(a.model_path, it, views, a.white_background)
         out = os.path.join(a.model_path, "test", f"ours_{it}")
-        render_test(tracker, views, out, a.optim_test_pose_iter, a.max_batch, a.workers)
+        render_test(tracker, views, out, a.optim_test_pose_iter, a.max_batch, a.workers, write)
     else:
         npy = os.path.join(a.model_path, "pose", f"ours_{it}", "pose_optimized.npy")
         if not os.path.isfile(npy):
@@ -140,7 +143,7 @@ def main(argv=None) -> int:
         views = load_views(a.source_path, a.n_views, 0, a.resolution)
         tracker = tracker_for(a.model_path, it, views, a.white_background)
         out = os.path.join(a.model_path, "train", f"ours_{it}")
-        render_train(tracker, views, np.load(npy), out, a.max_batch, a.workers)
+        render_train(tracker, views, np.load(npy), out, a.max_batch, a.workers, write)
     print(f"{len(views)} views -> {out}")
     return 0
 
