@@ -2,7 +2,7 @@
 on one GPU (DESIGN.md section 4.18).
 
     python -m instantsplat_b200.pipeline eval  --data_root ROOT --output_dir OUT --datasets D.. --scenes S..
-        --n_views N.. --iterations IT.. [--lpips_weights DIR] [--workers K] [--png_encoder pil|gpu]
+        --n_views N.. --iterations IT.. [--lpips_weights DIR] [--workers K] [--png_encoder pil|gpu] [--test_fps]
     python -m instantsplat_b200.pipeline infer --data_root ROOT --output_dir OUT --datasets D.. --scenes S..
         --n_views N.. --iterations IT.. [--workers K] [--png_encoder pil|gpu]
 
@@ -15,7 +15,9 @@ memory instead:
   * train: train.run; its trainer's final Gaussians (JointTrainer.ply_tensors, what point_cloud.ply holds, at the
     stored SH degree) and pose_optimized.npy's rows (scene_io.pose_matrices) are kept, then the trainer is released.
   * training-view renders: render_views.render_train on the train stage's decoded views.
-  * test-view renders: render_views.render_test on load_views(split=1), its 8-bit renders and gts kept.
+  * test-view renders: render_views.render_test on load_views(split=1), its 8-bit renders and gts kept; with
+    --test_fps (render.py's flag on the stage's line, as run_eval.sh's commented-out line would add it), then
+    render_views.report_fps at the last test view's best pose, which writes total_fps.json into the model directory.
   * metrics: metrics.evaluate with the current test/ours_<it> from memory, any earlier method from its files.
   * infer: freeview.fly_through.
 
@@ -82,13 +84,13 @@ def tasks(mode: str, data_root: str, output_dir: str, datasets: Sequence[str], s
     return out
 
 
-def stage_argv(t: Task, lpips_weights: Optional[str] = None) -> Dict[str, List[str]]:
-    """Each stage's command line as the script writes it."""
+def stage_argv(t: Task, lpips_weights: Optional[str] = None, test_fps: bool = False) -> Dict[str, List[str]]:
+    """Each stage's command line as the script writes it; test_fps adds --test_fps to the test-view renders'."""
     base = ["-s", t.source, "-m", t.model, "-r", "1", "--n_views", str(t.n_views), "--iterations", str(t.iterations)]
     out = {"train": base + ["--pp_optimizer", "--optim_pose"]}
     if t.mode == "eval":
         out["render_train"] = list(base)
-        out["render_test"] = base + ["--eval"]
+        out["render_test"] = base + ["--eval"] + (["--test_fps"] if test_fps else [])
         out["metrics"] = ["-s", t.source, "-m", t.model, "--n_views", str(t.n_views)] \
             + ([] if lpips_weights is None else ["--lpips_weights", lpips_weights])
     else:
@@ -96,15 +98,16 @@ def stage_argv(t: Task, lpips_weights: Optional[str] = None) -> Dict[str, List[s
     return out
 
 
-def stage_args(t: Task, lpips_weights: Optional[str] = None) -> Dict[str, argparse.Namespace]:
+def stage_args(t: Task, lpips_weights: Optional[str] = None, test_fps: bool = False) -> Dict[str, argparse.Namespace]:
     """stage_argv parsed by each stage's own parser."""
     parse = {"train": train.parse_args, "metrics": lambda a: metrics.parser().parse_args(a)}
     return {k: parse.get(k, lambda a: render_views.parser().parse_args(a))(v)
-            for k, v in stage_argv(t, lpips_weights).items()}
+            for k, v in stage_argv(t, lpips_weights, test_fps).items()}
 
 
-def refusals(t: Task) -> List[str]:
-    """Why the task cannot run, each reason with its path; empty when it can.  Reads the source, writes nothing."""
+def refusals(t: Task, test_fps: bool = False) -> List[str]:
+    """Why the task cannot run, each reason with its path; empty when it can.  Reads the source, writes nothing.
+    test_fps: the eval task's test-view renders carry --test_fps, which needs a test view."""
     out = []
     f0 = os.path.join(t.source, f"sparse_{t.n_views}", "0")
     for name in ("points3D.ply", "confidence_dsp.npy"):
@@ -114,6 +117,9 @@ def refusals(t: Task) -> List[str]:
         out.append(f"the test views are missing: {os.path.join(t.source, f'sparse_{t.n_views}', '1')} not found")
     if t.mode == "infer" and t.n_views < 2:
         out.append("--n_views must be at least 2: the fly-through joins consecutive key poses")
+    why = render_views.fps_refusal(t.source, t.n_views) if test_fps and t.mode == "eval" else None
+    if why:
+        out.append(why)
     if out:
         return out
     a = stage_args(t)["train"]
@@ -214,10 +220,10 @@ def _stage(t: Task, key: str, times: Dict[str, float]):
 
 
 def run_task(t: Task, pool: PngWriter, lpips_net=None, lpips_weights: Optional[str] = None,
-             device="cuda") -> Tuple[int, Dict[str, float]]:
-    """The script's run_on_gpu from stage 2 on.  Returns (model directories metrics could not evaluate, wall seconds
-    per stage).  The trainer and trackers are released before it returns."""
-    a = stage_args(t, lpips_weights)
+             device="cuda", test_fps: bool = False) -> Tuple[int, Dict[str, float]]:
+    """The script's run_on_gpu from stage 2 on, with test_fps: stage 4 with --test_fps.  Returns (model directories
+    metrics could not evaluate, wall seconds per stage).  The trainer and trackers are released before it returns."""
+    a = stage_args(t, lpips_weights, test_fps)
     times, failed = {}, 0
     print("=" * 55)
     print(f"Starting process: {t.label}")
@@ -256,8 +262,12 @@ def run_task(t: Task, pool: PngWriter, lpips_net=None, lpips_weights: Optional[s
         with _stage(t, "render_test", times):
             views = load_views(t.source, t.n_views, 1, r.resolution)
             out = os.path.join(t.model, "test", f"ours_{it}")
-            render_views.render_test(tracker(views, r.white_background), views, out, r.optim_test_pose_iter,
-                                     r.max_batch, write=keep)
+            tk = tracker(views, r.white_background)
+            start = time.time()
+            best = render_views.render_test(tk, views, out, r.optim_test_pose_iter, r.max_batch, write=keep)
+            if r.test_fps:
+                render_views.report_fps(tk, best[-1], t.model, start)
+            del tk
             print(f"{len(views)} views -> {out}")
         names = [n + ".png" for n in views.names]
         order = sorted(range(len(names)), key=names.__getitem__)         # metrics pairs the files in sorted order
@@ -279,16 +289,16 @@ def run_task(t: Task, pool: PngWriter, lpips_net=None, lpips_weights: Optional[s
 
 
 def run_tasks(ts: Sequence[Task], workers: Optional[int] = None, lpips_net=None, lpips_weights: Optional[str] = None,
-              device="cuda", png_encoder: str = "pil") -> Tuple[int, List[Dict[str, float]]]:
-    """Every task in order on one encoder pool (PngWriter with png_encoder), then every write waited for.  Returns
-    (model directories metrics could not evaluate, per-task stage times).  Raises WriteError when a PNG could not be
-    written."""
+              device="cuda", png_encoder: str = "pil", test_fps: bool = False) -> Tuple[int, List[Dict[str, float]]]:
+    """Every task in order on one encoder pool (PngWriter with png_encoder), then every write waited for; test_fps:
+    run_task's.  Returns (model directories metrics could not evaluate, per-task stage times).  Raises WriteError
+    when a PNG could not be written."""
     pool = PngWriter(workers, png_encoder)
     failed, times = 0, []
     try:
         for k, t in enumerate(ts, 1):
             print(f"Processing task {k} / {len(ts)}", flush=True)
-            f, s = run_task(t, pool, lpips_net, lpips_weights, device)
+            f, s = run_task(t, pool, lpips_net, lpips_weights, device, test_fps)
             failed += f
             times.append(s)
     finally:
@@ -313,6 +323,8 @@ def parser() -> argparse.ArgumentParser:
         p.add_argument("--iterations", nargs="+", type=int, required=True)
         if mode == "eval":
             p.add_argument("--lpips_weights", metavar="DIR", default=None, help="as metrics --lpips_weights")
+            p.add_argument("--test_fps", action="store_true", help="render.py --test_fps on the test-view renders: "
+                                                                    "each task's rate appended to total_fps.json")
         p.add_argument("--workers", type=int, default=None, help="PNG encoder threads for the whole run (default: up "
                                                                   "to 8)")
         freeview.add_png_encoder_arg(p)
@@ -324,9 +336,9 @@ def main(argv=None) -> int:
     a = ap.parse_args(argv)
     if a.workers is not None and a.workers < 1:
         ap.error("--workers must be at least 1")
-    weights = getattr(a, "lpips_weights", None)
+    weights, test_fps = getattr(a, "lpips_weights", None), getattr(a, "test_fps", False)
     ts = tasks(a.mode, a.data_root, a.output_dir, a.datasets, a.scenes, a.n_views, a.iterations)
-    bad = [f"{t.label}: {r}" for t in ts for r in refusals(t)]
+    bad = [f"{t.label}: {r}" for t in ts for r in refusals(t, test_fps)]
     if bad:
         raise SystemExit("\n".join(f"instantsplat_b200.pipeline: {b}" for b in bad))
     net = None
@@ -337,7 +349,7 @@ def main(argv=None) -> int:
         except (OSError, ValueError) as e:
             ap.error(str(e))
     try:
-        failed, _ = run_tasks(ts, a.workers, net, weights, png_encoder=a.png_encoder)
+        failed, _ = run_tasks(ts, a.workers, net, weights, png_encoder=a.png_encoder, test_fps=test_fps)
     except WriteError as e:
         raise SystemExit(f"instantsplat_b200.pipeline: {e}")
     print("=" * 55)

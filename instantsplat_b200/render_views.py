@@ -17,26 +17,36 @@ uint8 -> /255 -> uint8; that round trip is the identity on all 256 levels (check
 so the gt PNGs are encoded from the decoded bytes.  Every PNG is encoded on freeview.write_pngs' thread pool, or on the
 GPU by png.write_pngs with --png_encoder gpu.
 
+--test_fps with --eval is render.py's frame-rate report (render.py:172-186, report_fps): after the test renders, the
+last test view in sorted order is rendered 1000 times at its best pose, from a replayed CUDA graph
+(PoseTracker.time_renders), the rate of the trimmed mean is printed and appended to MODEL/total_fps.json, and the
+`[4] render` line of train_time.txt records the test stage's time with the loop in it.  Without the flag neither
+file is written.
+
 The background is black, or white with --white_background; the SH degree is the ply's.  The model's cfg_args is not
 read: render.py's get_combined_args lets every command-line value that is not None win, and ModelParams is built
 with sentinel=False, so its defaults (white_background False included) always override the saved config there too.
 
     python -m instantsplat_b200.render_views -s SOURCE -m MODEL --n_views N --iterations IT [--eval] [--infer_video]
         [--optim_test_pose_iter 500] [--white_background] [--max_batch B] [--workers K] [--png_encoder pil|gpu]
+        [--test_fps]
 """
 from __future__ import annotations
 
 import argparse
+import json
 import os
 import sys
-from typing import Optional
+import time
+from typing import Optional, Sequence, Tuple
 
 import numpy as np
 import torch
 
 from . import freeview
-from .scene_io import Views, load_views
+from .scene_io import Views, load_views, read_colmap_text
 from .tracking import PoseTracker
+from .train import save_time
 
 
 def gt_round_trip_is_identity() -> bool:
@@ -99,6 +109,41 @@ def render_test(tracker: PoseTracker, views: Views, out_dir: str, num_iter: int 
     return best
 
 
+def fps_from_times(durations: Sequence[float]) -> Tuple[float, str]:
+    """render.py:180-186 on frame times in seconds: (fps, the text appended to total_fps.json).  fps is the reciprocal
+    of the mean of the sorted times [100:900] (the 100 fastest and all past the 900th dropped); the text is
+    json.dump(f'{fps}', fp, indent=True) and a newline, a JSON string holding str(fps) on a line of its own."""
+    kept = sorted(durations)[100:900]
+    fps = 1 / (sum(kept) / len(kept))
+    return fps, json.dumps(f"{fps}", indent=True) + "\n"
+
+
+def report_fps(tracker: PoseTracker, pose: torch.Tensor, model_path: str, start: float, n: int = 1000) -> float:
+    """render.py's --test_fps and the end of its `[4] render` span (render.py:172-186, :219-231): prints
+    `>>> Calculate FPS: `, times n renders at pose [7] (PoseTracker.time_renders), prints `>>> FPS = ` and the rate,
+    appends fps_from_times' line to model_path/total_fps.json, then appends `[4] render` with the seconds since start
+    (a time.time() value) to model_path/train_time.txt.  Returns the rate."""
+    print(">>> Calculate FPS: ")
+    fps, line = fps_from_times(tracker.time_renders(pose, n))
+    print(">>> FPS = ", fps)
+    with open(os.path.join(model_path, "total_fps.json"), "a") as f:
+        f.write(line)
+    save_time(model_path, "[4] render", time.time() - start)
+    return fps
+
+
+def fps_refusal(source_path: str, n_views: int) -> Optional[str]:
+    """Why --eval --test_fps cannot run, or None: it times the last test view, and render.py fails when
+    sparse_<n_views>/1 lists none (its loop variable `view` is then undefined).  A folder that cannot be read is left
+    to load_views, which names the problem."""
+    folder = os.path.join(source_path, f"sparse_{n_views}", "1")
+    try:
+        _, images = read_colmap_text(folder, ("PINHOLE", "SIMPLE_PINHOLE"))
+    except (OSError, ValueError):
+        return None
+    return None if images else f"--test_fps times the last test view, and {folder}/images.txt lists none"
+
+
 def parser() -> argparse.ArgumentParser:
     """render.py's command line as this stage reads it."""
     ap = argparse.ArgumentParser(prog="python -m instantsplat_b200.render_views",
@@ -117,6 +162,8 @@ def parser() -> argparse.ArgumentParser:
                     help="views per batched loop; tracking scratch is about 150 P + 44 H W bytes a view")
     ap.add_argument("--workers", type=int, default=None, help="PNG encoder threads (default: up to 8)")
     freeview.add_png_encoder_arg(ap)
+    ap.add_argument("--test_fps", action="store_true",
+                    help="with --eval: time 1000 renders of the last test view and append the rate to total_fps.json")
     return ap
 
 
@@ -132,10 +179,16 @@ def main(argv=None) -> int:
     write = freeview.png_writer(a.png_encoder)
     it = freeview.max_iteration(a.model_path) if a.iterations == -1 else a.iterations
     if a.eval:
+        why = fps_refusal(a.source_path, a.n_views) if a.test_fps else None
+        if why:
+            raise SystemExit(f"render_views: {why}")
         views = load_views(a.source_path, a.n_views, 1, a.resolution)
         tracker = tracker_for(a.model_path, it, views, a.white_background)
         out = os.path.join(a.model_path, "test", f"ours_{it}")
-        render_test(tracker, views, out, a.optim_test_pose_iter, a.max_batch, a.workers, write)
+        start = time.time()
+        best = render_test(tracker, views, out, a.optim_test_pose_iter, a.max_batch, a.workers, write)
+        if a.test_fps:
+            report_fps(tracker, best[-1], a.model_path, start)
     else:
         npy = os.path.join(a.model_path, "pose", f"ours_{it}", "pose_optimized.npy")
         if not os.path.isfile(npy):

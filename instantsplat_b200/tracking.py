@@ -21,7 +21,8 @@ view index, and each view's result is bit-identical to optimize() on that view a
 from __future__ import annotations
 
 import math
-from typing import Optional
+import time
+from typing import List, Optional
 
 import torch
 
@@ -132,6 +133,45 @@ class PoseTracker:
             fr = self._frame_batch(V)
             self._forward_batch(fr, self._cam(), self._gauss(p), p, True)
             return fr.color.clone()
+
+    def time_renders(self, pose: torch.Tensor, n: int = 1000, out: Optional[torch.Tensor] = None) -> List[float]:
+        """The frame times of render.py's --test_fps loop (render.py:172-179) at pose [7]: n durations in seconds.
+
+        One eager forward at pose sizes a scratch frame's binning buffer from its instance count with the tracker's
+        headroom; the pose does not change, so neither does the count.  The single-view forward (render_batch of one
+        view, without the status copy to the host) is then captured into a CUDA graph that reads the pose from a
+        device row, and replayed n times.  Each duration is one replay on the host clock, ending in a stream
+        synchronise, so it is a whole frame and not an enqueue.  The status words are read once after the loop: a
+        binning overflow raises GsbError instead of returning the times of truncated frames.  out: an optional
+        [3, H, W] fp32 tensor that receives the last replay's image.  The graph and the scratch are released
+        before returning."""
+        if not isinstance(pose, torch.Tensor) or pose.numel() != 7:
+            raise ValueError(f"time_renders: expected a pose of 7 values, got {tuple(getattr(pose, 'shape', ()))}")
+        p = self._poses(pose.reshape(1, 7), "time_renders")
+        if int(n) < 1:
+            raise ValueError("time_renders: n must be >= 1")
+        with torch.cuda.device(self.dev):
+            fr = Frame(self.dev, self.P, self.W, self.H, views=1)
+            cam = self._cam()
+            self._forward_batch(fr, cam, self._gauss(p), p, True)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                fr.preprocess_batch(cam, self._gauss(p), p, None, self.filt)
+                fr.render_batch(cam)
+            stream = torch.cuda.current_stream()
+            stream.synchronize()
+            times = []
+            for _ in range(int(n)):
+                t0 = time.perf_counter()
+                graph.replay()
+                stream.synchronize()
+                times.append(time.perf_counter() - t0)
+            if int(fr.word(ST_OVERFLOW).item()):
+                raise _lib.GsbError("time_renders: the instance count outgrew the binning buffer; raise "
+                                    "PoseTracker.headroom")
+            if out is not None:
+                out.copy_(fr.color[0])
+        return times
 
     def optimize_batch(self, init_poses: torch.Tensor, gts: torch.Tensor, num_iter: int = 500, lr_T: float = 0.003,
                        lr_q: float = 0.001, weight_decay: float = 1e-4, eta_min: float = 1e-4, threshold: float = 0.0,
