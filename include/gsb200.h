@@ -347,7 +347,21 @@ GSB_API size_t gsb_png_scratch_bytes(int32_t V, int32_t H, int32_t W);
 GSB_API int gsb_png_encode_batch(int32_t V, int32_t H, int32_t W, const uint8_t* rgb, void* scratch,
                                  size_t scratch_bytes, uint8_t* out, int64_t* sizes, gsb_stream_t stream);
 
-/* ---- LPIPS, VGG16 v0.1 (metrics.py:69 lpips(render, gt, net_type='vgg'); lpipsPyTorch/modules/lpips.py,
+/* ---- Pillow's bicubic resize of 8-bit RGB images (PILtoTorch's pil_image.resize; DESIGN.md 4.21) ----
+ * in [V, H, W, 3] uint8 -> out [V, Ho, Wo, 3] uint8, byte for byte what Image.resize((Wo, Ho)) gives each view: a
+ * horizontal pass when Wo != W, then a vertical pass when Ho != H, each output channel
+ * clamp((2^21 + sum_k src[first + k] * coef[k]) >> 22, 0, 255) in int32 over Pillow's integer tables.  Per axis the
+ * tables are device int32: bounds [out, 2] (first source index, tap count) and coefs [out, ksize] (Pillow's weights
+ * times 2^22, rounded half away from zero), built on the host (resample.py coefficients); an axis that keeps its size
+ * takes no tables (NULL).  Both axes unchanged is a copy.  scratch: the horizontal pass's V * H * Wo * 3 bytes, needed
+ * only when both axes change.  A view's bytes depend on its own pixels only.  V, H and Ho in 1..65535, W and Wo >= 1
+ * with 3 W and 3 Wo at most 65535 * 256, ksize >= 1 for an axis that changes; else GSB_ERR_INVALID. */
+GSB_API int gsb_resample_u8_batch(int32_t V, int32_t H, int32_t W, int32_t Ho, int32_t Wo, const uint8_t* in,
+                                  uint8_t* out, const int32_t* x_bounds, const int32_t* x_coefs, int32_t x_ksize,
+                                  const int32_t* y_bounds, const int32_t* y_coefs, int32_t y_ksize, void* scratch,
+                                  size_t scratch_bytes, gsb_stream_t stream);
+
+/* ---- LPIPS, VGG16 v0.1(metrics.py:69 lpips(render, gt, net_type='vgg'); lpipsPyTorch/modules/lpips.py,
  * networks.py BaseNet / VGG16, utils.py normalize_activation).  DESIGN.md 4.15.  fp32 FFMA, NHWC activations, every
  * sum in one fixed order: an image's values are bit-identical from run to run and whatever else is in the batch.
  *

@@ -23,8 +23,13 @@ else: frames_u8(tracker, poses_from_w2c(np.load(".../pose_optimized.npy"))) and 
 
 Not done: the mp4 (images_to_video needs imageio / ffmpeg), the pose plots (matplotlib) and save_time.
 
+-r / --resolution (default 1) and --resample_images: render.py renders the fly-through at the training cameras' loaded
+size, loaded_size of cameras.txt's width and height at -r (init_geo writes the images' own size there).  With
+--resample_images the frames are rendered at that size; without it a -r that changes the size is refused, and the
+frames are the full-size ones.
+
     python -m instantsplat_b200.freeview -s SOURCE -m MODEL --n_views N --iterations IT [--white_background]
-        [--png_encoder pil|gpu]
+        [--png_encoder pil|gpu] [-r R --resample_images]
 """
 from __future__ import annotations
 
@@ -38,7 +43,7 @@ from typing import Iterable, Iterator, Optional, Sequence, Tuple
 import numpy as np
 import torch
 
-from . import _lib, png
+from . import _lib, png, resample
 from ._lib import check
 from .frame import ST_OVERFLOW
 from .tracking import PoseTracker
@@ -281,19 +286,35 @@ def intrinsics(source_path: str, n_views: int):
     return W, H, focal2fov(fx, W), focal2fov(fy, H)
 
 
+def frame_size(source_path: str, n_views: int, resolution: int = 1, resample_images: bool = False) -> Tuple[int, int]:
+    """The fly-through's (width, height): loaded_size of the cameras' size at -r resolution.  Raises ValueError for a
+    resolution that changes the size unless resample_images, and for an empty frame."""
+    from .scene_io import loaded_size
+    W, H, _, _ = intrinsics(source_path, n_views)
+    Wl, Hl = loaded_size(W, H, resolution)
+    if (Wl, Hl) != (W, H) and not resample_images:
+        raise ValueError(f"-r {resolution} resizes {W}x{H} to {Wl}x{Hl}; resampled images are not supported without "
+                         "--resample_images")
+    if Wl < 1 or Hl < 1:
+        raise ValueError(f"-r {resolution} resizes {W}x{H} to {Wl}x{Hl}, an empty frame")
+    return Wl, Hl
+
+
 def load(source_path: str, model_path: str, n_views: int, iteration: int = -1, white_background: bool = False,
-         device="cuda"):
+         device="cuda", resolution: int = 1, resample_images: bool = False):
     """What render.py loads for the fly-through: (tracker over point_cloud/iteration_<it>/point_cloud.ply, key poses
     pose/ours_<it>/pose_optimized.npy, it).  iteration -1: the largest saved one, for the model and the poses alike
     (render.py looks the poses up under the literal `ours_-1`).  Like render.py, no Mip-Splatting filters: a ply's
-    filter_3D is not used (build a PoseTracker with kernel_size and filter_3D and call frames_u8 for that)."""
+    filter_3D is not used (build a PoseTracker with kernel_size and filter_3D and call frames_u8 for that).  The
+    tracker renders at frame_size(resolution, resample_images)."""
     it = max_iteration(model_path) if int(iteration) == -1 else int(iteration)
     ply = os.path.join(model_path, "point_cloud", f"iteration_{it}", "point_cloud.ply")
     npy = os.path.join(model_path, "pose", f"ours_{it}", "pose_optimized.npy")
     for f in (ply, npy):
         if not os.path.isfile(f):
             raise FileNotFoundError(f"{f} not found")
-    W, H, fovx, fovy = intrinsics(source_path, n_views)
+    _, _, fovx, fovy = intrinsics(source_path, n_views)
+    W, H = frame_size(source_path, n_views, resolution, resample_images)
     return load_tracker(ply, W, H, fovx, fovy, white_background, device), np.load(npy), it
 
 
@@ -331,10 +352,15 @@ def main(argv=None) -> int:
                     help="frames per batched forward; scratch grows by about 150 P + 60 H W bytes a frame")
     ap.add_argument("--workers", type=int, default=None, help="PNG encoder threads (default: up to 8)")
     add_png_encoder_arg(ap)
+    ap.add_argument("-r", "--resolution", type=int, default=1,
+                    help="render at the size the training cameras load at with this -r (needs --resample_images when "
+                         "it changes the size)")
+    resample.add_arg(ap)
     a = ap.parse_args(argv)
     if a.n_views < 2:
         raise SystemExit("--n_views must be at least 2: the fly-through joins consecutive key poses")
-    tracker, keys, it = load(a.source_path, a.model_path, a.n_views, a.iterations, a.white_background)
+    tracker, keys, it = load(a.source_path, a.model_path, a.n_views, a.iterations, a.white_background, "cuda",
+                             a.resolution, resample.requested(a))
     n, folder = fly_through(tracker, keys, it, a.model_path, a.n_views, a.max_batch, a.workers,
                             png_writer(a.png_encoder))
     print(f"{n} frames -> {folder}")

@@ -17,6 +17,11 @@ uint8 -> /255 -> uint8; that round trip is the identity on all 256 levels (check
 so the gt PNGs are encoded from the decoded bytes.  Every PNG is encoded on freeview.write_pngs' thread pool, or on the
 GPU by png.write_pngs with --png_encoder gpu.
 
+--resample_images lets -r change the images' size: each stage's views are resized on the GPU to loadCam's size
+(Pillow's bicubic resize, byte for byte, resample.py), the renders are made at that size, and the gt files hold the
+resized bytes, as save_image(PILtoTorch(...)) writes them.  With --infer_video it also forwards -r to the fly-through.
+Without the flag such a -r is refused, and --infer_video renders at the full size as before.
+
 --test_fps with --eval is render.py's frame-rate report (render.py:172-186, report_fps): after the test renders, the
 last test view in sorted order is rendered 1000 times at its best pose, from a replayed CUDA graph
 (PoseTracker.time_renders), the rate of the trimmed mean is printed and appended to MODEL/total_fps.json, and the
@@ -29,7 +34,7 @@ with sentinel=False, so its defaults (white_background False included) always ov
 
     python -m instantsplat_b200.render_views -s SOURCE -m MODEL --n_views N --iterations IT [--eval] [--infer_video]
         [--optim_test_pose_iter 500] [--white_background] [--max_batch B] [--workers K] [--png_encoder pil|gpu]
-        [--test_fps]
+        [--test_fps] [-r R --resample_images]
 """
 from __future__ import annotations
 
@@ -43,7 +48,7 @@ from typing import Optional, Sequence, Tuple
 import numpy as np
 import torch
 
-from . import freeview
+from . import freeview, resample
 from .scene_io import Views, load_views, read_colmap_text
 from .tracking import PoseTracker
 from .train import save_time
@@ -164,6 +169,7 @@ def parser() -> argparse.ArgumentParser:
     freeview.add_png_encoder_arg(ap)
     ap.add_argument("--test_fps", action="store_true",
                     help="with --eval: time 1000 renders of the last test view and append the rate to total_fps.json")
+    resample.add_arg(ap)
     return ap
 
 
@@ -174,15 +180,17 @@ def main(argv=None) -> int:
     if a.infer_video and not a.eval:
         fv = ["-s", a.source_path, "-m", a.model_path, "--n_views", str(a.n_views), "--iterations", str(a.iterations),
               "--max_batch", str(a.max_batch)] + (["--white_background"] if a.white_background else []) \
-            + ([] if a.workers is None else ["--workers", str(a.workers)]) + ["--png_encoder", a.png_encoder]
+            + ([] if a.workers is None else ["--workers", str(a.workers)]) + ["--png_encoder", a.png_encoder] \
+            + (["-r", str(a.resolution), "--resample_images"] if resample.requested(a) else [])
         return freeview.main(fv)
     write = freeview.png_writer(a.png_encoder)
     it = freeview.max_iteration(a.model_path) if a.iterations == -1 else a.iterations
+    rdev = "cuda" if resample.requested(a) else None
     if a.eval:
         why = fps_refusal(a.source_path, a.n_views) if a.test_fps else None
         if why:
             raise SystemExit(f"render_views: {why}")
-        views = load_views(a.source_path, a.n_views, 1, a.resolution)
+        views = load_views(a.source_path, a.n_views, 1, a.resolution, resample_device=rdev)
         tracker = tracker_for(a.model_path, it, views, a.white_background)
         out = os.path.join(a.model_path, "test", f"ours_{it}")
         start = time.time()
@@ -193,7 +201,7 @@ def main(argv=None) -> int:
         npy = os.path.join(a.model_path, "pose", f"ours_{it}", "pose_optimized.npy")
         if not os.path.isfile(npy):
             raise FileNotFoundError(f"{npy} not found")
-        views = load_views(a.source_path, a.n_views, 0, a.resolution)
+        views = load_views(a.source_path, a.n_views, 0, a.resolution, resample_device=rdev)
         tracker = tracker_for(a.model_path, it, views, a.white_background)
         out = os.path.join(a.model_path, "train", f"ours_{it}")
         render_train(tracker, views, np.load(npy), out, a.max_batch, a.workers, write)

@@ -195,14 +195,19 @@ def split_train_test(items, n_views: int):
 class Views:
     """The cameras of one sparse_<n>/<k> folder, sorted by image_name: names [N] (image_name, the file name without
     its extension), w2c [N, 4, 4] fp64 world-to-camera matrices [qvec2rotmat(q) | t], images [N, H, W, 3] uint8 (the
-    decoded files), width / height (the images'), fovx / fovy (focal2fov of the intrinsics), camera_ids [N] (each
-    view's COLMAP camera id, intr.id: what readColmapCameras stores as the CameraInfo uid and train.py's save_pose
-    looks up as colmap_id; None when not known)."""
+    decoded files, resized to the loaded size when loadCam resizes them), width / height (the images'), fovx / fovy
+    (focal2fov of the intrinsics), camera_ids [N] (each view's COLMAP camera id, intr.id: what readColmapCameras
+    stores as the CameraInfo uid and train.py's save_pose looks up as colmap_id; None when not known),
+    source_width / source_height (the decoded files' size before any resize, CameraInfo's: what cameras.json and the
+    view-depth scale cap use; width / height when not given)."""
 
-    def __init__(self, names, w2c, images, width, height, fovx, fovy, camera_ids=None):
+    def __init__(self, names, w2c, images, width, height, fovx, fovy, camera_ids=None, source_width=None,
+                 source_height=None):
         self.names, self.w2c, self.images = list(names), w2c, images
         self.width, self.height, self.fovx, self.fovy = width, height, fovx, fovy
         self.camera_ids = None if camera_ids is None else [int(c) for c in camera_ids]
+        self.source_width = width if source_width is None else source_width
+        self.source_height = height if source_height is None else source_height
 
     def __len__(self) -> int:
         return len(self.names)
@@ -221,17 +226,26 @@ def loaded_size(width: int, height: int, resolution: int) -> Tuple[int, int]:
     return int(width / scale), int(height / scale)
 
 
-def load_views(source_path: str, n_views: int, split: int = 0, resolution: int = 1, images: str = "images") -> Views:
+def load_views(source_path: str, n_views: int, split: int = 0, resolution: int = 1, images: str = "images",
+               resample_device=None) -> Views:
     """render.py's cameras: readColmapSceneInfo (scene/dataset_readers.py:315-369) reads source/sparse_<n_views>/<split>
     ({0: the training views, 1: the test views of --eval}), cameras.txt (PINHOLE or SIMPLE_PINHOLE) and images.txt,
     opens source/<images>/<basename of the name> (`images`: train.py's -i, the folder name) and sorts the views by
     image_name; loadCam resizes each image to loaded_size(resolution) and divides by 255.
 
-    Refused, with the reason: a resolution at which loadCam would resample an image (only sizes PIL's resize copies
-    are kept), an image that is not 8-bit RGB (RGBA included: Camera's alpha mask is not implemented), and views
-    whose image size or field of view differ (one PoseTracker renders them all)."""
+    resample_device: None refuses a resolution at which loadCam would resample an image (only sizes PIL's resize
+    copies are kept); a CUDA device resizes the split's decoded images there, uploaded once and resized in one
+    resample.resize_u8 call (Pillow's bicubic resize, byte for byte), and keeps the decoded size in
+    Views.source_width / source_height.  Any other device is refused before a file is read.
+
+    Refused, with the reason: an image that is not 8-bit RGB (RGBA included: Camera's alpha mask is not implemented,
+    and Pillow's resize of RGBA premultiplies alpha), and views whose image size or field of view differ (one
+    PoseTracker renders them all)."""
     import math
     from PIL import Image
+    if resample_device is not None and _torch().device(resample_device).type != "cuda":
+        raise ValueError(f"resample_device {resample_device!r}: images are resized on a CUDA device only (there is no "
+                         "host resize)")
     folder = os.path.join(source_path, f"sparse_{n_views}", str(split))
     for f in ("cameras.txt", "images.txt"):
         if not os.path.isfile(os.path.join(folder, f)):
@@ -250,9 +264,10 @@ def load_views(source_path: str, n_views: int, split: int = 0, resolution: int =
                 raise ValueError(f"{path}: mode {im.mode}; only 8-bit RGB images are supported (an alpha channel "
                                  "would be Camera's gt_alpha_mask, which is not implemented)")
             W, H = im.size
-            if loaded_size(W, H, resolution) != (W, H):
+            if resample_device is None and loaded_size(W, H, resolution) != (W, H):
                 raise ValueError(f"{path}: -r {resolution} resizes {W}x{H} to {loaded_size(W, H, resolution)}; "
-                                 "resampled images are not supported (use -r 1, or -r -1 up to 1600 pixels wide)")
+                                 "resampled images are not supported (use -r 1, or -r -1 up to 1600 pixels wide, "
+                                 "or --resample_images)")
             pixels = np.array(im)
         fx = float(intr["params"][0])
         fy = fx if intr["model"] == "SIMPLE_PINHOLE" else float(intr["params"][1])
@@ -266,8 +281,21 @@ def load_views(source_path: str, n_views: int, split: int = 0, resolution: int =
         raise ValueError(f"{folder}: the cameras' intrinsics differ ({len(keys)} distinct image sizes and fields of "
                          "view); the views are rendered with one camera")
     W, H, fovx, fovy = keys.pop()
-    return Views([r[0] for r in recs], np.stack([r[1] for r in recs]), np.stack([r[2] for r in recs]), W, H, fovx, fovy,
-                 [r[4] for r in recs])
+    pixels = np.stack([r[2] for r in recs])
+    Wl, Hl = loaded_size(W, H, resolution)
+    if (Wl, Hl) != (W, H):
+        if Wl < 1 or Hl < 1:
+            raise ValueError(f"{folder}: -r {resolution} resizes {W}x{H} to {Wl}x{Hl}, an empty image")
+        from . import resample
+        pixels = resample.resize_u8(_torch().from_numpy(pixels).to(resample_device), (Wl, Hl)).cpu().numpy()
+    return Views([r[0] for r in recs], np.stack([r[1] for r in recs]), pixels, Wl, Hl, fovx, fovy,
+                 [r[4] for r in recs], W, H)
+
+
+def _torch():
+    import torch                 # only the GPU resize needs torch; the rest of this module is numpy
+    return torch
+
 
 
 # ----------------------------------------------------------------------------------------------

@@ -19,7 +19,12 @@ What train.py does between the parts this package already has, and where it live
   * cfg_args_text, cameras_json and input.ply: the files train.py writes beside the model, byte for byte.
 
 Refused with the reason before anything is written: --eval, --random_background, --sh_degree other than 3, a -r
-that resamples the images (load_views' refusals), camera ids that are not 1..n, a missing confidence_dsp.npy.
+that resamples the images without --resample_images (load_views' refusals), camera ids that are not 1..n, a missing
+confidence_dsp.npy.
+
+--resample_images (not one of train.py's flags, and not part of cfg_args) resizes the training images to loadCam's
+size on the GPU, Pillow's bicubic resize byte for byte (resample.py), and trains at that size; cameras.json and the
+view-depth scale cap keep the decoded size, as train.py's CameraInfo does.
 """
 from __future__ import annotations
 
@@ -37,7 +42,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 import torch
 
-from . import freeview
+from . import freeview, resample
 from .scene_io import Views, load_views, read_points3d_ply
 
 # ---- train.py's command line: arguments/__init__.py:47-94 and train.py:299-312 --------------------------------------
@@ -84,6 +89,7 @@ def parser() -> argparse.ArgumentParser:
     ap.add_argument("--disable_viewer", action="store_true", default=True, help="ignored (train.py's viewer)")
     ap.add_argument("--checkpoint_iterations", nargs="+", type=int, default=[])
     ap.add_argument("--start_checkpoint", type=str, default=None)
+    resample.add_arg(ap)
     return ap
 
 
@@ -214,11 +220,12 @@ class HostScene:
 
 
 def load_host_scene(source_path: str, n_views: int, resolution: int, images: str = "images",
-                    init_scale_from_view_depth: bool = False) -> HostScene:
-    """Everything of load_training_scene that is computed on the CPU.  Raises, before anything is written, on what
-    train.py cannot train: load_views' refusals, camera ids other than 1..n (save_pose looks up colmap ids 1..n and
-    would fail at the first save point), a missing points3D.ply or confidence_dsp.npy."""
-    views = load_views(source_path, n_views, 0, resolution, images)
+                    init_scale_from_view_depth: bool = False, resample_device=None) -> HostScene:
+    """Everything of load_training_scene that is computed on the CPU, except the image resize of a CUDA
+    resample_device (load_views').  Raises, before anything is written, on what train.py cannot train: load_views'
+    refusals, camera ids other than 1..n (save_pose looks up colmap ids 1..n and would fail at the first save point),
+    a missing points3D.ply or confidence_dsp.npy."""
+    views = load_views(source_path, n_views, 0, resolution, images, resample_device)
     ids = list(views.camera_ids)
     if sorted(ids) != list(range(1, len(views) + 1)):
         raise ValueError(f"sparse_{n_views}/0: camera ids {ids}; train.py's save_pose needs every camera id 1..{len(views)} "
@@ -234,7 +241,8 @@ def load_host_scene(source_path: str, n_views: int, resolution: int, images: str
     order = scene_order(len(views))
     sg = None
     if init_scale_from_view_depth:
-        sg = scale_from_view_depth(xyz, views.w2c, fov2focal(views.fovx, views.width), fov2focal(views.fovy, views.height))
+        sg = scale_from_view_depth(xyz, views.w2c, fov2focal(views.fovx, views.source_width),
+                                   fov2focal(views.fovy, views.source_height))
     return HostScene(views=views, order=order, colmap_ids=[ids[i] for i in order],
                      poses=freeview.poses_from_w2c(views.w2c[order]), extent=nerfpp_radius(views.w2c), points=xyz,
                      colors=rgb / 255.0, per_point_lr=ppl, scale_gaussian=sg, ply_path=ply_path)
@@ -251,17 +259,19 @@ class TrainingScene:
 
 def load_training_scene(source_path: str, n_views: int, resolution: int, images: str = "images", sh_degree: int = 3,
                         white_background: bool = False, init_scale_from_view_depth: bool = False,
-                        device="cuda") -> TrainingScene:
+                        device="cuda", resample_images: bool = False) -> TrainingScene:
     """train.py's Scene(dataset, gaussians) with its confidence: the cameras, their order, the pose table, the initial
     Gaussians (GaussianModel.create_from_pcd, spatial_lr_scale = the extent, its knn on the GPU), the per-point
-    learning rates and the targets."""
-    host = load_host_scene(source_path, n_views, resolution, images, init_scale_from_view_depth)
+    learning rates and the targets.  resample_images: resize the images on device when -r changes their size."""
+    host = load_host_scene(source_path, n_views, resolution, images, init_scale_from_view_depth,
+                           device if resample_images else None)
     return _device_scene(host, sh_degree, white_background, torch.device(device))
 
 
 # ---- the files train.py writes beside the model ------------------------------------------------------------------
 def cameras_json(views: Views) -> List[dict]:
-    """camera_to_JSON (utils/camera_utils.py:66-86) of every camera in image_name order, before the shuffle."""
+    """camera_to_JSON (utils/camera_utils.py:66-86) of every camera in image_name order, before the shuffle, at the
+    decoded size (CameraInfo's), whatever size the images are loaded at."""
     out = []
     for i, name in enumerate(views.names):
         Rt = np.zeros((4, 4))
@@ -269,9 +279,10 @@ def cameras_json(views: Views) -> List[dict]:
         Rt[:3, 3] = views.w2c[i][:3, 3]
         Rt[3, 3] = 1.0
         W2C = np.linalg.inv(Rt)
-        out.append({"id": i, "img_name": name, "width": views.width, "height": views.height,
+        W, H = views.source_width, views.source_height
+        out.append({"id": i, "img_name": name, "width": W, "height": H,
                     "position": W2C[:3, 3].tolist(), "rotation": [x.tolist() for x in W2C[:3, :3]],
-                    "fy": fov2focal(views.fovy, views.height), "fx": fov2focal(views.fovx, views.width)})
+                    "fy": fov2focal(views.fovy, H), "fx": fov2focal(views.fovx, W)})
     return out
 
 
@@ -342,7 +353,7 @@ def run(args: argparse.Namespace, device="cuda", log=print) -> RunResult:
     t0 = time.perf_counter()
     try:
         host = load_host_scene(args.source_path, args.n_views, args.resolution, args.images,
-                               args.init_scale_from_view_depth)
+                               args.init_scale_from_view_depth, dev if resample.requested(args) else None)
     except (ValueError, FileNotFoundError) as e:
         raise Refused(str(e)) from e
     phases["load"] = time.perf_counter() - t0
