@@ -73,6 +73,8 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
 // What the forward compares: the pixel values as they are (the training loss), clamped to [0, 1] (train.py's
 // training_report), or through torchvision's save_image and to_tensor (render.py -> metrics.py):
 // uint8(clamp(x * 255 + 0.5, 0, 255)) / 255 in fp32, truncating, so exact ties round up.
+// NaN: the clamp keeps it, as torch.clamp does, so a diverged render reports NaN metrics rather than plausible
+// finite ones (fminf / fmaxf alone would return the bound); save_image's quantisation makes it 0, as png8_level does.
 enum { kInRaw = 0, kInClamp = GSB_METRIC_CLAMP, kInPng8 = GSB_METRIC_PNG8 };
 
 // save_image's 8-bit level of x as a float in {0, ..., 255}: x.mul(255).add_(0.5).clamp_(0, 255).to(uint8) with each
@@ -83,7 +85,7 @@ __device__ __forceinline__ float png8_level(float x) {
 
 template <int kIn>
 __device__ __forceinline__ float metric_input(float x) {
-  if constexpr (kIn == kInClamp) return fminf(fmaxf(x, 0.f), 1.f);
+  if constexpr (kIn == kInClamp) return isnan(x) ? x : fminf(fmaxf(x, 0.f), 1.f);
   if constexpr (kIn == kInPng8) return __fdiv_rn(png8_level(x), 255.f);
   return x;
 }

@@ -8,6 +8,10 @@ Two conventions, both kept:
   * mode="png8": render and target through torchvision's save_image (8-bit, ties round up) and to_tensor (/255), as
     render.py -> metrics.py does.  metrics.py's PSNR is that of the whole image's MSE (a [1, 3, H, W] image): `psnr`.
 SSIM is the training loss's (utils/loss_utils.py:55-85) on the transformed images.
+
+NaN follows torch in both: the clamp keeps it (torch.clamp), so a render with a NaN pixel gets NaN l1, ssim and psnr,
+and NaN psnr_channels in that pixel's channel (its other channels and the other views are unaffected); save_image's
+quantisation makes it 0 (+inf 255, -inf 0), so png8 stays finite as render.py's PNG files do.
 """
 from __future__ import annotations
 
