@@ -45,14 +45,19 @@ NEAR = 0.2               # kNear
 REC_TOL = 2e-5
 
 
-def geom_layout(P):
-    """Byte offset and length of each GeomView part, and the total (= gsb_geom_bytes(P))."""
+def geom_layout(P, V=1, ntiles=0):
+    """Byte offset and length of each GeomView part, and the total (= gsb_geom_bytes(P); for a batch of V views of
+    frames of ntiles 16x16 tiles, gsb_geom_bytes_batch: every per-record part holds V * P records, cam, dscale,
+    pose_part and pose_acc one row per view, the per-tile parts max(V * ntiles, kMaxTiles) slots)."""
     pp = max(int(P), 1)
+    nv = max(int(V), 1)
+    vp = nv * pp
     nb = (pp + PT - 1) // PT
-    parts = (("cam", CAMCONST_BYTES), ("rec", pp * 48), ("brec", pp * 16), ("tiles", pp * 4), ("clamped", pp),
-             ("dacc", pp * DACC_SLOTS * 8), ("dscale", 4), ("pose_part", nb * 16 * 4), ("pose_acc", 16 * 4),
-             ("status", 8 * 4), ("aux", 64 * 4), ("tcount", MAX_TILES * 4), ("tstart", MAX_TILES * 4),
-             ("tcursor", MAX_TILES * 4), ("q_large", MAX_TILES * 4), ("q_huge", MAX_TILES * 4), ("q_big", pp * 4))
+    ts = max(nv * int(ntiles), MAX_TILES)
+    parts = (("cam", nv * CAMCONST_BYTES), ("rec", vp * 48), ("brec", vp * 16), ("tiles", vp * 4), ("clamped", vp),
+             ("dacc", vp * DACC_SLOTS * 8), ("dscale", nv * 4), ("pose_part", nv * nb * 16 * 4),
+             ("pose_acc", nv * 16 * 4), ("status", 8 * 4), ("aux", 64 * 4), ("tcount", ts * 4), ("tstart", ts * 4),
+             ("tcursor", ts * 4), ("q_large", ts * 4), ("q_huge", ts * 4), ("q_big", vp * 4))
     out, off = {}, 0
     for name, nbytes in parts:
         out[name] = (off, nbytes)

@@ -97,6 +97,9 @@ void host_project_bwd(const HostCam* h, int P, const float* means, const float* 
   }
 }
 
+// pose_grad_finalize alone: acc [16] = [dqc_raw(4), dt(3), dRc(9)] -> dpose [7]
+void host_pose_grad_finalize(const float* pose, const float* acc, float* dpose) { pose_grad_finalize(pose, acc, dpose); }
+
 // rect_may_contribute brute-force check helper: returns 1 if the predicate says "may contribute"
 int host_rect_may_contribute(float x, float y, float A, float B, float C, float opacity, float rx0,
                              float ry0, float rx1, float ry1) {
