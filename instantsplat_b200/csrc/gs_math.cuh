@@ -92,7 +92,8 @@ GS_HD void pose_grad_finalize(const float* pose, const float* acc, float* dpose)
 
 // Mip-Splatting filters (DESIGN.md section 4.7).  on2d: the 2D Mip filter, kappa * I replaces the 0.3 px^2 dilation and
 // the opacity is compensated by h2 = sqrt(max(kMipH2Min, det(Sigma2) / det(Sigma2 + kappa I))).  on3d: the 3D
-// smoothing filter of size f (world units, raw parameters only): s~ = sqrt(s^2 + f^2), opacity * prod_k s_k / s~_k.
+// smoothing filter of size f (world units, raw parameters only): s~ = sqrt(s^2 + f^2), opacity * prod_k s_k / s~_k;
+// f = 0: no 3D filter for that Gaussian.
 // Mip() (on == 0) is the reference path, operation for operation.
 constexpr float kMipH2Min = 2.5e-5f;
 struct Mip {
@@ -249,7 +250,10 @@ GS_HD void project_geometry(const CamConst& c, const GaussIn& in, const float* c
     o.mc[0] = in.m[0]; o.mc[1] = in.m[1]; o.mc[2] = in.m[2];
     o.q[0] = in.q[0]; o.q[1] = in.q[1]; o.q[2] = in.q[2]; o.q[3] = in.q[3];
   }
-  if (kMip && c.raw_params && mf.on3d) {                // kMip == false: folded away at compile time
+  // f == 0 is no 3D filter for this Gaussian: the unfiltered arithmetic, not (s*s)/(s*s), which is 0/0 once s*s
+  // underflows (log-scale <= -52)
+  const bool f3d = kMip && c.raw_params && mf.on3d && mf.f != 0.f;   // kMip == false: folded away at compile time
+  if (f3d) {
     const float f2 = mf.f * mf.f;
     float r = 1.f;                                 // prod_k s_k^2 / (s_k^2 + f^2), one bounded factor at a time
     for (int k = 0; k < 3; ++k) {
@@ -268,7 +272,7 @@ GS_HD void project_geometry(const CamConst& c, const GaussIn& in, const float* c
     o.s[0] = c.scale_mod * in.sc[0]; o.s[1] = c.scale_mod * in.sc[1]; o.s[2] = c.scale_mod * in.sc[2];
     o.opacity = in.op;
   }
-  if (kMip && mf.on) { if (!(c.raw_params && mf.on3d)) o.sig = o.opacity; o.o3 = o.opacity; }
+  if (kMip && mf.on) { if (!f3d) o.sig = o.opacity; o.o3 = o.opacity; }
   const float* m = o.mc;
   // ---- view / clip transforms
   float tx = m[0] * c.V[0] + m[1] * c.V[4] + m[2] * c.V[8] + c.V[12];
@@ -595,7 +599,7 @@ GS_HD void project_bwd(const CamConst& c, const GaussIn& in, const Proj& p, cons
   if (kMip && mf.on) {
     // o_eff = sig * h3 * h2 (h3 = prod_k s_k / s~_k with the 3D filter, else 1); neither filter's f or kappa is trained
     const float dsig = dop * p.h2 * p.h3;
-    if (c.raw_params && mf.on3d) {
+    if (c.raw_params && mf.on3d && mf.f != 0.f) {
       // o.s = mod * s~, s~^2 = s^2 + f^2, s = exp(sc):  d(mod s~)/dsc = o.s * s^2 / s~^2,  dh3/dsc = h3 f^2 / s~^2
       const float f2 = mf.f * mf.f, dh3 = dop * p.h2 * p.sig * p.h3;
       for (int k = 0; k < 3; ++k) {

@@ -290,25 +290,6 @@ def test_trainer_with_filters_is_deterministic_and_matches_boundary():
 
 
 # ---- records, cull, mass -------------------------------------------------------------------------------------------
-def _mip_records(sc, view, kappa, f3d, deg=3):
-    """`_geom.oracle_records` of the filtered projection (fp64)."""
-    p = {k: v.detach().double() for k, v in sc.params.items()}
-    cam = O.Camera.instantsplat(sc.width, sc.height, sc.fovx, sc.fovy, sh_degree=deg, dtype=torch.float64)
-    means, rots = O.pose_pretransform(p["xyz"], p["rotation"], sc.poses[view].double())
-    s, o = torch.exp(p["scaling"]), torch.sigmoid(p["opacity"]).reshape(-1)
-    if f3d is not None:
-        s, o = MIP.apply_filter3d(s, o, f3d.double())
-    shs = torch.cat([p["f_dc"], p["f_rest"]], 1)
-    with torch.no_grad():
-        proj = MIP.project_mip(means, s, rots, o, shs, cam, kappa)
-        proj["tview"] = means
-        d = means / means.norm(dim=1, keepdim=True)
-        proj["raw_rgb"] = O.eval_sh(deg, shs, d) + 0.5
-        proj["limx"], proj["limy"] = 1.3 * cam.tanfovx, 1.3 * cam.tanfovy
-        proj["W"], proj["H"], proj["mean_norm"] = cam.width, cam.height, means.norm(dim=1)
-    return proj
-
-
 def test_records_follow_the_filtered_opacity_and_cull_is_lossless():
     import instantsplat_b200 as I
     import instantsplat_b200.rasterizer as RZ
@@ -322,7 +303,8 @@ def test_records_follow_the_filtered_opacity_and_cull_is_lossless():
                 sc.poses[0].to(DEV), torch.zeros(sc.P, 3, device=DEV), rs, None if f is None else f.to(DEV))
         x = [t.clone().requires_grad_(True) if k < 7 else t for k, t in enumerate(args)]
         img, _ = I.rasterize_fused(*x)
-        o = _mip_records(sc, 0, kappa, f)
+        cam = O.Camera.instantsplat(sc.width, sc.height, sc.fovx, sc.fovy, sh_degree=3)
+        o = MIP.mip_records(sc.params, sc.poses[0], cam, kappa, f)
         d = G.decode(img.grad_fn.st)
         # h2 comes from det(Sigma2) = a0 c0 - b^2, resolved by fp32 to (a0 c0 + b^2) / det * 6e-8 relative: the record
         # opacity of an ill-conditioned Gaussian (a needle far below a pixel) is bounded on that scale, flagged and
