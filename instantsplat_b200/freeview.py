@@ -28,8 +28,13 @@ size, loaded_size of cameras.txt's width and height at -r (init_geo writes the i
 --resample_images the frames are rendered at that size; without it a -r that changes the size is refused, and the
 frames are the full-size ones.
 
+Like render.py, the fly-through renders without Mip-Splatting's filters, and a ply's filter_3D property is then not
+used.  --kernel_size K (mip.py) renders every frame with both filters: the 2D filter at K and the ply's filter_3D.
+It is refused, before anything is written, for a K that is negative, NaN or infinite and for a ply without filter_3D
+(a model trained without --kernel_size).
+
     python -m instantsplat_b200.freeview -s SOURCE -m MODEL --n_views N --iterations IT [--white_background]
-        [--png_encoder pil|gpu] [-r R --resample_images]
+        [--png_encoder pil|gpu] [-r R --resample_images] [--kernel_size K]
 """
 from __future__ import annotations
 
@@ -43,7 +48,7 @@ from typing import Iterable, Iterator, Optional, Sequence, Tuple
 import numpy as np
 import torch
 
-from . import _lib, png, resample
+from . import _lib, mip, png, resample
 from ._lib import check
 from .frame import ST_OVERFLOW
 from .tracking import PoseTracker
@@ -300,44 +305,62 @@ def frame_size(source_path: str, n_views: int, resolution: int = 1, resample_ima
     return Wl, Hl
 
 
-def load(source_path: str, model_path: str, n_views: int, iteration: int = -1, white_background: bool = False,
-         device="cuda", resolution: int = 1, resample_images: bool = False):
-    """What render.py loads for the fly-through: (tracker over point_cloud/iteration_<it>/point_cloud.ply, key poses
-    pose/ours_<it>/pose_optimized.npy, it).  iteration -1: the largest saved one, for the model and the poses alike
-    (render.py looks the poses up under the literal `ours_-1`).  Like render.py, no Mip-Splatting filters: a ply's
-    filter_3D is not used (build a PoseTracker with kernel_size and filter_3D and call frames_u8 for that).  The
-    tracker renders at frame_size(resolution, resample_images)."""
+def model_files(model_path: str, iteration: int = -1) -> Tuple[str, str, int]:
+    """(point_cloud/iteration_<it>/point_cloud.ply, pose/ours_<it>/pose_optimized.npy, it) of a trained model;
+    iteration -1: the largest saved one, for the model and the poses alike (render.py looks the poses up under the
+    literal `ours_-1`)."""
     it = max_iteration(model_path) if int(iteration) == -1 else int(iteration)
-    ply = os.path.join(model_path, "point_cloud", f"iteration_{it}", "point_cloud.ply")
-    npy = os.path.join(model_path, "pose", f"ours_{it}", "pose_optimized.npy")
+    return (os.path.join(model_path, "point_cloud", f"iteration_{it}", "point_cloud.ply"),
+            os.path.join(model_path, "pose", f"ours_{it}", "pose_optimized.npy"), it)
+
+
+def load(source_path: str, model_path: str, n_views: int, iteration: int = -1, white_background: bool = False,
+         device="cuda", resolution: int = 1, resample_images: bool = False, kernel_size: Optional[float] = None):
+    """What render.py loads for the fly-through: (tracker over model_files' ply, key poses from its
+    pose_optimized.npy, it).  Like render.py, no Mip-Splatting filters unless kernel_size is given; then the tracker
+    applies the 2D filter with it and the ply's filter_3D (load_tracker).  The tracker renders at
+    frame_size(resolution, resample_images)."""
+    ply, npy, it = model_files(model_path, iteration)
     for f in (ply, npy):
         if not os.path.isfile(f):
             raise FileNotFoundError(f"{f} not found")
     _, _, fovx, fovy = intrinsics(source_path, n_views)
     W, H = frame_size(source_path, n_views, resolution, resample_images)
-    return load_tracker(ply, W, H, fovx, fovy, white_background, device), np.load(npy), it
+    return load_tracker(ply, W, H, fovx, fovy, white_background, device, kernel_size), np.load(npy), it
 
 
 def load_tracker(ply: str, width: int, height: int, fovx: float, fovy: float, white_background: bool = False,
-                 device="cuda") -> PoseTracker:
+                 device="cuda", kernel_size: Optional[float] = None) -> PoseTracker:
     """A PoseTracker over a saved point_cloud.ply as render.py renders it: the SH degree from the file's coefficient
-    count, a black or white background, no Mip-Splatting filters."""
+    count, a black or white background.  No Mip-Splatting filters unless kernel_size is given (a filter_3D property
+    in the file is then not used); with it, the 2D filter at kernel_size and the file's filter_3D, which it must
+    carry (tracker_from_gaussians)."""
     from .scene_io import load_gaussians_ply
     g = {k: torch.from_numpy(np.ascontiguousarray(a)) for k, a in load_gaussians_ply(ply).items()}
-    return tracker_from_gaussians(g, width, height, fovx, fovy, white_background, device, ply)
+    return tracker_from_gaussians(g, width, height, fovx, fovy, white_background, device, ply, kernel_size)
 
 
 def tracker_from_gaussians(g, width: int, height: int, fovx: float, fovy: float, white_background: bool = False,
-                           device="cuda", where: str = "the model") -> PoseTracker:
+                           device="cuda", where: str = "the model", kernel_size: Optional[float] = None) -> PoseTracker:
     """load_tracker without the file: g holds load_gaussians_ply's tensors (JointTrainer.ply_tensors gives them from a
-    trainer).  Tensors already on the device, fp32 and contiguous are shared with the tracker, not copied."""
+    trainer).  Tensors already on the device, fp32 and contiguous are shared with the tracker, not copied.
+    kernel_size: Mip-Splatting's filters, the 2D one at kernel_size and the 3D one from g["filter_3D"] (a ValueError
+    when g has none); None: neither, whatever g holds."""
     M = 1 + g["f_rest"].shape[1]
     deg = int(round(M ** 0.5)) - 1
     if (deg + 1) ** 2 != M:
         raise ValueError(f"{where}: {M} SH coefficients per channel is not a square")
+    kw = {}
+    if kernel_size is not None:
+        why = mip.kernel_refusal(kernel_size)
+        if why:
+            raise ValueError(why)
+        if "filter_3D" not in g:
+            raise ValueError(f"{where}: no filter_3D, so there is no 3D filter to apply with kernel_size {kernel_size}")
+        kw = dict(kernel_size=float(kernel_size), filter_3D=g["filter_3D"])
     bg = torch.ones(3) if white_background else torch.zeros(3)
     return PoseTracker(g["xyz"], g["rotation"], g["scaling"], g["opacity"], g["f_dc"], g["f_rest"], width, height, fovx,
-                       fovy, bg=bg, sh_degree=deg, device=device)
+                       fovy, bg=bg, sh_degree=deg, device=device, **kw)
 
 
 def main(argv=None) -> int:
@@ -356,11 +379,17 @@ def main(argv=None) -> int:
                     help="render at the size the training cameras load at with this -r (needs --resample_images when "
                          "it changes the size)")
     resample.add_arg(ap)
+    mip.add_arg(ap)
     a = ap.parse_args(argv)
     if a.n_views < 2:
         raise SystemExit("--n_views must be at least 2: the fly-through joins consecutive key poses")
+    k = mip.kernel_size(a)
+    if k is not None:
+        why = mip.kernel_refusal(k) or mip.ply_refusal(k, model_files(a.model_path, a.iterations)[0])
+        if why:
+            raise SystemExit(f"freeview: {why}")
     tracker, keys, it = load(a.source_path, a.model_path, a.n_views, a.iterations, a.white_background, "cuda",
-                             a.resolution, resample.requested(a))
+                             a.resolution, resample.requested(a), **({} if k is None else {"kernel_size": k}))
     n, folder = fly_through(tracker, keys, it, a.model_path, a.n_views, a.max_batch, a.workers,
                             png_writer(a.png_encoder))
     print(f"{n} frames -> {folder}")

@@ -2,9 +2,10 @@
 on one GPU (DESIGN.md section 4.18).
 
     python -m instantsplat_b200.pipeline eval  --data_root ROOT --output_dir OUT --datasets D.. --scenes S..
-        --n_views N.. --iterations IT.. [--lpips_weights DIR] [--workers K] [--png_encoder pil|gpu] [--test_fps]
+        --n_views N.. --iterations IT.. [--lpips_weights DIR] [--workers W] [--png_encoder pil|gpu] [--test_fps]
+        [--kernel_size K]
     python -m instantsplat_b200.pipeline infer --data_root ROOT --output_dir OUT --datasets D.. --scenes S..
-        --n_views N.. --iterations IT.. [--workers K] [--png_encoder pil|gpu]
+        --n_views N.. --iterations IT.. [--workers W] [--png_encoder pil|gpu] [--kernel_size K]
 
 Tasks run in the scripts' loop order (dataset, scene, n_views, iterations), one after another.  The source is
 ROOT/D/S/24_views for eval and ROOT/D/S for infer; the model is OUT/D/S/<N>_views.  Each stage is the stage module's
@@ -20,6 +21,11 @@ memory instead:
     render_views.report_fps at the last test view's best pose, which writes total_fps.json into the model directory.
   * metrics: metrics.evaluate with the current test/ours_<it> from memory, any earlier method from its files.
   * infer: freeview.fly_through.
+
+Like the stage CLIs, the render stages use no Mip-Splatting filter unless --kernel_size K is given.  With it, the
+train, render and fly-through lines carry --kernel_size K (metrics scores PNGs and needs nothing), the trainer trains
+with both filters, and its filter_3D goes to the trackers with the rest of ply_tensors.  A K that is negative, NaN or
+infinite is refused with the other refusals.
 
 Every PNG goes to one process-wide encoder pool (PngWriter) that the GPU stages do not wait for, up to a bound on the
 frames queued; with --png_encoder gpu the frames are encoded on the GPU and the pool only writes the files.  Every
@@ -41,7 +47,7 @@ from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from . import freeview, metrics, png, render_views, train
+from . import freeview, metrics, mip, png, render_views, train
 from .scene_io import load_views, pose_matrices
 
 # stage -> (log file, the script's start line, its completion line)
@@ -84,31 +90,40 @@ def tasks(mode: str, data_root: str, output_dir: str, datasets: Sequence[str], s
     return out
 
 
-def stage_argv(t: Task, lpips_weights: Optional[str] = None, test_fps: bool = False) -> Dict[str, List[str]]:
-    """Each stage's command line as the script writes it; test_fps adds --test_fps to the test-view renders'."""
+def stage_argv(t: Task, lpips_weights: Optional[str] = None, test_fps: bool = False,
+               kernel_size: Optional[float] = None) -> Dict[str, List[str]]:
+    """Each stage's command line as the script writes it; test_fps adds --test_fps to the test-view renders';
+    kernel_size adds --kernel_size to the train, render and fly-through lines (not to metrics, which scores PNGs)."""
     base = ["-s", t.source, "-m", t.model, "-r", "1", "--n_views", str(t.n_views), "--iterations", str(t.iterations)]
-    out = {"train": base + ["--pp_optimizer", "--optim_pose"]}
+    k = mip.argv(kernel_size)
+    out = {"train": base + ["--pp_optimizer", "--optim_pose"] + k}
     if t.mode == "eval":
-        out["render_train"] = list(base)
-        out["render_test"] = base + ["--eval"] + (["--test_fps"] if test_fps else [])
+        out["render_train"] = base + k
+        out["render_test"] = base + ["--eval"] + (["--test_fps"] if test_fps else []) + k
         out["metrics"] = ["-s", t.source, "-m", t.model, "--n_views", str(t.n_views)] \
             + ([] if lpips_weights is None else ["--lpips_weights", lpips_weights])
     else:
-        out["render"] = base + ["--infer_video"]
+        out["render"] = base + ["--infer_video"] + k
     return out
 
 
-def stage_args(t: Task, lpips_weights: Optional[str] = None, test_fps: bool = False) -> Dict[str, argparse.Namespace]:
+def stage_args(t: Task, lpips_weights: Optional[str] = None, test_fps: bool = False,
+               kernel_size: Optional[float] = None) -> Dict[str, argparse.Namespace]:
     """stage_argv parsed by each stage's own parser."""
     parse = {"train": train.parse_args, "metrics": lambda a: metrics.parser().parse_args(a)}
     return {k: parse.get(k, lambda a: render_views.parser().parse_args(a))(v)
-            for k, v in stage_argv(t, lpips_weights, test_fps).items()}
+            for k, v in stage_argv(t, lpips_weights, test_fps, kernel_size).items()}
 
 
-def refusals(t: Task, test_fps: bool = False) -> List[str]:
+def refusals(t: Task, test_fps: bool = False, kernel_size: Optional[float] = None) -> List[str]:
     """Why the task cannot run, each reason with its path; empty when it can.  Reads the source, writes nothing.
-    test_fps: the eval task's test-view renders carry --test_fps, which needs a test view."""
+    test_fps: the eval task's test-view renders carry --test_fps, which needs a test view; kernel_size: the stages
+    carry --kernel_size, which must be a finite number >= 0.  The model the render stages read is the train stage's,
+    in memory, and carries filter_3D whenever the train stage has the flag."""
     out = []
+    why = mip.kernel_refusal(kernel_size)
+    if why:
+        out.append(why)
     f0 = os.path.join(t.source, f"sparse_{t.n_views}", "0")
     for name in ("points3D.ply", "confidence_dsp.npy"):
         if not os.path.isfile(os.path.join(f0, name)):
@@ -122,7 +137,7 @@ def refusals(t: Task, test_fps: bool = False) -> List[str]:
         out.append(why)
     if out:
         return out
-    a = stage_args(t)["train"]
+    a = stage_args(t, kernel_size=kernel_size)["train"]
     out += train.refusals(a)
     try:
         train.load_host_scene(a.source_path, a.n_views, a.resolution, a.images, a.init_scale_from_view_depth)
@@ -220,10 +235,11 @@ def _stage(t: Task, key: str, times: Dict[str, float]):
 
 
 def run_task(t: Task, pool: PngWriter, lpips_net=None, lpips_weights: Optional[str] = None,
-             device="cuda", test_fps: bool = False) -> Tuple[int, Dict[str, float]]:
-    """The script's run_on_gpu from stage 2 on, with test_fps: stage 4 with --test_fps.  Returns (model directories
-    metrics could not evaluate, wall seconds per stage).  The trainer and trackers are released before it returns."""
-    a = stage_args(t, lpips_weights, test_fps)
+             device="cuda", test_fps: bool = False, kernel_size: Optional[float] = None) -> Tuple[int, Dict[str, float]]:
+    """The script's run_on_gpu from stage 2 on, with test_fps: stage 4 with --test_fps; kernel_size: every stage but
+    metrics with --kernel_size (the trainer's filter_3D handed to the trackers).  Returns (model directories metrics
+    could not evaluate, wall seconds per stage).  The trainer and trackers are released before it returns."""
+    a = stage_args(t, lpips_weights, test_fps, kernel_size)
     times, failed = {}, 0
     print("=" * 55)
     print(f"Starting process: {t.label}")
@@ -237,19 +253,21 @@ def run_task(t: Task, pool: PngWriter, lpips_net=None, lpips_weights: Optional[s
         del res
         gc.collect()                                # the trainer, its graphs and scratch
     it = t.iterations
-    tracker = lambda v, white: freeview.tracker_from_gaussians(g, v.width, v.height, v.fovx, v.fovy, white, device)
+    tracker = lambda v, r: freeview.tracker_from_gaussians(g, v.width, v.height, v.fovx, v.fovy, r.white_background,
+                                                           device, kernel_size=mip.kernel_size(r))
     if t.mode == "infer":
         r = a["render"]
         with _stage(t, "render", times):
             W, H, fovx, fovy = freeview.intrinsics(t.source, t.n_views)
-            tk = freeview.tracker_from_gaussians(g, W, H, fovx, fovy, r.white_background, device)
+            tk = freeview.tracker_from_gaussians(g, W, H, fovx, fovy, r.white_background, device,
+                                                 kernel_size=mip.kernel_size(r))
             n, folder = freeview.fly_through(tk, keys, it, t.model, t.n_views, r.max_batch, write=pool.write)
             print(f"{n} frames -> {folder}")
     else:
         r = a["render_train"]
         with _stage(t, "render_train", times):
             out = os.path.join(t.model, "train", f"ours_{it}")
-            render_views.render_train(tracker(views, r.white_background), views, keys, out, r.max_batch,
+            render_views.render_train(tracker(views, r), views, keys, out, r.max_batch,
                                       write=pool.write)
             print(f"{len(views)} views -> {out}")
         r = a["render_test"]
@@ -262,7 +280,7 @@ def run_task(t: Task, pool: PngWriter, lpips_net=None, lpips_weights: Optional[s
         with _stage(t, "render_test", times):
             views = load_views(t.source, t.n_views, 1, r.resolution)
             out = os.path.join(t.model, "test", f"ours_{it}")
-            tk = tracker(views, r.white_background)
+            tk = tracker(views, r)
             start = time.time()
             best = render_views.render_test(tk, views, out, r.optim_test_pose_iter, r.max_batch, write=keep)
             if r.test_fps:
@@ -289,16 +307,17 @@ def run_task(t: Task, pool: PngWriter, lpips_net=None, lpips_weights: Optional[s
 
 
 def run_tasks(ts: Sequence[Task], workers: Optional[int] = None, lpips_net=None, lpips_weights: Optional[str] = None,
-              device="cuda", png_encoder: str = "pil", test_fps: bool = False) -> Tuple[int, List[Dict[str, float]]]:
-    """Every task in order on one encoder pool (PngWriter with png_encoder), then every write waited for; test_fps:
-    run_task's.  Returns (model directories metrics could not evaluate, per-task stage times).  Raises WriteError
+              device="cuda", png_encoder: str = "pil", test_fps: bool = False,
+              kernel_size: Optional[float] = None) -> Tuple[int, List[Dict[str, float]]]:
+    """Every task in order on one encoder pool (PngWriter with png_encoder), then every write waited for; test_fps
+    and kernel_size: run_task's.  Returns (model directories metrics could not evaluate, per-task stage times).  Raises WriteError
     when a PNG could not be written."""
     pool = PngWriter(workers, png_encoder)
     failed, times = 0, []
     try:
         for k, t in enumerate(ts, 1):
             print(f"Processing task {k} / {len(ts)}", flush=True)
-            f, s = run_task(t, pool, lpips_net, lpips_weights, device, test_fps)
+            f, s = run_task(t, pool, lpips_net, lpips_weights, device, test_fps, kernel_size)
             failed += f
             times.append(s)
     finally:
@@ -328,6 +347,7 @@ def parser() -> argparse.ArgumentParser:
         p.add_argument("--workers", type=int, default=None, help="PNG encoder threads for the whole run (default: up "
                                                                   "to 8)")
         freeview.add_png_encoder_arg(p)
+        mip.add_arg(p)
     return ap
 
 
@@ -337,8 +357,9 @@ def main(argv=None) -> int:
     if a.workers is not None and a.workers < 1:
         ap.error("--workers must be at least 1")
     weights, test_fps = getattr(a, "lpips_weights", None), getattr(a, "test_fps", False)
+    k = mip.kernel_size(a)
     ts = tasks(a.mode, a.data_root, a.output_dir, a.datasets, a.scenes, a.n_views, a.iterations)
-    bad = [f"{t.label}: {r}" for t in ts for r in refusals(t, test_fps)]
+    bad = [f"{t.label}: {r}" for t in ts for r in refusals(t, test_fps, k)]
     if bad:
         raise SystemExit("\n".join(f"instantsplat_b200.pipeline: {b}" for b in bad))
     net = None
@@ -349,7 +370,8 @@ def main(argv=None) -> int:
         except (OSError, ValueError) as e:
             ap.error(str(e))
     try:
-        failed, _ = run_tasks(ts, a.workers, net, weights, png_encoder=a.png_encoder, test_fps=test_fps)
+        failed, _ = run_tasks(ts, a.workers, net, weights, png_encoder=a.png_encoder, test_fps=test_fps,
+                              kernel_size=k)
     except WriteError as e:
         raise SystemExit(f"instantsplat_b200.pipeline: {e}")
     print("=" * 55)

@@ -28,13 +28,19 @@ last test view in sorted order is rendered 1000 times at its best pose, from a r
 `[4] render` line of train_time.txt records the test stage's time with the loop in it.  Without the flag neither
 file is written.
 
+Like render.py, both stages render without Mip-Splatting's filters, and a ply's filter_3D property is then not used.
+--kernel_size K (mip.py) builds the tracker with both filters, the 2D filter at K and the ply's filter_3D, so the
+training-view renders, the test-view tracking, the best-pose renders and the --test_fps loop all run the filtered
+forward; with --infer_video the flag is forwarded to the fly-through.  It is refused, before anything is written, for
+a K that is negative, NaN or infinite and for a ply without filter_3D (a model trained without --kernel_size).
+
 The background is black, or white with --white_background; the SH degree is the ply's.  The model's cfg_args is not
 read: render.py's get_combined_args lets every command-line value that is not None win, and ModelParams is built
 with sentinel=False, so its defaults (white_background False included) always override the saved config there too.
 
     python -m instantsplat_b200.render_views -s SOURCE -m MODEL --n_views N --iterations IT [--eval] [--infer_video]
         [--optim_test_pose_iter 500] [--white_background] [--max_batch B] [--workers K] [--png_encoder pil|gpu]
-        [--test_fps] [-r R --resample_images]
+        [--test_fps] [-r R --resample_images] [--kernel_size K]
 """
 from __future__ import annotations
 
@@ -48,7 +54,7 @@ from typing import Optional, Sequence, Tuple
 import numpy as np
 import torch
 
-from . import freeview, resample
+from . import freeview, mip, resample
 from .scene_io import Views, load_views, read_colmap_text
 from .tracking import PoseTracker
 from .train import save_time
@@ -67,11 +73,15 @@ def gt_images(views: Views, device) -> torch.Tensor:
     return (u8 / 255.0).permute(0, 3, 1, 2).contiguous()
 
 
-def tracker_for(model_path: str, it: int, views: Views, white_background: bool = False, device="cuda") -> PoseTracker:
+def tracker_for(model_path: str, it: int, views: Views, white_background: bool = False, device="cuda",
+                kernel_size: Optional[float] = None) -> PoseTracker:
+    """freeview.load_tracker of point_cloud/iteration_<it>/point_cloud.ply at the views' size and field of view;
+    kernel_size: with Mip-Splatting's filters (the ply's filter_3D)."""
     ply = os.path.join(model_path, "point_cloud", f"iteration_{it}", "point_cloud.ply")
     if not os.path.isfile(ply):
         raise FileNotFoundError(f"{ply} not found")
-    return freeview.load_tracker(ply, views.width, views.height, views.fovx, views.fovy, white_background, device)
+    return freeview.load_tracker(ply, views.width, views.height, views.fovx, views.fovy, white_background, device,
+                                 kernel_size)
 
 
 def _write_gt(views: Views, folder: str, names, workers: Optional[int], write=freeview.write_pngs) -> None:
@@ -170,6 +180,7 @@ def parser() -> argparse.ArgumentParser:
     ap.add_argument("--test_fps", action="store_true",
                     help="with --eval: time 1000 renders of the last test view and append the rate to total_fps.json")
     resample.add_arg(ap)
+    mip.add_arg(ap)
     return ap
 
 
@@ -177,21 +188,28 @@ def main(argv=None) -> int:
     a = parser().parse_args(argv)
     if a.max_batch < 1:
         raise SystemExit("--max_batch must be at least 1")
+    k = mip.kernel_size(a)
+    why = mip.kernel_refusal(k)
+    if why:
+        raise SystemExit(f"render_views: {why}")
     if a.infer_video and not a.eval:
         fv = ["-s", a.source_path, "-m", a.model_path, "--n_views", str(a.n_views), "--iterations", str(a.iterations),
               "--max_batch", str(a.max_batch)] + (["--white_background"] if a.white_background else []) \
             + ([] if a.workers is None else ["--workers", str(a.workers)]) + ["--png_encoder", a.png_encoder] \
-            + (["-r", str(a.resolution), "--resample_images"] if resample.requested(a) else [])
+            + (["-r", str(a.resolution), "--resample_images"] if resample.requested(a) else []) + mip.argv(k)
         return freeview.main(fv)
     write = freeview.png_writer(a.png_encoder)
     it = freeview.max_iteration(a.model_path) if a.iterations == -1 else a.iterations
+    why = mip.ply_refusal(k, freeview.model_files(a.model_path, it)[0])
+    if why:
+        raise SystemExit(f"render_views: {why}")
     rdev = "cuda" if resample.requested(a) else None
     if a.eval:
         why = fps_refusal(a.source_path, a.n_views) if a.test_fps else None
         if why:
             raise SystemExit(f"render_views: {why}")
         views = load_views(a.source_path, a.n_views, 1, a.resolution, resample_device=rdev)
-        tracker = tracker_for(a.model_path, it, views, a.white_background)
+        tracker = tracker_for(a.model_path, it, views, a.white_background, kernel_size=k)
         out = os.path.join(a.model_path, "test", f"ours_{it}")
         start = time.time()
         best = render_test(tracker, views, out, a.optim_test_pose_iter, a.max_batch, a.workers, write)
@@ -202,7 +220,7 @@ def main(argv=None) -> int:
         if not os.path.isfile(npy):
             raise FileNotFoundError(f"{npy} not found")
         views = load_views(a.source_path, a.n_views, 0, a.resolution, resample_device=rdev)
-        tracker = tracker_for(a.model_path, it, views, a.white_background)
+        tracker = tracker_for(a.model_path, it, views, a.white_background, kernel_size=k)
         out = os.path.join(a.model_path, "train", f"ours_{it}")
         render_train(tracker, views, np.load(npy), out, a.max_batch, a.workers, write)
     print(f"{len(views)} views -> {out}")

@@ -321,25 +321,36 @@ def _write_ply(path: str, fields: List[Tuple[str, str]], columns: List[np.ndarra
         f.write(arr.tobytes())
 
 
+def _read_ply_header(f) -> Tuple[int, List[Tuple[str, str]]]:
+    if f.readline().strip() != b"ply":
+        raise ValueError("not a PLY file")
+    fmt = f.readline().split()
+    if fmt[1] != b"binary_little_endian":
+        raise ValueError("only binary_little_endian PLY is supported")
+    n, fields = None, []
+    while True:
+        line = f.readline().strip()
+        if line == b"end_header":
+            break
+        tok = line.split()
+        if tok[:2] == [b"element", b"vertex"]:
+            n = int(tok[2])
+        elif tok[0] == b"property":
+            fields.append((tok[2].decode(), "<" + _PLY_REV[tok[1].decode()]))
+    return n, fields
+
+
 def _read_ply(path: str) -> np.ndarray:
     with open(path, "rb") as f:
-        if f.readline().strip() != b"ply":
-            raise ValueError("not a PLY file")
-        fmt = f.readline().split()
-        if fmt[1] != b"binary_little_endian":
-            raise ValueError("only binary_little_endian PLY is supported")
-        n, fields = None, []
-        while True:
-            line = f.readline().strip()
-            if line == b"end_header":
-                break
-            tok = line.split()
-            if tok[:2] == [b"element", b"vertex"]:
-                n = int(tok[2])
-            elif tok[0] == b"property":
-                fields.append((tok[2].decode(), "<" + _PLY_REV[tok[1].decode()]))
+        n, fields = _read_ply_header(f)
         data = np.frombuffer(f.read(n * np.dtype(fields).itemsize), dtype=np.dtype(fields), count=n)
     return data
+
+
+def ply_properties(path: str) -> List[str]:
+    """The vertex property names of a PLY file, in file order, from its header alone."""
+    with open(path, "rb") as f:
+        return [name for name, _ in _read_ply_header(f)[1]]
 
 
 def write_points3d_ply(path: str, xyz: np.ndarray, rgb_u8: np.ndarray, normals: np.ndarray = None) -> None:

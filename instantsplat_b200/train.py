@@ -25,6 +25,12 @@ confidence_dsp.npy.
 --resample_images (not one of train.py's flags, and not part of cfg_args) resizes the training images to loadCam's
 size on the GPU, Pillow's bicubic resize byte for byte (resample.py), and trains at that size; cameras.json and the
 view-depth scale cap keep the decoded size, as train.py's CameraInfo does.
+
+--kernel_size K (Mip-Splatting, not one of train.py's flags, and not part of cfg_args; mip.py) trains with both
+Mip-Splatting filters, OptimConfig.mip_kernel_size = K: the 3D filter is computed when the trainer is built (or
+restored from --start_checkpoint) and recomputed every mip_filter3d_interval iterations except in the last 100,
+point_cloud.ply gets the filter_3D property, checkpoints carry the filter, and the `Evaluating train` line renders with
+the filters.  A K that is negative, NaN or infinite is refused.  Without the flag no filter is used.
 """
 from __future__ import annotations
 
@@ -42,7 +48,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 import torch
 
-from . import freeview, resample
+from . import freeview, mip, resample
 from .scene_io import Views, load_views, read_points3d_ply
 
 # ---- train.py's command line: arguments/__init__.py:47-94 and train.py:299-312 --------------------------------------
@@ -90,6 +96,7 @@ def parser() -> argparse.ArgumentParser:
     ap.add_argument("--checkpoint_iterations", nargs="+", type=int, default=[])
     ap.add_argument("--start_checkpoint", type=str, default=None)
     resample.add_arg(ap)
+    mip.add_arg(ap)
     return ap
 
 
@@ -116,6 +123,9 @@ def refusals(args: argparse.Namespace) -> List[str]:
                    "would change the ply and checkpoint shapes")
     if args.start_checkpoint is not None and not os.path.isfile(args.start_checkpoint):
         out.append(f"--start_checkpoint: {args.start_checkpoint} not found")
+    why = mip.kernel_refusal(mip.kernel_size(args))
+    if why:
+        out.append(why)
     return out
 
 
@@ -307,13 +317,17 @@ def save_time(model_path: str, name: str, seconds: float) -> None:
 
 def optim_config(args: argparse.Namespace, extent: float):
     """JointTrainer's OptimConfig from the command line: the OptimizationParams fields the loop reads (train.py's
-    defaults, so pp_optimizer and optim_pose are off unless given), spatial_lr_scale = the extent, max_sh_degree."""
+    defaults, so pp_optimizer and optim_pose are off unless given), spatial_lr_scale = the extent, max_sh_degree, and
+    mip_kernel_size = --kernel_size when it is given."""
     from .trainer import OptimConfig
     c = OptimConfig()
     for k in LOOP_FIELDS:
         setattr(c, k, getattr(args, k))
     c.spatial_lr_scale = float(extent)
     c.max_sh_degree = int(args.sh_degree)
+    k = mip.kernel_size(args)
+    if k is not None:
+        c.mip_kernel_size = k
     return c
 
 
