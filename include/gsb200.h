@@ -361,6 +361,32 @@ GSB_API int gsb_resample_u8_batch(int32_t V, int32_t H, int32_t W, int32_t Ho, i
                                   const int32_t* y_bounds, const int32_t* y_coefs, int32_t y_ksize, void* scratch,
                                   size_t scratch_bytes, gsb_stream_t stream);
 
+/* ---- point_cloud.ply vertex records (GaussianModel.save_ply / load_ply, scene/gaussian_model.py:261-278, 285-;
+ * DESIGN.md 4.23) ----
+ * A record is R <= GSB_PLY_MAX_FLOATS 32-bit words, filled column by column by up to GSB_PLY_MAX_SEGMENTS segments in
+ * record order.  Segment s is a [P, width] array of 32-bit words (row p at data + p * width); its row, read as
+ * [width / inner, inner], is stored transposed: element (r, k) at record column col_s + k * (width / inner) + r, col_s
+ * the sum of the earlier segments' widths.  inner == width keeps the row as it is; f_rest [P, M-1, 3] takes inner 3
+ * (construct_list_of_attributes' channel-major f_rest_*, transpose(1, 2).flatten(1)).  Words are copied, never
+ * converted (NaN payloads, -0 and denormals survive), and offsets are 64-bit.  The record buffer is device memory or
+ * pinned host memory the device can reach, 4-byte aligned (any 16-byte phase); segment data 4-byte aligned.  Width
+ * and inner >= 1 with inner dividing width, R <= GSB_PLY_MAX_FLOATS, P >= 0 (0: nothing launched); else
+ * GSB_ERR_INVALID. */
+#define GSB_PLY_MAX_SEGMENTS 8
+#define GSB_PLY_MAX_FLOATS 64
+typedef struct GsbPlySegment {
+  void* data;     /* pack: read, NULL for zeros (the normals); unpack: written, NULL to skip the columns */
+  int32_t width;  /* words per record */
+  int32_t inner;  /* the row's minor extent, made major in the record */
+} GsbPlySegment;
+/* Replaces save_ply's np.concatenate of the attributes and the structured array PlyData writes: P records, P * R * 4
+ * bytes, into out. */
+GSB_API int gsb_ply_pack(int64_t P, int32_t n_segments, const GsbPlySegment* segments, void* out,
+                         gsb_stream_t stream);
+/* Replaces load_ply's per-property np.asarray columns: P records from in into the segments' arrays. */
+GSB_API int gsb_ply_unpack(int64_t P, const void* in, int32_t n_segments, const GsbPlySegment* segments,
+                           gsb_stream_t stream);
+
 /* ---- LPIPS, VGG16 v0.1(metrics.py:69 lpips(render, gt, net_type='vgg'); lpipsPyTorch/modules/lpips.py,
  * networks.py BaseNet / VGG16, utils.py normalize_activation).  DESIGN.md 4.15.  fp32 FFMA, NHWC activations, every
  * sum in one fixed order: an image's values are bit-identical from run to run and whatever else is in the batch.

@@ -62,6 +62,13 @@ class GsbAdamTensor(ctypes.Structure):
                 ("eps", ctypes.c_double), ("weight_decay", ctypes.c_double)]
 
 
+class GsbPlySegment(ctypes.Structure):
+    _fields_ = [("data", ctypes.c_void_p), ("width", ctypes.c_int32), ("inner", ctypes.c_int32)]
+
+
+PLY_MAX_SEGMENTS = 8
+
+
 class GsbShardPiece(ctypes.Structure):
     _fields_ = [("begin", ctypes.c_int64), ("end", ctypes.c_int64), ("seg_begin", ctypes.c_int64),
                 ("per_point_lr", ctypes.c_void_p), ("row_len", ctypes.c_int32), ("flag_index", ctypes.c_int32),
@@ -83,7 +90,8 @@ EXPORTS = ("gsb_geom_bytes", "gsb_binning_bytes", "gsb_image_bytes", "gsb_prepro
            "gsb_backward_batch_stats", "gsb_image_metrics_scratch_bytes", "gsb_image_metrics_batch",
            "gsb_frames_u8_batch", "gsb_lpips_scratch_bytes", "gsb_lpips_prepare", "gsb_lpips_conv3x3_relu",
            "gsb_lpips_maxpool2", "gsb_lpips_head", "gsb_render_batch_bg", "gsb_backward_batch_stats_bg",
-           "gsb_png_bound", "gsb_png_scratch_bytes", "gsb_png_encode_batch", "gsb_resample_u8_batch")
+           "gsb_png_bound", "gsb_png_scratch_bytes", "gsb_png_encode_batch", "gsb_resample_u8_batch",
+           "gsb_ply_pack", "gsb_ply_unpack")
 KERNEL_IDS = ("preprocess", "sort_depth", "scan", "duplicate", "sort_tile", "gather", "blend_fwd", "blend_bwd",
               "preprocess_bwd", "loss_fwd", "loss_bwd", "adam")
 
@@ -186,11 +194,14 @@ def lib() -> ctypes.CDLL:
     L.gsb_png_scratch_bytes.argtypes = [i32, i32, i32]
     L.gsb_png_encode_batch.argtypes = [i32, i32, i32, vp, vp, sz, vp, vp, vp]
     L.gsb_resample_u8_batch.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, i32, vp, vp, i32, vp, sz, vp]
+    L.gsb_ply_pack.argtypes = [i64, i32, ctypes.POINTER(GsbPlySegment), vp, vp]
+    L.gsb_ply_unpack.argtypes = [i64, vp, i32, ctypes.POINTER(GsbPlySegment), vp]
     for f in ("gsb_preprocess_batch", "gsb_render_batch", "gsb_backward_pose_batch", "gsb_l1_mask_fwd_bwd_batch",
               "gsb_track_step_batch", "gsb_backward_batch", "gsb_loss_forward_batch", "gsb_loss_backward_batch",
               "gsb_backward_batch_stats", "gsb_image_metrics_batch", "gsb_frames_u8_batch", "gsb_lpips_prepare",
               "gsb_lpips_conv3x3_relu", "gsb_lpips_maxpool2", "gsb_lpips_head", "gsb_render_batch_bg",
-              "gsb_backward_batch_stats_bg", "gsb_png_encode_batch", "gsb_resample_u8_batch"):
+              "gsb_backward_batch_stats_bg", "gsb_png_encode_batch", "gsb_resample_u8_batch", "gsb_ply_pack",
+              "gsb_ply_unpack"):
         getattr(L, f).restype = ctypes.c_int
     L.gsb_adam_step_gated.argtypes = [i32, ctypes.POINTER(GsbAdamTensor), vp, vp, vp]
     L.gsb_adam_step_gated.restype = ctypes.c_int

@@ -33,8 +33,11 @@ used.  --kernel_size K (mip.py) renders every frame with both filters: the 2D fi
 It is refused, before anything is written, for a K that is negative, NaN or infinite and for a ply without filter_3D
 (a model trained without --kernel_size).
 
+--ply_io gpu (ply.py) reads point_cloud.ply on the GPU: the records unpacked by one kernel into the tracker's device
+tensors, the same values as without it (a file not in save_gaussians_ply's exact layout is read the numpy way).
+
     python -m instantsplat_b200.freeview -s SOURCE -m MODEL --n_views N --iterations IT [--white_background]
-        [--png_encoder pil|gpu] [-r R --resample_images] [--kernel_size K]
+        [--png_encoder pil|gpu] [-r R --resample_images] [--kernel_size K] [--ply_io numpy|gpu]
 """
 from __future__ import annotations
 
@@ -48,7 +51,7 @@ from typing import Iterable, Iterator, Optional, Sequence, Tuple
 import numpy as np
 import torch
 
-from . import _lib, mip, png, resample
+from . import _lib, mip, ply, png, resample
 from ._lib import check
 from .frame import ST_OVERFLOW
 from .tracking import PoseTracker
@@ -315,29 +318,36 @@ def model_files(model_path: str, iteration: int = -1) -> Tuple[str, str, int]:
 
 
 def load(source_path: str, model_path: str, n_views: int, iteration: int = -1, white_background: bool = False,
-         device="cuda", resolution: int = 1, resample_images: bool = False, kernel_size: Optional[float] = None):
+         device="cuda", resolution: int = 1, resample_images: bool = False, kernel_size: Optional[float] = None,
+         ply_io: str = "numpy"):
     """What render.py loads for the fly-through: (tracker over model_files' ply, key poses from its
     pose_optimized.npy, it).  Like render.py, no Mip-Splatting filters unless kernel_size is given; then the tracker
     applies the 2D filter with it and the ply's filter_3D (load_tracker).  The tracker renders at
-    frame_size(resolution, resample_images)."""
+    frame_size(resolution, resample_images); ply_io: load_tracker's."""
     ply, npy, it = model_files(model_path, iteration)
     for f in (ply, npy):
         if not os.path.isfile(f):
             raise FileNotFoundError(f"{f} not found")
     _, _, fovx, fovy = intrinsics(source_path, n_views)
     W, H = frame_size(source_path, n_views, resolution, resample_images)
-    return load_tracker(ply, W, H, fovx, fovy, white_background, device, kernel_size), np.load(npy), it
+    return load_tracker(ply, W, H, fovx, fovy, white_background, device, kernel_size, ply_io), np.load(npy), it
 
 
-def load_tracker(ply: str, width: int, height: int, fovx: float, fovy: float, white_background: bool = False,
-                 device="cuda", kernel_size: Optional[float] = None) -> PoseTracker:
+def load_tracker(path: str, width: int, height: int, fovx: float, fovy: float, white_background: bool = False,
+                 device="cuda", kernel_size: Optional[float] = None, ply_io: str = "numpy") -> PoseTracker:
     """A PoseTracker over a saved point_cloud.ply as render.py renders it: the SH degree from the file's coefficient
     count, a black or white background.  No Mip-Splatting filters unless kernel_size is given (a filter_3D property
     in the file is then not used); with it, the 2D filter at kernel_size and the file's filter_3D, which it must
-    carry (tracker_from_gaussians)."""
+    carry (tracker_from_gaussians).  ply_io "numpy": scene_io.load_gaussians_ply; "gpu": ply.load, the tensors
+    unpacked on the device (the same values)."""
     from .scene_io import load_gaussians_ply
-    g = {k: torch.from_numpy(np.ascontiguousarray(a)) for k, a in load_gaussians_ply(ply).items()}
-    return tracker_from_gaussians(g, width, height, fovx, fovy, white_background, device, ply, kernel_size)
+    if ply_io == "gpu":
+        g = ply.load(path, device)
+    elif ply_io == "numpy":
+        g = {k: torch.from_numpy(np.ascontiguousarray(a)) for k, a in load_gaussians_ply(path).items()}
+    else:
+        raise ValueError(f"load_tracker: ply_io must be 'numpy' or 'gpu', got {ply_io!r}")
+    return tracker_from_gaussians(g, width, height, fovx, fovy, white_background, device, path, kernel_size)
 
 
 def tracker_from_gaussians(g, width: int, height: int, fovx: float, fovy: float, white_background: bool = False,
@@ -380,6 +390,7 @@ def main(argv=None) -> int:
                          "it changes the size)")
     resample.add_arg(ap)
     mip.add_arg(ap)
+    ply.add_arg(ap)
     a = ap.parse_args(argv)
     if a.n_views < 2:
         raise SystemExit("--n_views must be at least 2: the fly-through joins consecutive key poses")
@@ -389,7 +400,8 @@ def main(argv=None) -> int:
         if why:
             raise SystemExit(f"freeview: {why}")
     tracker, keys, it = load(a.source_path, a.model_path, a.n_views, a.iterations, a.white_background, "cuda",
-                             a.resolution, resample.requested(a), **({} if k is None else {"kernel_size": k}))
+                             a.resolution, resample.requested(a), **({} if k is None else {"kernel_size": k}),
+                             **ply.kwargs(a))
     n, folder = fly_through(tracker, keys, it, a.model_path, a.n_views, a.max_batch, a.workers,
                             png_writer(a.png_encoder))
     print(f"{n} frames -> {folder}")

@@ -3,9 +3,9 @@ on one GPU (DESIGN.md section 4.18).
 
     python -m instantsplat_b200.pipeline eval  --data_root ROOT --output_dir OUT --datasets D.. --scenes S..
         --n_views N.. --iterations IT.. [--lpips_weights DIR] [--workers W] [--png_encoder pil|gpu] [--test_fps]
-        [--kernel_size K]
+        [--kernel_size K] [--ply_io numpy|gpu]
     python -m instantsplat_b200.pipeline infer --data_root ROOT --output_dir OUT --datasets D.. --scenes S..
-        --n_views N.. --iterations IT.. [--workers W] [--png_encoder pil|gpu] [--kernel_size K]
+        --n_views N.. --iterations IT.. [--workers W] [--png_encoder pil|gpu] [--kernel_size K] [--ply_io numpy|gpu]
 
 Tasks run in the scripts' loop order (dataset, scene, n_views, iterations), one after another.  The source is
 ROOT/D/S/24_views for eval and ROOT/D/S for infer; the model is OUT/D/S/<N>_views.  Each stage is the stage module's
@@ -27,6 +27,9 @@ train, render and fly-through lines carry --kernel_size K (metrics scores PNGs a
 with both filters, and its filter_3D goes to the trackers with the rest of ply_tensors.  A K that is negative, NaN or
 infinite is refused with the other refusals.
 
+--ply_io gpu goes on the train stage's line only: its save points write point_cloud.ply on the GPU (ply.py).  The
+render stages get the model in memory and read no ply.
+
 Every PNG goes to one process-wide encoder pool (PngWriter) that the GPU stages do not wait for, up to a bound on the
 frames queued; with --png_encoder gpu the frames are encoded on the GPU and the pool only writes the files.  Every
 task is checked before anything is written (refusals).  The scripts' nvidia-smi GPU picker and init_geo (stage 1) are
@@ -47,7 +50,7 @@ from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from . import freeview, metrics, mip, png, render_views, train
+from . import freeview, metrics, mip, ply, png, render_views, train
 from .scene_io import load_views, pose_matrices
 
 # stage -> (log file, the script's start line, its completion line)
@@ -91,12 +94,13 @@ def tasks(mode: str, data_root: str, output_dir: str, datasets: Sequence[str], s
 
 
 def stage_argv(t: Task, lpips_weights: Optional[str] = None, test_fps: bool = False,
-               kernel_size: Optional[float] = None) -> Dict[str, List[str]]:
+               kernel_size: Optional[float] = None, ply_io: Optional[str] = None) -> Dict[str, List[str]]:
     """Each stage's command line as the script writes it; test_fps adds --test_fps to the test-view renders';
-    kernel_size adds --kernel_size to the train, render and fly-through lines (not to metrics, which scores PNGs)."""
+    kernel_size adds --kernel_size to the train, render and fly-through lines (not to metrics, which scores PNGs);
+    ply_io adds --ply_io to the train line."""
     base = ["-s", t.source, "-m", t.model, "-r", "1", "--n_views", str(t.n_views), "--iterations", str(t.iterations)]
     k = mip.argv(kernel_size)
-    out = {"train": base + ["--pp_optimizer", "--optim_pose"] + k}
+    out = {"train": base + ["--pp_optimizer", "--optim_pose"] + k + ply.argv(ply_io)}
     if t.mode == "eval":
         out["render_train"] = base + k
         out["render_test"] = base + ["--eval"] + (["--test_fps"] if test_fps else []) + k
@@ -108,11 +112,11 @@ def stage_argv(t: Task, lpips_weights: Optional[str] = None, test_fps: bool = Fa
 
 
 def stage_args(t: Task, lpips_weights: Optional[str] = None, test_fps: bool = False,
-               kernel_size: Optional[float] = None) -> Dict[str, argparse.Namespace]:
+               kernel_size: Optional[float] = None, ply_io: Optional[str] = None) -> Dict[str, argparse.Namespace]:
     """stage_argv parsed by each stage's own parser."""
     parse = {"train": train.parse_args, "metrics": lambda a: metrics.parser().parse_args(a)}
     return {k: parse.get(k, lambda a: render_views.parser().parse_args(a))(v)
-            for k, v in stage_argv(t, lpips_weights, test_fps, kernel_size).items()}
+            for k, v in stage_argv(t, lpips_weights, test_fps, kernel_size, ply_io).items()}
 
 
 def refusals(t: Task, test_fps: bool = False, kernel_size: Optional[float] = None) -> List[str]:
@@ -235,11 +239,13 @@ def _stage(t: Task, key: str, times: Dict[str, float]):
 
 
 def run_task(t: Task, pool: PngWriter, lpips_net=None, lpips_weights: Optional[str] = None,
-             device="cuda", test_fps: bool = False, kernel_size: Optional[float] = None) -> Tuple[int, Dict[str, float]]:
+             device="cuda", test_fps: bool = False, kernel_size: Optional[float] = None,
+             ply_io: Optional[str] = None) -> Tuple[int, Dict[str, float]]:
     """The script's run_on_gpu from stage 2 on, with test_fps: stage 4 with --test_fps; kernel_size: every stage but
-    metrics with --kernel_size (the trainer's filter_3D handed to the trackers).  Returns (model directories metrics
-    could not evaluate, wall seconds per stage).  The trainer and trackers are released before it returns."""
-    a = stage_args(t, lpips_weights, test_fps, kernel_size)
+    metrics with --kernel_size (the trainer's filter_3D handed to the trackers); ply_io: the train stage with
+    --ply_io.  Returns (model directories metrics could not evaluate, wall seconds per stage).  The trainer and
+    trackers are released before it returns."""
+    a = stage_args(t, lpips_weights, test_fps, kernel_size, ply_io)
     times, failed = {}, 0
     print("=" * 55)
     print(f"Starting process: {t.label}")
@@ -308,16 +314,16 @@ def run_task(t: Task, pool: PngWriter, lpips_net=None, lpips_weights: Optional[s
 
 def run_tasks(ts: Sequence[Task], workers: Optional[int] = None, lpips_net=None, lpips_weights: Optional[str] = None,
               device="cuda", png_encoder: str = "pil", test_fps: bool = False,
-              kernel_size: Optional[float] = None) -> Tuple[int, List[Dict[str, float]]]:
-    """Every task in order on one encoder pool (PngWriter with png_encoder), then every write waited for; test_fps
-    and kernel_size: run_task's.  Returns (model directories metrics could not evaluate, per-task stage times).  Raises WriteError
+              kernel_size: Optional[float] = None, ply_io: Optional[str] = None) -> Tuple[int, List[Dict[str, float]]]:
+    """Every task in order on one encoder pool (PngWriter with png_encoder), then every write waited for; test_fps,
+    kernel_size and ply_io: run_task's.  Returns (model directories metrics could not evaluate, per-task stage times).  Raises WriteError
     when a PNG could not be written."""
     pool = PngWriter(workers, png_encoder)
     failed, times = 0, []
     try:
         for k, t in enumerate(ts, 1):
             print(f"Processing task {k} / {len(ts)}", flush=True)
-            f, s = run_task(t, pool, lpips_net, lpips_weights, device, test_fps, kernel_size)
+            f, s = run_task(t, pool, lpips_net, lpips_weights, device, test_fps, kernel_size, ply_io)
             failed += f
             times.append(s)
     finally:
@@ -348,6 +354,7 @@ def parser() -> argparse.ArgumentParser:
                                                                   "to 8)")
         freeview.add_png_encoder_arg(p)
         mip.add_arg(p)
+        ply.add_arg(p)
     return ap
 
 
@@ -371,7 +378,7 @@ def main(argv=None) -> int:
             ap.error(str(e))
     try:
         failed, _ = run_tasks(ts, a.workers, net, weights, png_encoder=a.png_encoder, test_fps=test_fps,
-                              kernel_size=k)
+                              kernel_size=k, ply_io=ply.io(a))
     except WriteError as e:
         raise SystemExit(f"instantsplat_b200.pipeline: {e}")
     print("=" * 55)

@@ -40,7 +40,10 @@ with sentinel=False, so its defaults (white_background False included) always ov
 
     python -m instantsplat_b200.render_views -s SOURCE -m MODEL --n_views N --iterations IT [--eval] [--infer_video]
         [--optim_test_pose_iter 500] [--white_background] [--max_batch B] [--workers K] [--png_encoder pil|gpu]
-        [--test_fps] [-r R --resample_images] [--kernel_size K]
+        [--test_fps] [-r R --resample_images] [--kernel_size K] [--ply_io numpy|gpu]
+
+--ply_io gpu reads point_cloud.ply on the GPU (ply.py), for the stage here or the fly-through it hands over to; the
+renders are the same as without it.
 """
 from __future__ import annotations
 
@@ -54,7 +57,7 @@ from typing import Optional, Sequence, Tuple
 import numpy as np
 import torch
 
-from . import freeview, mip, resample
+from . import freeview, mip, ply, resample
 from .scene_io import Views, load_views, read_colmap_text
 from .tracking import PoseTracker
 from .train import save_time
@@ -74,14 +77,14 @@ def gt_images(views: Views, device) -> torch.Tensor:
 
 
 def tracker_for(model_path: str, it: int, views: Views, white_background: bool = False, device="cuda",
-                kernel_size: Optional[float] = None) -> PoseTracker:
+                kernel_size: Optional[float] = None, ply_io: str = "numpy") -> PoseTracker:
     """freeview.load_tracker of point_cloud/iteration_<it>/point_cloud.ply at the views' size and field of view;
-    kernel_size: with Mip-Splatting's filters (the ply's filter_3D)."""
+    kernel_size: with Mip-Splatting's filters (the ply's filter_3D); ply_io: read it the numpy way or on the GPU."""
     ply = os.path.join(model_path, "point_cloud", f"iteration_{it}", "point_cloud.ply")
     if not os.path.isfile(ply):
         raise FileNotFoundError(f"{ply} not found")
     return freeview.load_tracker(ply, views.width, views.height, views.fovx, views.fovy, white_background, device,
-                                 kernel_size)
+                                 kernel_size, ply_io)
 
 
 def _write_gt(views: Views, folder: str, names, workers: Optional[int], write=freeview.write_pngs) -> None:
@@ -181,6 +184,7 @@ def parser() -> argparse.ArgumentParser:
                     help="with --eval: time 1000 renders of the last test view and append the rate to total_fps.json")
     resample.add_arg(ap)
     mip.add_arg(ap)
+    ply.add_arg(ap)
     return ap
 
 
@@ -196,7 +200,7 @@ def main(argv=None) -> int:
         fv = ["-s", a.source_path, "-m", a.model_path, "--n_views", str(a.n_views), "--iterations", str(a.iterations),
               "--max_batch", str(a.max_batch)] + (["--white_background"] if a.white_background else []) \
             + ([] if a.workers is None else ["--workers", str(a.workers)]) + ["--png_encoder", a.png_encoder] \
-            + (["-r", str(a.resolution), "--resample_images"] if resample.requested(a) else []) + mip.argv(k)
+            + ply.argv(ply.io(a)) + (["-r", str(a.resolution), "--resample_images"] if resample.requested(a) else []) + mip.argv(k)
         return freeview.main(fv)
     write = freeview.png_writer(a.png_encoder)
     it = freeview.max_iteration(a.model_path) if a.iterations == -1 else a.iterations
@@ -209,7 +213,7 @@ def main(argv=None) -> int:
         if why:
             raise SystemExit(f"render_views: {why}")
         views = load_views(a.source_path, a.n_views, 1, a.resolution, resample_device=rdev)
-        tracker = tracker_for(a.model_path, it, views, a.white_background, kernel_size=k)
+        tracker = tracker_for(a.model_path, it, views, a.white_background, kernel_size=k, **ply.kwargs(a))
         out = os.path.join(a.model_path, "test", f"ours_{it}")
         start = time.time()
         best = render_test(tracker, views, out, a.optim_test_pose_iter, a.max_batch, a.workers, write)
@@ -220,7 +224,7 @@ def main(argv=None) -> int:
         if not os.path.isfile(npy):
             raise FileNotFoundError(f"{npy} not found")
         views = load_views(a.source_path, a.n_views, 0, a.resolution, resample_device=rdev)
-        tracker = tracker_for(a.model_path, it, views, a.white_background, kernel_size=k)
+        tracker = tracker_for(a.model_path, it, views, a.white_background, kernel_size=k, **ply.kwargs(a))
         out = os.path.join(a.model_path, "train", f"ours_{it}")
         render_train(tracker, views, np.load(npy), out, a.max_batch, a.workers, write)
     print(f"{len(views)} views -> {out}")

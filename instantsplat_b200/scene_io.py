@@ -306,6 +306,14 @@ _PLY_REV = {"float": "f4", "float32": "f4", "uchar": "u1", "uint8": "u1", "doubl
             "int": "i4", "int32": "i4"}
 
 
+def _ply_header(n: int, fields: List[Tuple[str, str]]) -> bytes:
+    """The header _write_ply writes for n vertices with these (name, numpy type) properties."""
+    hdr = ["ply", "format binary_little_endian 1.0", f"element vertex {n}"]
+    hdr += [f"property {_PLY_TYPES[t]} {name}" for name, t in fields]
+    hdr.append("end_header")
+    return ("\n".join(hdr) + "\n").encode("ascii")
+
+
 def _write_ply(path: str, fields: List[Tuple[str, str]], columns: List[np.ndarray]) -> None:
     n = columns[0].shape[0]
     dt = np.dtype([(name, "<" + t) for name, t in fields])
@@ -314,10 +322,7 @@ def _write_ply(path: str, fields: List[Tuple[str, str]], columns: List[np.ndarra
         arr[name] = col
     os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
     with open(path, "wb") as f:
-        hdr = ["ply", "format binary_little_endian 1.0", f"element vertex {n}"]
-        hdr += [f"property {_PLY_TYPES[t]} {name}" for name, t in fields]
-        hdr.append("end_header")
-        f.write(("\n".join(hdr) + "\n").encode("ascii"))
+        f.write(_ply_header(n, fields))
         f.write(arr.tobytes())
 
 
@@ -376,14 +381,25 @@ def gaussian_ply_fields(n_rest: int = 45) -> List[str]:
             + ["opacity"] + [f"scale_{i}" for i in range(3)] + [f"rot_{i}" for i in range(4)])
 
 
+def gaussian_ply_header(P: int, n_rest: int, filter_3D: bool) -> bytes:
+    """The header save_gaussians_ply writes for P Gaussians with n_rest f_rest_* properties, with or without
+    filter_3D."""
+    names = gaussian_ply_fields(n_rest) + (["filter_3D"] if filter_3D else [])
+    return _ply_header(P, [(n, "f4") for n in names])
+
+
 def save_gaussians_ply(path: str, xyz, f_dc, f_rest, opacity, scaling, rotation, filter_3D=None) -> None:
     """Model tensors -> point_cloud.ply; f_dc [P,1,3], f_rest [P,M-1,3] are stored channel-major
     (transpose(1,2).flatten(1)), raw (un-activated) opacity / scaling / rotation, zero normals.  filter_3D [P] or
     [P,1] (Mip-Splatting's 3D smoothing filter), when given, is the last property, as Mip-Splatting stores it."""
     xyz = np.asarray(xyz, np.float32)
     P = xyz.shape[0]
-    dc = np.asarray(f_dc, np.float32).reshape(P, -1, 3).transpose(0, 2, 1).reshape(P, -1)
-    rest = np.asarray(f_rest, np.float32).reshape(P, -1, 3).transpose(0, 2, 1).reshape(P, -1)
+
+    def channel_major(a):
+        a = np.asarray(a, np.float32)
+        k = a.size // P if P else int(np.prod(a.shape[1:]))      # an empty model keeps its width from the shape
+        return a.reshape(P, k // 3, 3).transpose(0, 2, 1).reshape(P, k)
+    dc, rest = channel_major(f_dc), channel_major(f_rest)
     attrs = np.concatenate([xyz, np.zeros_like(xyz), dc, rest, np.asarray(opacity, np.float32).reshape(P, 1),
                             np.asarray(scaling, np.float32).reshape(P, 3), np.asarray(rotation, np.float32).reshape(P, 4)],
                            axis=1)

@@ -31,6 +31,9 @@ Mip-Splatting filters, OptimConfig.mip_kernel_size = K: the 3D filter is compute
 restored from --start_checkpoint) and recomputed every mip_filter3d_interval iterations except in the last 100,
 point_cloud.ply gets the filter_3D property, checkpoints carry the filter, and the `Evaluating train` line renders with
 the filters.  A K that is negative, NaN or infinite is refused.  Without the flag no filter is used.
+
+--ply_io gpu (not one of train.py's flags, and not part of cfg_args; ply.py) writes point_cloud.ply at the save points
+with JointTrainer.save_ply(io="gpu"): the records packed from the flat buffers on the GPU, the same bytes as without it.
 """
 from __future__ import annotations
 
@@ -48,7 +51,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 import torch
 
-from . import freeview, mip, resample
+from . import freeview, mip, ply, resample
 from .scene_io import Views, load_views, read_points3d_ply
 
 # ---- train.py's command line: arguments/__init__.py:47-94 and train.py:299-312 --------------------------------------
@@ -97,6 +100,7 @@ def parser() -> argparse.ArgumentParser:
     ap.add_argument("--start_checkpoint", type=str, default=None)
     resample.add_arg(ap)
     mip.add_arg(ap)
+    ply.add_arg(ap)
     return ap
 
 
@@ -437,7 +441,7 @@ def run(args: argparse.Namespace, device="cuda", log=print) -> RunResult:
         ts0 = time.perf_counter()
         if it in args.save_iterations:
             say(f"\n[ITER {it}] Saving Gaussians")
-            tr.save_ply(os.path.join(mp, "point_cloud", f"iteration_{it}", "point_cloud.ply"))
+            tr.save_ply(os.path.join(mp, "point_cloud", f"iteration_{it}", "point_cloud.ply"), ply.io(args) or "numpy")
             tr.save_poses(os.path.join(mp, "pose", f"ours_{it}", "pose_optimized.npy"), ids)
         if it in args.checkpoint_iterations:
             say(f"\n[ITER {it}] Saving Checkpoint")

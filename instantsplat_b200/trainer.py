@@ -1259,8 +1259,17 @@ class JointTrainer:
             else:
                 self.background_generator.manual_seed(int(self.cfg.background_seed))
 
-    def save_ply(self, path: str) -> None:
-        """scene.save: point_cloud.ply of the current Gaussians (with the filter_3D property when Mip is on)."""
+    def save_ply(self, path: str, io: str = "numpy") -> None:
+        """scene.save: point_cloud.ply of the current Gaussians (with the filter_3D property when Mip is on).  io
+        "numpy": scene_io.save_gaussians_ply of host copies; "gpu": ply.save, records packed straight from the flat
+        buffers on the device (the same bytes)."""
+        if io == "gpu":
+            from . import ply
+            t = {name: self.view(self.params, name) for name, _ in self.widths}
+            ply.save(path, dict(t, filter_3D=self.filter_3D))
+            return
+        if io != "numpy":
+            raise ValueError(f"save_ply: io must be 'numpy' or 'gpu', got {io!r}")
         from .scene_io import save_gaussians_ply
         v = lambda name: self.view(self.params, name).cpu().numpy()
         save_gaussians_ply(path, v("xyz"), v("f_dc"), v("f_rest"), v("opacity"), v("scaling"), v("rotation"),
