@@ -416,6 +416,20 @@ GS_HD float cull_threshold(float opacity) {
   return q * 1.0005f + 0.01f;
 }
 
+// Rounding margin of the culls.  q is evaluated in fp32 twice: by the cull at an edge minimiser m, and by the blend at
+// every pixel p (pair_eval).  Both sums cancel: on a long needle each of A dx^2, 2B dx dy, C dy^2 is up to ~1e7 q.
+// With s = |A dx^2| + |2B dx dy| + |C dy^2| and u = 2^-24 (first order, fused or not):
+//  - the cull: each term takes 3 roundings and 2 rounded inputs (ex = rx0 - x, dy clamped to ry0 - y), the sum 2 more:
+//    |fl(q_m) - q_m| <= 7u s_m.  The minimiser's error delta (fast division) costs C delta^2 <= 9u^2 s_m.
+//  - the blend: dx = x - px rounded, 3 roundings per term, 2 in the sum: |fl(q_p) - q_p| <= 6u s_p.  N(d) = A dx^2 +
+//    C dy^2 is a squared norm with N <= s <= 2N (|2B dx dy| <= A dx^2 + C dy^2), and p lies within 15 px of m in each
+//    axis, so sqrt(N(p)) <= sqrt(N(m)) + 15 sqrt(A + C) and s_p <= 4 s_m + 900 (A + C).
+// A pixel the blend accepts has exact q_p <= qthr_exact + 6u s_p, and q_m <= q_p; the cull keeps it when it rejects only
+// if fl(q_m) - gamma s_m > qthr with gamma >= 7u + 24u.  The rest, 5400u (A + C) <= 4.7e-3 (A + C <= 14.4 in the log2
+// domain with the 2-D low-pass >= 0.1 px^2), is inside cull_threshold's + 0.01 (0.0072 in the log2 domain).
+// gamma = 32u.  Measured: the long needles and degenerate conics of tests/test_cull_edges_cpu.py lose tiles without it.
+constexpr float kCullGamma = 1.9073486328125e-06f;   // 2^-19 = 32 u
+
 GS_HD bool rect_may_contribute(float x, float y, float A, float B, float C, float qthr,
                                float rx0, float ry0, float rx1, float ry1) {
   if (qthr < 0.f) return false;
@@ -424,21 +438,51 @@ GS_HD bool rect_may_contribute(float x, float y, float A, float B, float C, floa
   bool iny = (dy0 <= 0.f) && (dy1 >= 0.f);
   if (inx && iny) return true;
   // The 1-D minimiser along an edge only has to be approximately right: q evaluated at any point of the
-  // edge is >= the true minimum, an error delta in the minimiser costs C*delta^2 (~1e-12 relative), far inside
-  // the safety margin of cull_threshold().  So the fast (MUFU.RCP based) division is enough on the device.
+  // edge is >= the true minimum, an error delta in the minimiser costs C*delta^2 (second order in u, see kCullGamma).
+  // So the fast (MUFU.RCP based) division is enough on the device.  Each edge's q is lowered by its rounding margin.
   float qmin = 3.0e38f;
   if (!inx) {
     float ex = dx0 > 0.f ? dx0 : dx1;
     float dy = fminf(dy1, fmaxf(dy0, gs_fdiv(-B * ex, C)));
-    qmin = A * ex * ex + 2.f * B * ex * dy + C * dy * dy;
+    const float a = A * ex * ex, b = 2.f * B * ex * dy, c = C * dy * dy;
+    qmin = (a + b + c) - kCullGamma * (fabsf(a) + fabsf(b) + fabsf(c));
   }
   if (!iny) {
     float ey = dy0 > 0.f ? dy0 : dy1;
     float dx = fminf(dx1, fmaxf(dx0, gs_fdiv(-B * ey, A)));
-    float q = A * dx * dx + 2.f * B * dx * ey + C * ey * ey;
-    qmin = fminf(qmin, q);
+    const float a = A * dx * dx, b = 2.f * B * dx * ey, c = C * ey * ey;
+    qmin = fminf(qmin, (a + b + c) - kCullGamma * (fabsf(a) + fabsf(b) + fabsf(c)));
   }
   return !(qmin > qthr);       // NaN -> keep
+}
+
+// Threshold for the cull's ellipse q <= qthr in closed form (the row form below, k_preprocess's rect tightening), whose
+// extents come from det = A C - B^2.  det cancels like q: |fl(det) - det| <= 3u A C.  On the ellipse's bounding box
+// (|dx| <= hx, |dy| <= hy, A hx^2 = C hy^2 = qthr A C / det) s <= 2N <= 4 qthr A C / det, so the equivalent widening is
+// qthr + 4 gamma qthr A C / det.  It is only trusted while det > gamma A C (then fl(det) is within 1 +- 3/32 of det and
+// the widening, >= 4 (3u A C / det) qthr, covers that error too); below, the callers take the per-tile test.
+GS_HD bool cull_ellipse_ok(float A, float C, float det) { return det > kCullGamma * A * C; }
+GS_HD float cull_ellipse_qthr(float A, float C, float qthr, float rdet) {
+  return qthr + 4.f * kCullGamma * qthr * A * C * rdet;
+}
+
+// k_preprocess's lossless tightening of the tile rect [rx0, rx1) x [ry0, ry1): the ellipse q <= qthr (widened as above)
+// has the bounding box half-extents sqrt(qthr C / det), sqrt(qthr A / det); +1 px, the tile range rounded outwards.
+// An empty intersection becomes the empty rect 0; a near-degenerate conic keeps the rect.
+GS_HD void tighten_cull_rect(float x, float y, float A, float B, float C, float qthr, int& rx0, int& ry0, int& rx1,
+                             int& ry1) {
+  const float det = A * C - B * B;
+  if (!cull_ellipse_ok(A, C, det)) return;
+  const float rdet = 1.0f / det, qw = cull_ellipse_qthr(A, C, qthr, rdet);
+  const float hx = sqrtf(qw * C * rdet) + 1.0f, hy = sqrtf(qw * A * rdet) + 1.0f;
+  const float big = 1.0e8f;
+  const int tx0 = (int)floorf(fmaxf(-big, fminf(big, (x - hx) * (1.0f / kBlock))));
+  const int tx1 = (int)floorf(fmaxf(-big, fminf(big, (x + hx) * (1.0f / kBlock)))) + 1;
+  const int ty0 = (int)floorf(fmaxf(-big, fminf(big, (y - hy) * (1.0f / kBlock))));
+  const int ty1 = (int)floorf(fmaxf(-big, fminf(big, (y + hy) * (1.0f / kBlock)))) + 1;
+  rx0 = rx0 > tx0 ? rx0 : tx0; rx1 = rx1 < tx1 ? rx1 : tx1;
+  ry0 = ry0 > ty0 ? ry0 : ty0; ry1 = ry1 < ty1 ? ry1 : ty1;
+  if (rx1 <= rx0 || ry1 <= ry0) { rx0 = rx1 = ry0 = ry1 = 0; }
 }
 
 // The same predicate for a whole tile ROW at once.  The kept tiles of a row are those whose pixel-centre span
@@ -455,13 +499,14 @@ GS_HD RowCull row_cull_setup(float x, float y, float A, float B, float C, float 
   RowCull r;
   r.x = x; r.y = y; r.B = B;
   r.det = A * C - B * B;
-  r.ok = (r.det > 0.f) && (A > 0.f) && (C > 0.f) && (qthr >= 0.f);
+  r.ok = cull_ellipse_ok(A, C, r.det) && (A > 0.f) && (C > 0.f) && (qthr >= 0.f);
   const float rdet = 1.0f / r.det;
-  r.hx = sqrtf(qthr * C * rdet);
-  r.hy = sqrtf(qthr * A * rdet) + kRowEps;
+  const float qw = cull_ellipse_qthr(A, C, qthr, rdet);  // widened by the rounding margin (kCullGamma)
+  r.hx = sqrtf(qw * C * rdet);
+  r.hy = sqrtf(qw * A * rdet) + kRowEps;
   r.dyR = -B * r.hx / C;                                  // dy of the rightmost point (the leftmost one is at -dyR)
   r.invA = 1.0f / A;
-  r.aq = A * qthr;
+  r.aq = A * qw;
   return r;
 }
 // tiles [ta, tb] of row ty (clipped to [rx0, rx1)) are kept; returns false when the row keeps nothing

@@ -418,20 +418,7 @@ k_preprocess(InPtrs in, GeomView gv, int* __restrict__ radii) {
     // reference's square 3-sigma rect (which stays what `radii` reports).  Tiles outside it would fail the per-tile test
     // anyway; not walking them keeps the count/emit loops proportional to what is kept, also for Gaussians that grow
     // large during training.  (+1 px margin; the tile range is rounded outwards.)
-    if (cull && qthr >= 0.f) {
-      const float det = sr_.A * sr_.C - sr_.B * sr_.B;
-      if (det > 0.f) {
-        const float hx = sqrtf(sr_.qthr * sr_.C / det) + 1.0f, hy = sqrtf(sr_.qthr * sr_.A / det) + 1.0f;
-        const float big = 1.0e8f;
-        const int tx0 = (int)floorf(fmaxf(-big, fminf(big, (p.x - hx) * (1.0f / kBlock))));
-        const int tx1 = (int)floorf(fmaxf(-big, fminf(big, (p.x + hx) * (1.0f / kBlock)))) + 1;
-        const int ty0 = (int)floorf(fmaxf(-big, fminf(big, (p.y - hy) * (1.0f / kBlock))));
-        const int ty1 = (int)floorf(fmaxf(-big, fminf(big, (p.y + hy) * (1.0f / kBlock)))) + 1;
-        p.rx0 = max(p.rx0, tx0); p.rx1 = min(p.rx1, tx1);
-        p.ry0 = max(p.ry0, ty0); p.ry1 = min(p.ry1, ty1);
-        if (p.rx1 <= p.rx0 || p.ry1 <= p.ry0) { p.rx0 = p.rx1 = p.ry0 = p.ry1 = 0; }
-      }
-    }
+    if (cull && qthr >= 0.f) tighten_cull_rect(sr_.x, sr_.y, sr_.A, sr_.B, sr_.C, sr_.qthr, p.rx0, p.ry0, p.rx1, p.ry1);
     sr_.rx0 = p.rx0; sr_.rx1 = p.rx1; sr_.ry0 = p.ry0; sr_.ry1 = p.ry1;
     const int area = (p.rx1 - p.rx0) * (p.ry1 - p.ry0);
     if (cull && qthr < 0.f) ntiles = 0;

@@ -120,4 +120,37 @@ int host_row_keep(float x, float y, float A, float B, float C, float opacity, in
   }
   return 1;
 }
+
+// The culls as the kernels call them, on a conic and threshold already in the log2 domain (k_preprocess's SplatRect,
+// the blend's slab entry).  cull_threshold alone:
+float host_cull_threshold(float opacity) { return cull_threshold(opacity); }
+
+// rect_may_contribute over n pixel-centre rectangles rects[4 k .. 4 k + 3] = x0, y0, x1, y1 -> keep[k]
+void host_rect_keep_many(float x, float y, float A, float B, float C, float qthr, int n, const float* rects,
+                         int* keep) {
+  for (int k = 0; k < n; ++k) {
+    const float* r = rects + 4 * k;
+    keep[k] = rect_may_contribute(x, y, A, B, C, qthr, r[0], r[1], r[2], r[3]) ? 1 : 0;
+  }
+}
+
+// tighten_cull_rect on the tile rect rect[4] = rx0, ry0, rx1, ry1 (in place)
+void host_tighten_cull_rect(float x, float y, float A, float B, float C, float qthr, int* rect) {
+  tighten_cull_rect(x, y, A, B, C, qthr, rect[0], rect[1], rect[2], rect[3]);
+}
+
+// row_keep_range for tile rows ry0 .. ry1 - 1 of the tile rect [rx0, rx1): row ry0 + k keeps tiles ta[k] .. tb[k]
+// (ta > tb: none).  Returns 0 when row_cull_setup falls back to the per-tile test (nothing is written then).
+int host_row_ranges(float x, float y, float A, float B, float C, float qthr, int H, int rx0, int ry0, int rx1, int ry1,
+                    int* ta, int* tb) {
+  const RowCull rc = row_cull_setup(x, y, A, B, C, qthr);
+  if (!rc.ok) return 0;
+  for (int ty = ry0; ty < ry1; ++ty) {
+    int a, b;
+    if (!row_keep_range(rc, ty, H, rx0, rx1, a, b)) { a = 1; b = 0; }
+    ta[ty - ry0] = a;
+    tb[ty - ry0] = b;
+  }
+  return 1;
+}
 }
