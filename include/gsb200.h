@@ -387,6 +387,52 @@ GSB_API int gsb_ply_pack(int64_t P, int32_t n_segments, const GsbPlySegment* seg
 GSB_API int gsb_ply_unpack(int64_t P, const void* in, int32_t n_segments, const GsbPlySegment* segments,
                            gsb_stream_t stream);
 
+/* ---- Baseline JPEG decoding (PIL.Image.open(path) on libjpeg-turbo; DESIGN.md 4.24) ----
+ * One call decodes n files of any sizes, each a single interleaved Huffman scan of 8-bit YCbCr with chroma 1x1 and
+ * luma sampling 1x1, 2x1, 1x2 or 2x2, into out[out_offset .. + height * width * 3) as RGB bytes: jdhuff.c's decode,
+ * the DC prediction in int32 per component reset at each restart, jidctint.c's islow IDCT, jdsample.c's fancy
+ * upsampling and jdcolor.c's fixed-point conversion, so the bytes are Pillow's.  The host parses the marker segments
+ * (quantisation and derived Huffman tables, DRI); data holds each file's entropy-coded segment exactly as stored
+ * (stuffed bytes and RSTn included), file after file: files[i].data_offset is the sum of the earlier data_bytes.
+ * Without restart markers the scan is split into subseq_bits-bit subsequences decoded in parallel and synchronised
+ * (Weissenberger & Schmidt, ICPP 2018); the call blocks until the decode is done, the synchronisation's rounds
+ * reading a counter each.  status[i] (device int32) is 0 for a file decoded exactly, else GSB_JPEG_* bits naming the
+ * stream libjpeg would warn about or handle in ways not reproduced here; such a file's pixels are undefined and the
+ * caller decodes it another way.  n <= 65535; subseq_bits a multiple of 8 in 32..2^20; width, height in 1..65535;
+ * each entropy segment below 2^28 bytes; scratch 256-byte aligned, at least gsb_jpeg_scratch_bytes; else
+ * GSB_ERR_INVALID. */
+#define GSB_JPEG_LOOKAHEAD 9
+typedef struct GsbJpegHuff {
+  uint16_t look[1 << GSB_JPEG_LOOKAHEAD]; /* codes of <= 9 bits, indexed by the next 9 bits: (length << 8) | symbol,
+                                             0 for a longer code */
+  int32_t maxcode[18];   /* jpeg_make_d_derived_tbl's: the largest code of each length, -1 when there is none */
+  int32_t valoffset[18]; /* huffval index = code + valoffset[length] */
+  uint8_t huffval[256];
+} GsbJpegHuff;
+typedef struct GsbJpegFile {
+  int32_t width, height;
+  int32_t h, v;             /* luma sampling factors, 1 or 2; both chroma components 1x1 */
+  int32_t restart_interval; /* MCUs per restart interval, 0 for none */
+  int32_t reserved;
+  int64_t data_offset;      /* the entropy-coded segment in data */
+  int64_t data_bytes;
+  int64_t out_offset;       /* the [height, width, 3] image in out */
+  uint16_t quant[3][64];    /* per component (Y, Cb, Cr), natural order */
+  GsbJpegHuff dc[3], ac[3]; /* per component */
+} GsbJpegFile;
+#define GSB_JPEG_BAD_CODE 1       /* a code with no table entry */
+#define GSB_JPEG_PAST_END 2       /* bits needed past the end of an entropy segment or restart interval */
+#define GSB_JPEG_RUN_PAST_63 4    /* a run past coefficient 63 */
+#define GSB_JPEG_RESTART 8        /* RSTn missing, extra or out of sequence */
+#define GSB_JPEG_MCUS_LEFT 16     /* a segment or interval ended with MCUs left to decode */
+#define GSB_JPEG_TRAILING 32      /* a whole byte or more left after an interval's last MCU */
+#define GSB_JPEG_COEF_RANGE 64    /* a dequantised coefficient outside int16, or a DC sum outside int32 */
+#define GSB_JPEG_UNSYNCED 128     /* the subsequences did not synchronise */
+GSB_API size_t gsb_jpeg_scratch_bytes(int32_t n, const GsbJpegFile* files, int32_t subseq_bits);
+GSB_API int gsb_jpeg_decode_batch(int32_t n, const GsbJpegFile* files, const uint8_t* data, int32_t subseq_bits,
+                                  void* scratch, size_t scratch_bytes, uint8_t* out, int32_t* status,
+                                  gsb_stream_t stream);
+
 /* ---- LPIPS, VGG16 v0.1(metrics.py:69 lpips(render, gt, net_type='vgg'); lpipsPyTorch/modules/lpips.py,
  * networks.py BaseNet / VGG16, utils.py normalize_activation).  DESIGN.md 4.15.  fp32 FFMA, NHWC activations, every
  * sum in one fixed order: an image's values are bit-identical from run to run and whatever else is in the batch.

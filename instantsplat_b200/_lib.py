@@ -67,6 +67,19 @@ class GsbPlySegment(ctypes.Structure):
 
 
 PLY_MAX_SEGMENTS = 8
+JPEG_LOOKAHEAD = 9
+
+
+class GsbJpegHuff(ctypes.Structure):
+    _fields_ = [("look", ctypes.c_uint16 * (1 << JPEG_LOOKAHEAD)), ("maxcode", ctypes.c_int32 * 18),
+                ("valoffset", ctypes.c_int32 * 18), ("huffval", ctypes.c_uint8 * 256)]
+
+
+class GsbJpegFile(ctypes.Structure):
+    _fields_ = [("width", ctypes.c_int32), ("height", ctypes.c_int32), ("h", ctypes.c_int32), ("v", ctypes.c_int32),
+                ("restart_interval", ctypes.c_int32), ("reserved", ctypes.c_int32),
+                ("data_offset", ctypes.c_int64), ("data_bytes", ctypes.c_int64), ("out_offset", ctypes.c_int64),
+                ("quant", (ctypes.c_uint16 * 64) * 3), ("dc", GsbJpegHuff * 3), ("ac", GsbJpegHuff * 3)]
 
 
 class GsbShardPiece(ctypes.Structure):
@@ -91,7 +104,7 @@ EXPORTS = ("gsb_geom_bytes", "gsb_binning_bytes", "gsb_image_bytes", "gsb_prepro
            "gsb_frames_u8_batch", "gsb_lpips_scratch_bytes", "gsb_lpips_prepare", "gsb_lpips_conv3x3_relu",
            "gsb_lpips_maxpool2", "gsb_lpips_head", "gsb_render_batch_bg", "gsb_backward_batch_stats_bg",
            "gsb_png_bound", "gsb_png_scratch_bytes", "gsb_png_encode_batch", "gsb_resample_u8_batch",
-           "gsb_ply_pack", "gsb_ply_unpack")
+           "gsb_ply_pack", "gsb_ply_unpack", "gsb_jpeg_scratch_bytes", "gsb_jpeg_decode_batch")
 KERNEL_IDS = ("preprocess", "sort_depth", "scan", "duplicate", "sort_tile", "gather", "blend_fwd", "blend_bwd",
               "preprocess_bwd", "loss_fwd", "loss_bwd", "adam")
 
@@ -196,12 +209,15 @@ def lib() -> ctypes.CDLL:
     L.gsb_resample_u8_batch.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, i32, vp, vp, i32, vp, sz, vp]
     L.gsb_ply_pack.argtypes = [i64, i32, ctypes.POINTER(GsbPlySegment), vp, vp]
     L.gsb_ply_unpack.argtypes = [i64, vp, i32, ctypes.POINTER(GsbPlySegment), vp]
+    L.gsb_jpeg_scratch_bytes.restype = sz
+    L.gsb_jpeg_scratch_bytes.argtypes = [i32, ctypes.POINTER(GsbJpegFile), i32]
+    L.gsb_jpeg_decode_batch.argtypes = [i32, ctypes.POINTER(GsbJpegFile), vp, i32, vp, sz, vp, vp, vp]
     for f in ("gsb_preprocess_batch", "gsb_render_batch", "gsb_backward_pose_batch", "gsb_l1_mask_fwd_bwd_batch",
               "gsb_track_step_batch", "gsb_backward_batch", "gsb_loss_forward_batch", "gsb_loss_backward_batch",
               "gsb_backward_batch_stats", "gsb_image_metrics_batch", "gsb_frames_u8_batch", "gsb_lpips_prepare",
               "gsb_lpips_conv3x3_relu", "gsb_lpips_maxpool2", "gsb_lpips_head", "gsb_render_batch_bg",
               "gsb_backward_batch_stats_bg", "gsb_png_encode_batch", "gsb_resample_u8_batch", "gsb_ply_pack",
-              "gsb_ply_unpack"):
+              "gsb_ply_unpack", "gsb_jpeg_decode_batch"):
         getattr(L, f).restype = ctypes.c_int
     L.gsb_adam_step_gated.argtypes = [i32, ctypes.POINTER(GsbAdamTensor), vp, vp, vp]
     L.gsb_adam_step_gated.restype = ctypes.c_int

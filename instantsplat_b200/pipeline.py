@@ -3,9 +3,10 @@ on one GPU (DESIGN.md section 4.18).
 
     python -m instantsplat_b200.pipeline eval  --data_root ROOT --output_dir OUT --datasets D.. --scenes S..
         --n_views N.. --iterations IT.. [--lpips_weights DIR] [--workers W] [--png_encoder pil|gpu] [--test_fps]
-        [--kernel_size K] [--ply_io numpy|gpu]
+        [--kernel_size K] [--ply_io numpy|gpu] [--jpeg_decoder pil|gpu]
     python -m instantsplat_b200.pipeline infer --data_root ROOT --output_dir OUT --datasets D.. --scenes S..
         --n_views N.. --iterations IT.. [--workers W] [--png_encoder pil|gpu] [--kernel_size K] [--ply_io numpy|gpu]
+        [--jpeg_decoder pil|gpu]
 
 Tasks run in the scripts' loop order (dataset, scene, n_views, iterations), one after another.  The source is
 ROOT/D/S/24_views for eval and ROOT/D/S for infer; the model is OUT/D/S/<N>_views.  Each stage is the stage module's
@@ -30,6 +31,10 @@ infinite is refused with the other refusals.
 --ply_io gpu goes on the train stage's line only: its save points write point_cloud.ply on the GPU (ply.py).  The
 render stages get the model in memory and read no ply.
 
+--jpeg_decoder gpu goes on the train line and the test-view renders' line, the two stages that decode source images:
+the refusal pass, the train stage and the test views loaded for stage 4 decode their JPEG files on the GPU (jpeg.py),
+Pillow's pixels byte for byte.
+
 Every PNG goes to one process-wide encoder pool (PngWriter) that the GPU stages do not wait for, up to a bound on the
 frames queued; with --png_encoder gpu the frames are encoded on the GPU and the pool only writes the files.  Every
 task is checked before anything is written (refusals).  The scripts' nvidia-smi GPU picker and init_geo (stage 1) are
@@ -50,7 +55,7 @@ from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from . import freeview, metrics, mip, ply, png, render_views, train
+from . import freeview, jpeg, metrics, mip, ply, png, render_views, train
 from .scene_io import load_views, pose_matrices
 
 # stage -> (log file, the script's start line, its completion line)
@@ -94,16 +99,17 @@ def tasks(mode: str, data_root: str, output_dir: str, datasets: Sequence[str], s
 
 
 def stage_argv(t: Task, lpips_weights: Optional[str] = None, test_fps: bool = False,
-               kernel_size: Optional[float] = None, ply_io: Optional[str] = None) -> Dict[str, List[str]]:
+               kernel_size: Optional[float] = None, ply_io: Optional[str] = None,
+               jpeg_decoder: Optional[str] = None) -> Dict[str, List[str]]:
     """Each stage's command line as the script writes it; test_fps adds --test_fps to the test-view renders';
     kernel_size adds --kernel_size to the train, render and fly-through lines (not to metrics, which scores PNGs);
-    ply_io adds --ply_io to the train line."""
+    ply_io adds --ply_io to the train line; jpeg_decoder adds --jpeg_decoder to the train and test-view render lines."""
     base = ["-s", t.source, "-m", t.model, "-r", "1", "--n_views", str(t.n_views), "--iterations", str(t.iterations)]
     k = mip.argv(kernel_size)
-    out = {"train": base + ["--pp_optimizer", "--optim_pose"] + k + ply.argv(ply_io)}
+    out = {"train": base + ["--pp_optimizer", "--optim_pose"] + k + ply.argv(ply_io) + jpeg.argv(jpeg_decoder)}
     if t.mode == "eval":
         out["render_train"] = base + k
-        out["render_test"] = base + ["--eval"] + (["--test_fps"] if test_fps else []) + k
+        out["render_test"] = base + ["--eval"] + (["--test_fps"] if test_fps else []) + k + jpeg.argv(jpeg_decoder)
         out["metrics"] = ["-s", t.source, "-m", t.model, "--n_views", str(t.n_views)] \
             + ([] if lpips_weights is None else ["--lpips_weights", lpips_weights])
     else:
@@ -112,18 +118,21 @@ def stage_argv(t: Task, lpips_weights: Optional[str] = None, test_fps: bool = Fa
 
 
 def stage_args(t: Task, lpips_weights: Optional[str] = None, test_fps: bool = False,
-               kernel_size: Optional[float] = None, ply_io: Optional[str] = None) -> Dict[str, argparse.Namespace]:
+               kernel_size: Optional[float] = None, ply_io: Optional[str] = None,
+               jpeg_decoder: Optional[str] = None) -> Dict[str, argparse.Namespace]:
     """stage_argv parsed by each stage's own parser."""
     parse = {"train": train.parse_args, "metrics": lambda a: metrics.parser().parse_args(a)}
     return {k: parse.get(k, lambda a: render_views.parser().parse_args(a))(v)
-            for k, v in stage_argv(t, lpips_weights, test_fps, kernel_size, ply_io).items()}
+            for k, v in stage_argv(t, lpips_weights, test_fps, kernel_size, ply_io, jpeg_decoder).items()}
 
 
-def refusals(t: Task, test_fps: bool = False, kernel_size: Optional[float] = None) -> List[str]:
+def refusals(t: Task, test_fps: bool = False, kernel_size: Optional[float] = None,
+             jpeg_decoder: Optional[str] = None) -> List[str]:
     """Why the task cannot run, each reason with its path; empty when it can.  Reads the source, writes nothing.
     test_fps: the eval task's test-view renders carry --test_fps, which needs a test view; kernel_size: the stages
     carry --kernel_size, which must be a finite number >= 0.  The model the render stages read is the train stage's,
-    in memory, and carries filter_3D whenever the train stage has the flag."""
+    in memory, and carries filter_3D whenever the train stage has the flag.  jpeg_decoder "gpu": the training views
+    are decoded on the GPU, as the train stage will decode them."""
     out = []
     why = mip.kernel_refusal(kernel_size)
     if why:
@@ -141,10 +150,11 @@ def refusals(t: Task, test_fps: bool = False, kernel_size: Optional[float] = Non
         out.append(why)
     if out:
         return out
-    a = stage_args(t, kernel_size=kernel_size)["train"]
+    a = stage_args(t, kernel_size=kernel_size, jpeg_decoder=jpeg_decoder)["train"]
     out += train.refusals(a)
     try:
-        train.load_host_scene(a.source_path, a.n_views, a.resolution, a.images, a.init_scale_from_view_depth)
+        train.load_host_scene(a.source_path, a.n_views, a.resolution, a.images, a.init_scale_from_view_depth,
+                              decode_device="cuda" if jpeg.requested(a) else None)
         if t.mode == "infer":
             freeview.intrinsics(t.source, t.n_views)
     except (ValueError, FileNotFoundError) as e:
@@ -240,12 +250,12 @@ def _stage(t: Task, key: str, times: Dict[str, float]):
 
 def run_task(t: Task, pool: PngWriter, lpips_net=None, lpips_weights: Optional[str] = None,
              device="cuda", test_fps: bool = False, kernel_size: Optional[float] = None,
-             ply_io: Optional[str] = None) -> Tuple[int, Dict[str, float]]:
+             ply_io: Optional[str] = None, jpeg_decoder: Optional[str] = None) -> Tuple[int, Dict[str, float]]:
     """The script's run_on_gpu from stage 2 on, with test_fps: stage 4 with --test_fps; kernel_size: every stage but
     metrics with --kernel_size (the trainer's filter_3D handed to the trackers); ply_io: the train stage with
-    --ply_io.  Returns (model directories metrics could not evaluate, wall seconds per stage).  The trainer and
-    trackers are released before it returns."""
-    a = stage_args(t, lpips_weights, test_fps, kernel_size, ply_io)
+    --ply_io; jpeg_decoder: the train stage and the test views with --jpeg_decoder.  Returns (model directories
+    metrics could not evaluate, wall seconds per stage).  The trainer and trackers are released before it returns."""
+    a = stage_args(t, lpips_weights, test_fps, kernel_size, ply_io, jpeg_decoder)
     times, failed = {}, 0
     print("=" * 55)
     print(f"Starting process: {t.label}")
@@ -284,7 +294,8 @@ def run_task(t: Task, pool: PngWriter, lpips_net=None, lpips_weights: Optional[s
             return pool.write([(0, held[folder])], folder, workers, names)
 
         with _stage(t, "render_test", times):
-            views = load_views(t.source, t.n_views, 1, r.resolution)
+            views = load_views(t.source, t.n_views, 1, r.resolution,
+                               decode_device=device if jpeg.requested(r) else None)
             out = os.path.join(t.model, "test", f"ours_{it}")
             tk = tracker(views, r)
             start = time.time()
@@ -314,16 +325,17 @@ def run_task(t: Task, pool: PngWriter, lpips_net=None, lpips_weights: Optional[s
 
 def run_tasks(ts: Sequence[Task], workers: Optional[int] = None, lpips_net=None, lpips_weights: Optional[str] = None,
               device="cuda", png_encoder: str = "pil", test_fps: bool = False,
-              kernel_size: Optional[float] = None, ply_io: Optional[str] = None) -> Tuple[int, List[Dict[str, float]]]:
+              kernel_size: Optional[float] = None, ply_io: Optional[str] = None,
+              jpeg_decoder: Optional[str] = None) -> Tuple[int, List[Dict[str, float]]]:
     """Every task in order on one encoder pool (PngWriter with png_encoder), then every write waited for; test_fps,
-    kernel_size and ply_io: run_task's.  Returns (model directories metrics could not evaluate, per-task stage times).  Raises WriteError
-    when a PNG could not be written."""
+    kernel_size, ply_io and jpeg_decoder: run_task's.  Returns (model directories metrics could not evaluate,
+    per-task stage times).  Raises WriteError when a PNG could not be written."""
     pool = PngWriter(workers, png_encoder)
     failed, times = 0, []
     try:
         for k, t in enumerate(ts, 1):
             print(f"Processing task {k} / {len(ts)}", flush=True)
-            f, s = run_task(t, pool, lpips_net, lpips_weights, device, test_fps, kernel_size, ply_io)
+            f, s = run_task(t, pool, lpips_net, lpips_weights, device, test_fps, kernel_size, ply_io, jpeg_decoder)
             failed += f
             times.append(s)
     finally:
@@ -355,6 +367,7 @@ def parser() -> argparse.ArgumentParser:
         freeview.add_png_encoder_arg(p)
         mip.add_arg(p)
         ply.add_arg(p)
+        jpeg.add_arg(p)
     return ap
 
 
@@ -366,7 +379,8 @@ def main(argv=None) -> int:
     weights, test_fps = getattr(a, "lpips_weights", None), getattr(a, "test_fps", False)
     k = mip.kernel_size(a)
     ts = tasks(a.mode, a.data_root, a.output_dir, a.datasets, a.scenes, a.n_views, a.iterations)
-    bad = [f"{t.label}: {r}" for t in ts for r in refusals(t, test_fps, k)]
+    dec = jpeg.decoder(a)
+    bad = [f"{t.label}: {r}" for t in ts for r in refusals(t, test_fps, k, dec)]
     if bad:
         raise SystemExit("\n".join(f"instantsplat_b200.pipeline: {b}" for b in bad))
     net = None
@@ -378,7 +392,7 @@ def main(argv=None) -> int:
             ap.error(str(e))
     try:
         failed, _ = run_tasks(ts, a.workers, net, weights, png_encoder=a.png_encoder, test_fps=test_fps,
-                              kernel_size=k, ply_io=ply.io(a))
+                              kernel_size=k, ply_io=ply.io(a), jpeg_decoder=dec)
     except WriteError as e:
         raise SystemExit(f"instantsplat_b200.pipeline: {e}")
     print("=" * 55)

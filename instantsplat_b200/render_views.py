@@ -40,10 +40,13 @@ with sentinel=False, so its defaults (white_background False included) always ov
 
     python -m instantsplat_b200.render_views -s SOURCE -m MODEL --n_views N --iterations IT [--eval] [--infer_video]
         [--optim_test_pose_iter 500] [--white_background] [--max_batch B] [--workers K] [--png_encoder pil|gpu]
-        [--test_fps] [-r R --resample_images] [--kernel_size K] [--ply_io numpy|gpu]
+        [--test_fps] [-r R --resample_images] [--kernel_size K] [--ply_io numpy|gpu] [--jpeg_decoder pil|gpu]
 
 --ply_io gpu reads point_cloud.ply on the GPU (ply.py), for the stage here or the fly-through it hands over to; the
 renders are the same as without it.
+
+--jpeg_decoder gpu decodes the stage's JPEG source images (the training split, or --eval's test split) on the GPU in
+one call (jpeg.py), Pillow's pixels byte for byte, so the gt files and renders are the same as without it.
 """
 from __future__ import annotations
 
@@ -57,7 +60,7 @@ from typing import Optional, Sequence, Tuple
 import numpy as np
 import torch
 
-from . import freeview, mip, ply, resample
+from . import freeview, jpeg, mip, ply, resample
 from .scene_io import Views, load_views, read_colmap_text
 from .tracking import PoseTracker
 from .train import save_time
@@ -185,6 +188,7 @@ def parser() -> argparse.ArgumentParser:
     resample.add_arg(ap)
     mip.add_arg(ap)
     ply.add_arg(ap)
+    jpeg.add_arg(ap)
     return ap
 
 
@@ -208,11 +212,12 @@ def main(argv=None) -> int:
     if why:
         raise SystemExit(f"render_views: {why}")
     rdev = "cuda" if resample.requested(a) else None
+    ddev = "cuda" if jpeg.requested(a) else None
     if a.eval:
         why = fps_refusal(a.source_path, a.n_views) if a.test_fps else None
         if why:
             raise SystemExit(f"render_views: {why}")
-        views = load_views(a.source_path, a.n_views, 1, a.resolution, resample_device=rdev)
+        views = load_views(a.source_path, a.n_views, 1, a.resolution, resample_device=rdev, decode_device=ddev)
         tracker = tracker_for(a.model_path, it, views, a.white_background, kernel_size=k, **ply.kwargs(a))
         out = os.path.join(a.model_path, "test", f"ours_{it}")
         start = time.time()
@@ -223,7 +228,7 @@ def main(argv=None) -> int:
         npy = os.path.join(a.model_path, "pose", f"ours_{it}", "pose_optimized.npy")
         if not os.path.isfile(npy):
             raise FileNotFoundError(f"{npy} not found")
-        views = load_views(a.source_path, a.n_views, 0, a.resolution, resample_device=rdev)
+        views = load_views(a.source_path, a.n_views, 0, a.resolution, resample_device=rdev, decode_device=ddev)
         tracker = tracker_for(a.model_path, it, views, a.white_background, kernel_size=k, **ply.kwargs(a))
         out = os.path.join(a.model_path, "train", f"ours_{it}")
         render_train(tracker, views, np.load(npy), out, a.max_batch, a.workers, write)

@@ -227,7 +227,7 @@ def loaded_size(width: int, height: int, resolution: int) -> Tuple[int, int]:
 
 
 def load_views(source_path: str, n_views: int, split: int = 0, resolution: int = 1, images: str = "images",
-               resample_device=None) -> Views:
+               resample_device=None, decode_device=None) -> Views:
     """render.py's cameras: readColmapSceneInfo (scene/dataset_readers.py:315-369) reads source/sparse_<n_views>/<split>
     ({0: the training views, 1: the test views of --eval}), cameras.txt (PINHOLE or SIMPLE_PINHOLE) and images.txt,
     opens source/<images>/<basename of the name> (`images`: train.py's -i, the folder name) and sorts the views by
@@ -238,6 +238,11 @@ def load_views(source_path: str, n_views: int, split: int = 0, resolution: int =
     resample.resize_u8 call (Pillow's bicubic resize, byte for byte), and keeps the decoded size in
     Views.source_width / source_height.  Any other device is refused before a file is read.
 
+    decode_device: None decodes every file with Pillow; a CUDA device decodes the split's JPEG files there in one
+    jpeg.decode_u8 call (Pillow's pixels, byte for byte; files outside its subset and flagged streams are decoded by
+    Pillow), and a resize then runs on the decoded batch without a round trip through the host.  Other files always
+    go through Pillow.  Any other device is refused before a file is read.
+
     Refused, with the reason: an image that is not 8-bit RGB (RGBA included: Camera's alpha mask is not implemented,
     and Pillow's resize of RGBA premultiplies alpha), and views whose image size or field of view differ (one
     PoseTracker renders them all)."""
@@ -246,6 +251,9 @@ def load_views(source_path: str, n_views: int, split: int = 0, resolution: int =
     if resample_device is not None and _torch().device(resample_device).type != "cuda":
         raise ValueError(f"resample_device {resample_device!r}: images are resized on a CUDA device only (there is no "
                          "host resize)")
+    if decode_device is not None and _torch().device(decode_device).type != "cuda":
+        raise ValueError(f"decode_device {decode_device!r}: JPEG files are decoded on a CUDA device only (Pillow "
+                         "decodes them without one)")
     folder = os.path.join(source_path, f"sparse_{n_views}", str(split))
     for f in ("cameras.txt", "images.txt"):
         if not os.path.isfile(os.path.join(folder, f)):
@@ -268,7 +276,8 @@ def load_views(source_path: str, n_views: int, split: int = 0, resolution: int =
                 raise ValueError(f"{path}: -r {resolution} resizes {W}x{H} to {loaded_size(W, H, resolution)}; "
                                  "resampled images are not supported (use -r 1, or -r -1 up to 1600 pixels wide, "
                                  "or --resample_images)")
-            pixels = np.array(im)
+            # the GPU decodes the split's JPEG files together after this loop; a placeholder keeps the place
+            pixels = path if decode_device is not None and im.format == "JPEG" else np.array(im)
         fx = float(intr["params"][0])
         fy = fx if intr["model"] == "SIMPLE_PINHOLE" else float(intr["params"][1])
         w2c = np.eye(4)
@@ -281,13 +290,34 @@ def load_views(source_path: str, n_views: int, split: int = 0, resolution: int =
         raise ValueError(f"{folder}: the cameras' intrinsics differ ({len(keys)} distinct image sizes and fields of "
                          "view); the views are rendered with one camera")
     W, H, fovx, fovy = keys.pop()
-    pixels = np.stack([r[2] for r in recs])
     Wl, Hl = loaded_size(W, H, resolution)
+    if (Wl, Hl) != (W, H) and (Wl < 1 or Hl < 1):
+        raise ValueError(f"{folder}: -r {resolution} resizes {W}x{H} to {Wl}x{Hl}, an empty image")
+    on_gpu = [i for i, r in enumerate(recs) if isinstance(r[2], str)]
+    if on_gpu:
+        from . import jpeg
+        torch = _torch()
+        decoded = jpeg.decode_u8([recs[i][2] for i in on_gpu], decode_device)
+        if len(on_gpu) == len(recs):
+            pixels = jpeg.stack(decoded)
+        else:
+            dev = decoded[0].device
+            pixels = torch.empty((len(recs), H, W, 3), dtype=torch.uint8, device=dev)
+            for i, im in zip(on_gpu, decoded):
+                pixels[i] = im
+            for i, r in enumerate(recs):
+                if not isinstance(r[2], str):
+                    pixels[i] = torch.from_numpy(r[2]).to(dev)
+        if (Wl, Hl) == (W, H):
+            pixels = pixels.cpu().numpy()
+    else:
+        pixels = np.stack([r[2] for r in recs])
     if (Wl, Hl) != (W, H):
-        if Wl < 1 or Hl < 1:
-            raise ValueError(f"{folder}: -r {resolution} resizes {W}x{H} to {Wl}x{Hl}, an empty image")
         from . import resample
-        pixels = resample.resize_u8(_torch().from_numpy(pixels).to(resample_device), (Wl, Hl)).cpu().numpy()
+        torch = _torch()
+        src = pixels.to(resample_device) if isinstance(pixels, torch.Tensor) else \
+            torch.from_numpy(pixels).to(resample_device)
+        pixels = resample.resize_u8(src, (Wl, Hl)).cpu().numpy()
     return Views([r[0] for r in recs], np.stack([r[1] for r in recs]), pixels, Wl, Hl, fovx, fovy,
                  [r[4] for r in recs], W, H)
 

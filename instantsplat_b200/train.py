@@ -34,6 +34,10 @@ the filters.  A K that is negative, NaN or infinite is refused.  Without the fla
 
 --ply_io gpu (not one of train.py's flags, and not part of cfg_args; ply.py) writes point_cloud.ply at the save points
 with JointTrainer.save_ply(io="gpu"): the records packed from the flat buffers on the GPU, the same bytes as without it.
+
+--jpeg_decoder gpu (not one of train.py's flags, and not part of cfg_args; jpeg.py) decodes the training views' JPEG
+files on the GPU in one call, Pillow's pixels byte for byte; other files, and JPEG files outside the decoder's subset,
+go through Pillow as without it.
 """
 from __future__ import annotations
 
@@ -51,7 +55,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 import torch
 
-from . import freeview, mip, ply, resample
+from . import freeview, jpeg, mip, ply, resample
 from .scene_io import Views, load_views, read_points3d_ply
 
 # ---- train.py's command line: arguments/__init__.py:47-94 and train.py:299-312 --------------------------------------
@@ -101,6 +105,7 @@ def parser() -> argparse.ArgumentParser:
     resample.add_arg(ap)
     mip.add_arg(ap)
     ply.add_arg(ap)
+    jpeg.add_arg(ap)
     return ap
 
 
@@ -234,12 +239,12 @@ class HostScene:
 
 
 def load_host_scene(source_path: str, n_views: int, resolution: int, images: str = "images",
-                    init_scale_from_view_depth: bool = False, resample_device=None) -> HostScene:
+                    init_scale_from_view_depth: bool = False, resample_device=None, decode_device=None) -> HostScene:
     """Everything of load_training_scene that is computed on the CPU, except the image resize of a CUDA
-    resample_device (load_views').  Raises, before anything is written, on what train.py cannot train: load_views'
-    refusals, camera ids other than 1..n (save_pose looks up colmap ids 1..n and would fail at the first save point),
-    a missing points3D.ply or confidence_dsp.npy."""
-    views = load_views(source_path, n_views, 0, resolution, images, resample_device)
+    resample_device and the JPEG decode of a CUDA decode_device (load_views').  Raises, before anything is written,
+    on what train.py cannot train: load_views' refusals, camera ids other than 1..n (save_pose looks up colmap ids
+    1..n and would fail at the first save point), a missing points3D.ply or confidence_dsp.npy."""
+    views = load_views(source_path, n_views, 0, resolution, images, resample_device, decode_device)
     ids = list(views.camera_ids)
     if sorted(ids) != list(range(1, len(views) + 1)):
         raise ValueError(f"sparse_{n_views}/0: camera ids {ids}; train.py's save_pose needs every camera id 1..{len(views)} "
@@ -371,7 +376,8 @@ def run(args: argparse.Namespace, device="cuda", log=print) -> RunResult:
     t0 = time.perf_counter()
     try:
         host = load_host_scene(args.source_path, args.n_views, args.resolution, args.images,
-                               args.init_scale_from_view_depth, dev if resample.requested(args) else None)
+                               args.init_scale_from_view_depth, dev if resample.requested(args) else None,
+                               dev if jpeg.requested(args) else None)
     except (ValueError, FileNotFoundError) as e:
         raise Refused(str(e)) from e
     phases["load"] = time.perf_counter() - t0
